@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- frames/s of MaskFusion::processFrame on a synthetic 640x480 .klg replay.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A step is one processFrame call (one pass of the per-frame dense hot path) on one frame of a seeded synthetic replay.
 
@@ -18,6 +18,10 @@ N = 1  workload = BASELINE.json configs[1]: "-static" single-model path, 640x480
   ref_cuda (the reference's own CUDA kernels recompiled, one model-frame of tracking in its calling pattern), multi_object
   (configs[2]: 3 tracked objects + the Mask R-CNN backbone on the same GPU), eight_objects (configs[3] on one GPU), ate (ATE-RMSE of
   every model's exported trajectory against the oracle on the first frames of the 8-object replay), backbone.
+
+  --dump-outputs DIR : after the timed steps, the results a caller of processFrame reads back from the background model are written as
+                 DIR/<name>.npy (float32 / float64): pose (4x4), pose_log (one row per processed frame), surfel_count, and
+                 every 5th row of the surfel map (at most 1M rows) (12 floats per surfel).  Inputs are seeded: equal arguments give equal inputs.
 
 N > 1  (torchrun) workload = configs[3]: ONE 640x480 replay with 8 tracked objects, the object Models sharded over the N GPUs
        (strong scaling: the replay is the same for every N).  The three exchanges of a frame -- frame-packet broadcast, pose-row
@@ -52,7 +56,7 @@ def load_peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W part)"
 
 
 class ClockSampler:
@@ -160,7 +164,7 @@ def algorithmic_bytes(name, S, P):
 
 def ncu_traffic(kernel):
     """dram__bytes_read.sum + dram__bytes_write.sum of one launch of `kernel`, from the newest committed `ncu --set full`
-    summary under profiles/ (scripts/summarize_ncu.py); None when no capture of that kernel is committed"""
+    summary under profiles/ (scripts/summarize_ncu.py, git-ignored); None when no local capture of that kernel exists"""
     import glob
     import re
     files = sorted(glob.glob(os.path.join(ROOT, "profiles", f"*_prof_{kernel}.txt")))
@@ -176,7 +180,19 @@ def ncu_traffic(kernel):
     return int(tot), os.path.basename(files[-1])
 
 
-def static_leg(torch, mfb, stream, local, rank, world, K, Wm):
+def dump_outputs(out_dir, model):
+    """what a caller reads back from `model` after the last step (see --dump-outputs)"""
+    os.makedirs(out_dir, exist_ok=True)
+    surf = model.downloadMap()
+    n = surf.shape[0]
+    idx = np.arange(0, min(n, 5_000_000), 5)         # fixed rows: builds with different counts still share the sampled prefix
+    arrays = {"pose": model.getPose().astype(np.float32), "pose_log": model.poseLog().astype(np.float64),
+              "surfel_count": np.array([n], np.float64), "surfels_sample": np.ascontiguousarray(surf[idx], np.float32)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def static_leg(torch, mfb, stream, local, rank, world, K, Wm, dump_dir=None):
     """configs[1]: the main line at N = 1, the `replicas` leg at N > 1"""
     n_need = 1 + 3 * (Wm + K) + 2
     sc, frames = make_replay(n_need, seed=rank)
@@ -233,6 +249,8 @@ def static_leg(torch, mfb, stream, local, rank, world, K, Wm):
     stages = mf.stageTimes()
     mf.setProfiling(False)
     S_live = mf.getBackgroundModel().lastCount()
+    if dump_dir:
+        dump_outputs(dump_dir, mf.getBackgroundModel())
     ms_all = sorted(r[0] for r in dev_runs)
     ms_dev, launches = ms_all[1], dev_runs[0][1]           # median of three passes
     if world > 1:
@@ -396,7 +414,7 @@ def run_ours(args, rank, world):
     pre = None
     if world > 1 and rank == 0:
         # the loader rank renders the replay before CUDA / NCCL exist in this process (the renderer forks worker processes)
-        n_pre = min(34 + args.warmup + args.steps, 160)
+        n_pre = 34 + args.warmup + args.steps
         pre = multi_frames(8, n_pre)
     torch.cuda.set_device(local)
     if world > 1:
@@ -408,7 +426,7 @@ def run_ours(args, rank, world):
     torch.cuda.set_stream(stream)
     if world > 1:
         return run_sharded(args, rank, world, torch, mfb, stream, local, pre)
-    st = static_leg(torch, mfb, stream, local, rank, world, K, Wm)
+    st = static_leg(torch, mfb, stream, local, rank, world, K, Wm, dump_dir=args.dump_outputs)
     P = W * H
     fps = K / (st["ms_dev"] / 1e3)
     fps_e2e = K / (st["ms_e2e"] / 1e3)
@@ -416,9 +434,9 @@ def run_ours(args, rank, world):
         "metric": METRIC, "value": round(fps, 3), "unit": "frames/s", "n_gpus": 1, "steps": K, "warmup": Wm,
         "ms_per_step": round(st["ms_dev"] / K, 4), "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
-        "config": {"workload": "configs[1]: -static single model, 640x480 synthetic .klg replay, ICP+RGB+SO3 tracking + surfel fuse, 1 B200",
+        "config": {"workload": "configs[1]: -static single model, 640x480 synthetic .klg replay, ICP+RGB+SO3 tracking + surfel fuse, 1 H100",
                    "surfels_live": int(st["S_live"]), "surfel_capacity": CAPACITY, "tracking": "GUI defaults icpWeight=20 so3=1 pyramid=1",
-                   "l2": "surfel store (227 MB: three float4 planes x 4.73 M capacity, one copy) + per-frame maps exceed the 126 MB L2 between steps (no explicit flush)",
+                   "l2": "surfel store (227 MB: three float4 planes x 4.73 M capacity, one copy) + per-frame maps exceed the 50 MB L2 between steps (no explicit flush)",
                    "parallelism": "single", "numerics": "fp32 per element; Gauss-Newton sums in fp64 of exact products, rounded to the reference's float record"},
         "timed_region": {"passes_ms": [round(m, 3) for m in st["ms_passes"]], "value_from": "median of three device-resident passes",
                          "min_ms_per_step": round(st["ms_passes"][0] / K, 4), "max_ms_per_step": round(st["ms_passes"][-1] / K, 4)},
@@ -526,7 +544,7 @@ def run_ours(args, rank, world):
                                                   "note": "ResNet-101-FPN forward (1024x1024, synthetic weights) enqueued on a second stream every 5th frame (the reference's sidecar runs at ~5 Hz)"}
         except Exception as e:          # noqa: BLE001
             r["with_backbone_every_5th_frame"] = {"error": f"{type(e).__name__}: {e}"[:300]}
-        r["workload"] = "configs[2]: 3 tracked objects, 640x480, 1 B200, Mask R-CNN backbone on the same GPU; masks are inputs (-maskdir mode: the R-CNN heads are not built)"
+        r["workload"] = "configs[2]: 3 tracked objects, 640x480, 1 H100, Mask R-CNN backbone on the same GPU; masks are inputs (-maskdir mode: the R-CNN heads are not built)"
         return r
     leg("multi_object", three)
 
@@ -544,8 +562,7 @@ def run_sharded(args, rank, world, torch, mfb, stream, local, pre):
     from maskfusion_b200.sharding import ShardedMaskFusion
     K, Wm = args.steps, args.warmup
     warm_to = 34                                            # 8 objects spawned (one every 3 frames), 30 static frames over
-    n = min(warm_to + Wm + K, 160)
-    K = n - warm_to - Wm
+    n = warm_to + Wm + K
     frames = cls = None
     single = None
     if rank == 0:
@@ -689,7 +706,10 @@ def main():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last step's results as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.gpus > 1 or args.impl != "ours"):
+        ap.error("--dump-outputs applies to the single-GPU run of this library (--gpus 1 --impl ours)")
     rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
     if args.impl == "reference":
         # the CPU arm uses all host threads it can, also under torchrun (which exports OMP_NUM_THREADS=1 for its workers)

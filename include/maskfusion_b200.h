@@ -1,5 +1,5 @@
 /*
- * include/maskfusion_b200.h -- C ABI of the B200-native MaskFusion dense pipeline.
+ * include/maskfusion_b200.h -- C ABI of the H100-native MaskFusion dense pipeline.
  *
  * The reference has no FFI: its hot path sits behind C++ methods of libmaskfusion.so
  * that take Eigen / OpenCV / OpenGL types (SURVEY.md section 8(b)).  This header is
@@ -173,7 +173,7 @@ int mf_get_stage_times(mf_context* ctx, char* buf, int bufsize);   /* lines: "na
 int mf_debug_set_poses(mf_context* ctx, int i, const float pose16[16], const float last_pose16[16]);   /* sets Model::pose and Model::lastPose verbatim */
 int mf_icp_step(mf_context* ctx, int i, int level, const float Rcurr9[9], const float tcurr3[3], float out29[29]);  /* icpStep, reduce.cu:446-525 */
 
-/* ---- Mask R-CNN backbone: ResNet-101 + FPN as tcgen05/TMEM GEMMs (replaces the dense part of the Keras/TF sidecar,
+/* ---- Mask R-CNN backbone: ResNet-101 + FPN as wgmma GEMMs (replaces the dense part of the Keras/TF sidecar,
  *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded: no COCO weights offline) ---- */
 typedef struct mf_backbone mf_backbone;
 const char* mf_cnn_last_error(void);

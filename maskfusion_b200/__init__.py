@@ -1,4 +1,4 @@
-"""maskfusion_b200 -- B200-native (sm_100a) implementation of MaskFusion's per-frame dense
+"""maskfusion_b200 -- H100-native (sm_90a) implementation of MaskFusion's per-frame dense
 pipeline behind the reference's MaskFusion::processFrame / Model::{performTracking,fuse,...}
 interface.  The product is the CUDA library (csrc/ -> libmaskfusion_b200.so, C ABI in
 include/maskfusion_b200.h); this package is the thin host-side mirror used by tests/bench."""

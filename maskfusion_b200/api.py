@@ -585,7 +585,7 @@ def write_klg(path: str, timestamps, depth_mm: np.ndarray, rgb: np.ndarray):
 
 
 class Backbone:
-    """Mask R-CNN ResNet-101-FPN backbone on tcgen05 GEMMs (csrc/mf_cnn.cu).  Weights are synthetic (seeded)."""
+    """Mask R-CNN ResNet-101-FPN backbone on wgmma GEMMs (csrc/mf_cnn.cu).  Weights are synthetic (seeded)."""
 
     def __init__(self, input_size=1024, seed=1, stream: int | None = None):
         self.L = load_library()

@@ -1,4 +1,4 @@
-// mf_cnn.cu -- Mask R-CNN backbone (ResNet-101 + FPN) as tcgen05 / TMEM tensor-core GEMMs (sm_100a).
+// mf_cnn.cu -- Mask R-CNN backbone (ResNet-101 + FPN) as wgmma tensor-core GEMMs (sm_90a).
 //
 // Replaces the dense-contraction part of the reference's Keras/TensorFlow sidecar
 // (Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111 -> matterport mrcnn `resnet_graph` +
@@ -7,16 +7,16 @@
 // K = kh*kw*Cin, activations NHWC bf16, frozen BatchNorm + conv bias folded into the weights
 // and a per-channel bias, residual add and ReLU fused into the epilogue.
 //
-// GEMM kernel (one 128 x BN output tile per CTA, 192 threads):
-//   warp 0     TMA producer: cp.async.bulk.tensor.2d (SWIZZLE_128B) A/B k-blocks of 64 into a
-//              4-stage shared-memory ring, mbarrier expect_tx / complete_tx
-//   warp 1     TMEM allocator + single-thread tcgen05.mma.cta_group::1.kind::f16 issuer
-//              (M=128, N=BN, K=16 x4 per k-block, fp32 accumulators in TMEM), tcgen05.commit
-//              releases ring slots and finally signals the epilogue
-//   warps 2-5  epilogue: tcgen05.ld 32x32b.x32 (each warp its 32-lane TMEM quarter) ->
-//              + bias, + residual, ReLU -> bf16 -> 64-byte row segments to HBM
-// 1x1 stride-1 convolutions feed the activation tensor straight to TMA (no im2col); 3x3, 7x7
-// and strided 1x1 go through a bf16 im2col buffer (round 1; TMA im2col descriptors = next).
+// GEMM kernel (one 128 x BN output tile per CTA, three warpgroups = 384 threads):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor.2d/3d (SWIZZLE_128B) A/B
+//                   k-blocks of 64 into a 4-stage shared-memory ring, mbarrier expect_tx / complete_tx
+//   warpgroups 1-2  consumers: each owns 64 rows of the tile and issues wgmma.mma_async m64nBNk16
+//                   (bf16 in, fp32 accumulators in registers) straight from the swizzled ring slots;
+//                   a slot is released (mbarrier arrive) once the wgmma group that read it has retired.
+//                   Tile width BN = 128 when that still gives every SM a tile, else 64.
+//                   Epilogue from registers: + bias, + residual, ReLU -> bf16 pairs to HBM
+// 1x1 stride-1 convolutions feed the activation tensor straight to TMA (no im2col); 3x3 / stride 1
+// convolutions use a 3-D tensor map (implicit GEMM); 7x7 and strided 1x1 go through a bf16 im2col buffer.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 #include <cuda.h>
@@ -37,6 +37,7 @@ namespace mfb {
 MF_D uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 MF_D void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count)); }
 MF_D void mbar_expect_tx(uint64_t* bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory"); }
+MF_D void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
 MF_D void mbar_wait(uint64_t* bar, uint32_t parity)
 {
     asm volatile(
@@ -57,44 +58,46 @@ MF_D void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, 
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-MF_D void tcgen05_commit(uint64_t* bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-MF_D void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-MF_D void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-MF_D void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// shared-memory matrix descriptor: K-major operand, SWIZZLE_128B, rows of 128 B, 8-row groups 1024 B apart
+// shared-memory matrix descriptor (sm_90 wgmma): K-major operand, SWIZZLE_128B, rows of 128 B, 8-row groups 1024 B apart
 MF_D uint64_t make_smem_desc(uint32_t saddr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address, 16-byte units          bits [0,14)
     d |= (uint64_t)1 << 16;                            // leading byte offset (unused for SW128 K-major) = 1
     d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset: 8 rows x 128 B      bits [32,46)
-    d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                            // layout type: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                            // layout type: SWIZZLE_128B               bits [62,64)
     return d;
 }
-MF_D void tmem_ld32(uint32_t taddr, uint32_t* r)
+MF_D void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+MF_D void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+MF_D void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory; scale-d = 1 (the accumulators start at zero)
+#define WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define WG_D32(i) WG_D8(i), WG_D8(i + 8), WG_D8(i + 16), WG_D8(i + 24)
+MF_D void wgmma_m64n64(float* d, uint64_t adesc, uint64_t bdesc)
 {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                   "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                   "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : WG_D32(0) : "l"(adesc), "l"(bdesc) : "memory");
+}
+MF_D void wgmma_m64n128(float* d, uint64_t adesc, uint64_t bdesc)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : WG_D32(0), WG_D32(32) : "l"(adesc), "l"(bdesc) : "memory");
+}
+template <int BN>
+MF_D void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc)
+{
+    if constexpr (BN == 128) wgmma_m64n128(d, adesc, bdesc);
+    else wgmma_m64n64(d, adesc, bdesc);
 }
 
 // ------------------------------------------------------------------------------------------
 // GEMM: out[M x N] (bf16) = relu?( A[M x K] * B[N x K]^T + bias[N] + residual[M x N] )
 // ------------------------------------------------------------------------------------------
-constexpr int GEMM_BM = 128, GEMM_BK = 64, GEMM_STAGES = 3, GEMM_THREADS = 192;   // 3 stages (<= 99 KB): two CTAs per SM, one's epilogue overlaps the other's main loop
+constexpr int GEMM_BM = 128, GEMM_BK = 64, GEMM_STAGES = 4, GEMM_THREADS = 384;   // 4 stages x 32 KB (BN = 128): one CTA per SM
 
 // implicit-GEMM geometry of a 3x3 / stride 1 / pad 1 convolution: the A operand is the NHWC activation itself, seen through a 3-D
 // tensor map (C, W, H); an M tile is a Wbox x Hbox pixel block (Wbox*Hbox = 128) and each of the 9 taps is the same block shifted
@@ -102,43 +105,33 @@ constexpr int GEMM_BM = 128, GEMM_BK = 64, GEMM_STAGES = 3, GEMM_THREADS = 192; 
 struct ConvGeom { int mode; int Wimg, Himg, Wbox, Hbox, cblocks; };
 
 template <int BN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                                                                        const float* __restrict__ bias, const __nv_bfloat16* __restrict__ residual,
-                                                                        __nv_bfloat16* __restrict__ out, int M, int N, int K, int relu, ConvGeom geo)
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_wgmma(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                                                                      const float* __restrict__ bias, const __nv_bfloat16* __restrict__ residual,
+                                                                      __nv_bfloat16* __restrict__ out, int M, int N, int K, int relu, ConvGeom geo)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages x A tile 16 KB][stages x B tile BN*128 B][barriers][tmem ptr]
+    // carve: [stages x A tile 16 KB][stages x B tile BN*128 B][barriers]
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2, B_BYTES = BN * GEMM_BK * 2;
     uint8_t* sA = smem;
     uint8_t* sB = smem + GEMM_STAGES * A_BYTES;
     uint64_t* full = (uint64_t*)(sB + GEMM_STAGES * B_BYTES);
     uint64_t* empty = full + GEMM_STAGES;
-    uint64_t* tmem_full = empty + GEMM_STAGES;
-    uint32_t* tmem_ptr = (uint32_t*)(tmem_full + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
     const int tile_m = blockIdx.x, tile_n = blockIdx.y;
     const int num_k = K / GEMM_BK;
     int px0 = 0, py0 = 0;
     if (geo.mode) { const int tilesX = geo.Wimg / geo.Wbox; py0 = (tile_m / tilesX) * geo.Hbox; px0 = (tile_m % tilesX) * geo.Wbox; }
 
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < GEMM_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < GEMM_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], GEMM_THREADS - 128); }      // empty: one arrival per consumer thread
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (t == 0) {
             // ===== TMA producer =====
             for (int kb = 0; kb < num_k; ++kb) {
                 const int s = kb % GEMM_STAGES;
@@ -153,67 +146,45 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_tcgen05(const __g
                 tma_load_2d(&mapB, &full[s], sB + s * B_BYTES, kb * GEMM_BK, tile_n * BN);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            // instruction descriptor: D=f32 (bit 4), A=B=bf16 (bits 7, 10), K-major both, N>>3 at 17, M>>4 at 24
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(GEMM_BM >> 4) << 24);
-            for (int kb = 0; kb < num_k; ++kb) {
-                const int s = kb % GEMM_STAGES;
-                const uint32_t ph = (kb / GEMM_STAGES) & 1;
-                mbar_wait(&full[s], ph);
-                tcgen05_fence_after();
-                const uint64_t adesc = make_smem_desc(smem_u32(sA + s * A_BYTES));
-                const uint64_t bdesc = make_smem_desc(smem_u32(sB + s * B_BYTES));
-#pragma unroll
-                for (int k = 0; k < GEMM_BK / 16; ++k)          // UMMA_K = 16 bf16 = 32 bytes: advance the start address by 2 (16-byte units)
-                    umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-                tcgen05_commit(&empty[s]);                      // frees the ring slot when these MMAs retire
-            }
-            tcgen05_commit(tmem_full);                          // accumulator complete
-        }
-    } else {
-        // ===== epilogue: warps 2..5 own TMEM lane quarters (warp id % 4) =====
-        const int q = warp & 3;
-        mbar_wait(tmem_full, 0);
-        tcgen05_fence_after();
-        const int rt = q * 32 + lane;
-        const int row = geo.mode ? (py0 + rt / geo.Wbox) * geo.Wimg + px0 + rt % geo.Wbox : tile_m * GEMM_BM + rt;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-            const int col = tile_n * BN + c0;
-            if (row < M) {
-                __nv_bfloat16* optr = out + (size_t)row * N + col;
-                const __nv_bfloat16* rptr = residual ? residual + (size_t)row * N + col : nullptr;
-#pragma unroll
-                for (int v = 0; v < 4; ++v) {                  // 4 x 16 bytes = 32 bf16
-                    uint4 res4 = make_uint4(0, 0, 0, 0);
-                    if (rptr) res4 = *reinterpret_cast<const uint4*>(rptr + v * 8);
-                    const __nv_bfloat16* rb = reinterpret_cast<const __nv_bfloat16*>(&res4);
-                    uint4 o4;
-                    __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(&o4);
-#pragma unroll
-                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col + v * 8)), b1 = __ldg(reinterpret_cast<const float4*>(bias + col + v * 8 + 4));
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        float x = __uint_as_float(r[v * 8 + e]) + bb[e];
-                        if (rptr) x += __bfloat162float(rb[e]);
-                        if (relu) x = fmaxf(x, 0.f);
-                        ob[e] = __float2bfloat16(x);
-                    }
-                    *reinterpret_cast<uint4*>(optr + v * 8) = o4;
-                }
-            }
-        }
+        return;
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(BN) : "memory");
+    // ===== consumers: warpgroup c = wg - 1 owns tile rows [64 c, 64 c + 64) =====
+    const int c = wg - 1;
+    float d[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+    for (int kb = 0; kb < num_k; ++kb) {
+        const int s = kb % GEMM_STAGES;
+        mbar_wait(&full[s], (kb / GEMM_STAGES) & 1);
+        const uint64_t adesc = make_smem_desc(smem_u32(sA + s * A_BYTES + c * 64 * 128));
+        const uint64_t bdesc = make_smem_desc(smem_u32(sB + s * B_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k)           // K = 16 bf16 = 32 bytes per wgmma: advance the start address by 2 (16-byte units)
+            wgmma_tile<BN>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+        wgmma_commit();
+        wgmma_wait<1>();                                 // the group of k-block kb-1 has retired: its ring slot may be refilled
+        if (kb > 0) mbar_arrive(&empty[(kb - 1) % GEMM_STAGES]);
+    }
+    wgmma_wait<0>();
+    // ===== epilogue: accumulator fragment of m64nBN -- d[4j + 2h + e] is row 16 w + lane/4 + 8 h, column 8 j + 2 (lane%4) + e =====
+    const int w = t >> 5, lane = t & 31;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int rt = c * 64 + w * 16 + (lane >> 2) + 8 * h;
+        const int row = geo.mode ? (py0 + rt / geo.Wbox) * geo.Wimg + px0 + rt % geo.Wbox : tile_m * GEMM_BM + rt;
+        if (row >= M) continue;
+        __nv_bfloat16* optr = out + (size_t)row * N + tile_n * BN + 2 * (lane & 3);
+        const __nv_bfloat16* rptr = residual ? residual + (size_t)row * N + tile_n * BN + 2 * (lane & 3) : nullptr;
+        const float* bptr = bias + tile_n * BN + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bptr + 8 * j));
+            float x0 = d[4 * j + 2 * h] + b2.x, x1 = d[4 * j + 2 * h + 1] + b2.y;
+            if (rptr) { const __nv_bfloat162 r2 = *reinterpret_cast<const __nv_bfloat162*>(rptr + 8 * j); x0 += __low2float(r2); x1 += __high2float(r2); }
+            if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            *reinterpret_cast<__nv_bfloat162*>(optr + 8 * j) = __floats2bfloat162_rn(x0, x1);
+        }
     }
 }
 
@@ -381,7 +352,7 @@ static bool cached_map_nhwc(CUtensorMap* m, const void* ptr, int Cin, int Wimg, 
 }
 
 template <int BN>
-static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 256 + 1024; }
+static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 2 * GEMM_STAGES * 8 + 1024; }
 
 const char* cnn_last_error() { return g_cnn_err.c_str(); }
 
@@ -394,7 +365,7 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
     if (K % 64 || N % 64 || M <= 0) { g_cnn_err = "gemm: need K % 64 == 0 and N % 64 == 0"; return -2; }
     const int mtiles = (M + GEMM_BM - 1) / GEMM_BM;
     // fill the machine: with few M tiles prefer the narrow N tile (twice the CTAs)
-    const int BN = (N % 128 == 0 && mtiles * (N / 128) >= 148) ? 128 : 64;
+    const int BN = (N % 128 == 0 && mtiles * (N / 128) >= num_sms()) ? 128 : 64;
     CUtensorMap mA, mB;
     ConvGeom geo; memset(&geo, 0, sizeof geo);
     if (conv3x3) {
@@ -405,15 +376,15 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
     } else if (!cached_map(&mA, A, (uint64_t)M, (uint64_t)K, GEMM_BM)) return -3;
     if (!cached_map(&mB, B, (uint64_t)N, (uint64_t)K, (uint32_t)BN)) return -3;
     dim3 grid(mtiles, N / BN);
-    prof_mark(s, BN == 128 ? "k_gemm_bf16_tcgen05_n128" : "k_gemm_bf16_tcgen05_n64");
+    prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128" : "k_gemm_bf16_wgmma_n64");
     if (BN == 128) {
         static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_tcgen05<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<128>()); attr = true; }
-        k_gemm_bf16_tcgen05<128><<<grid, GEMM_THREADS, gemm_smem_bytes<128>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
+        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<128>()); attr = true; }
+        k_gemm_bf16_wgmma<128><<<grid, GEMM_THREADS, gemm_smem_bytes<128>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
     } else {
         static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_tcgen05<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<64>()); attr = true; }
-        k_gemm_bf16_tcgen05<64><<<grid, GEMM_THREADS, gemm_smem_bytes<64>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
+        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<64>()); attr = true; }
+        k_gemm_bf16_wgmma<64><<<grid, GEMM_THREADS, gemm_smem_bytes<64>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { g_cnn_err = std::string("gemm launch: ") + cudaGetErrorString(e); return -4; }
@@ -478,9 +449,9 @@ static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int W
     }
     if (!(L.k == 1 && L.stride == 1)) {
         if (L.k == 1 && L.stride == 2 && (L.Cin % 8) == 0) {
-            prof_mark(s, "k_subsample2"); k_subsample2<<<592, 256, 0, s>>>(in, Hin, Win, L.Cin, b->col);
+            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, b->col);
         } else {
-            prof_mark(s, "k_im2col"); k_im2col<<<1184, 256, 0, s>>>(in, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, b->col);
+            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, b->col);
         }
         A = b->col;
     }
@@ -601,7 +572,7 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     int H, W;
     // C1: 7x7/2 + ReLU, max-pool 3x3/2
     if (run_conv(b, h->stem, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W)) return -2;
-    prof_mark(s, "k_maxpool3s2"); k_maxpool3s2<<<1184, 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
+    prof_mark(s, "k_maxpool3s2"); k_maxpool3s2<<<8 * num_sms(), 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
     H /= 2; W /= 2;
     __nv_bfloat16* x = b->bufB;                      // current block input
     __nv_bfloat16* pool[3] = {b->bufA, b->bufC, b->bufS};
@@ -637,7 +608,7 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     for (int i = 2; i >= 0; --i) {
         if (run_conv(b, h->fpnLat[i], Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s)) return -2;
         __nv_bfloat16* nt = tdBuf[i & 1];
-        prof_mark(s, "k_upsample_add"); k_upsample_add<<<1184, 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
+        prof_mark(s, "k_upsample_add"); k_upsample_add<<<8 * num_sms(), 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
         top = nt;
         if (run_conv(b, h->fpnOut[i], top, fs[i], fs[i], b->P[i], nullptr, 0, s)) return -2;
     }
@@ -678,6 +649,6 @@ extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H
     int newW = (int)lroundf(W * scale), newH = (int)lroundf(H * scale);
     int offx = (S - newW) / 2, offy = (S - newH) / 2;
     prof_mark(h->stream, "k_mold_input");
-    k_mold_input<<<1184, 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, scale, offx, offy, newW, newH, b->input);
+    k_mold_input<<<8 * num_sms(), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, scale, offx, offy, newW, newH, b->input);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }

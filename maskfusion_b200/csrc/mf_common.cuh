@@ -1,4 +1,4 @@
-// mf_common.cuh -- shared device helpers for the sm_100a MaskFusion kernels.
+// mf_common.cuh -- shared device helpers for the sm_90a MaskFusion kernels.
 //
 // Arithmetic contract: every per-element kernel is compiled with -fmad=false and
 // uses only IEEE + - * / sqrt, in the operation order written here, so that its

@@ -1,4 +1,4 @@
-// mf_frame.cu -- per-frame preprocessing kernels (sm_100a):
+// mf_frame.cu -- per-frame preprocessing kernels (sm_90a):
 //   depth bilateral filter        <- Core/Shaders/depth_bilateral_metric.frag:30-76 (MaskFusion::filterDepth)
 //   depth / intensity pyramids    <- Core/Cuda/cudafuncs.cu:333-364, 534-564
 //   vertex + normal maps (fused)  <- Core/Cuda/cudafuncs.cu:109-189 (Model::generateCUDATextures, Model.cpp:350-389)
@@ -21,7 +21,7 @@ __global__ void k_unpack_rgb(const uint8_t* __restrict__ rgb3, uchar4* __restric
 // 13x13 bilateral, one thread per pixel, (32+12)x(8+12) depth tile staged in shared memory.
 // Accumulation order (cy outer, cx inner, ascending) is part of the parity contract.
 #ifndef MFB200_DEFAULT_BILATERAL_BULK
-#define MFB200_DEFAULT_BILATERAL_BULK 1      // validated on the B200: compute-sanitizer clean, bit-exact, 97.1 vs 96.4 us
+#define MFB200_DEFAULT_BILATERAL_BULK 1      // bit-exact with the staging loop (tests/test_gpu_parity.py)
 #endif
 #define BIL_R 6
 #define BIL_BX 32
@@ -96,8 +96,8 @@ __global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral(const float* __res
 // [32 bx - 8, 32 bx + 40) of the 44 columns the filter reads (bulk copies need 16-byte aligned source, destination and size; the halo
 // starts 6 pixels left of the block).  Rows above / below the image and the column ranges left / right of it are zero-filled by the
 // threads themselves (disjoint shared-memory words: no proxy ordering needed); everything else arrives without a single load instruction
-// or bounds branch in the kernel.  The descriptor-based 2-D tensor copy of round 2a (zero fill by the copy engine) trapped in this kernel
-// (profiles/r02_bilateral_tma_sanitizer.txt); the descriptor-free form does the same job.  Arithmetic: bilateralPixel, the same bits out.
+// or bounds branch in the kernel.  The descriptor-based 2-D tensor copy of round 2a (zero fill by the copy engine) trapped in this kernel;
+// the descriptor-free form does the same job.  Arithmetic: bilateralPixel, the same bits out.
 #define BIL_BW (BIL_BX + 16)             // 48 floats per staged row
 #define BIL_XO 2                         // the halo's first column sits at index 2 of the staged row (x0 = 32 bx - 6 = (32 bx - 8) + 2)
 __global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral_bulk(const float* __restrict__ depth, float* __restrict__ out, int W, int H)

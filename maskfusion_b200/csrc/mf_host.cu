@@ -275,8 +275,8 @@ void Model::clean(int time, int timeDelta, float /*depthCutoff*/)
     MaskFusion* o = owner;
     float4* m[3] = {meas[0].p, meas[1].p, meas[2].p};
     const bool inPlace = o->cleanInPlace;
-    // In-place compaction moves only the surfels behind the first removal: 22 us instead of the copy's 68 when removals sit in the young tail
-    // of the store (the steady state), but its ticketed hand-over needs ~140 us when most of a 4.5 M store moves (a removal near the front:
+    // In-place compaction moves only the surfels behind the first removal, cheap when removals sit in the young tail of the store (the
+    // steady state), but its ticketed hand-over is slower than the copy when most of a large store moves (a removal near the front:
     // e.g. the first frames after a map upload).  Both produce the same store, so the choice is free: a large store uses the copy into
     // a second plane set (allocated on first need) for the frame that FOLLOWS one in which more than 40 % of it moved -- the statistic
     // comes back with an asynchronous 8-byte copy and is read without waiting (a stale value only delays the switch).

@@ -1,4 +1,4 @@
-// mf_host.h -- host classes of the B200-native dense pipeline.  Class and method names
+// mf_host.h -- host classes of the H100-native dense pipeline.  Class and method names
 // mirror the reference so that its call sites read the same:
 //   mfb::MaskFusion  <-> MaskFusion   (Core/MaskFusion.h:47-70)
 //   mfb::Model       <-> Model        (Core/Model/Model.h:128-164)
@@ -198,7 +198,7 @@ public:
     int64_t fTimestamp = 0; Mat4 fInPose; bool fHasPose = false, fBootstrap = false;
 
     mf_config cfg; Cam cam; int W, H, P; int device; cudaStream_t stream; bool ownStream;
-    int numSMs = 148;
+    int numSMs = 132;
     bool fuseIndexIntoClean = true;         // Model::predictIndices rides inside the following Model::clean (one stream over the store); MFB200_FUSE_INDEX=0: two passes (A/B)
     bool cleanInPlace = true;               // Model::clean compacts the store in place, touching only the tail behind the first removal; MFB200_CLEAN_INPLACE=0: ping-pong copy of the whole store (A/B)
     bool trackValidBits = true;             // MFB200_TRACK_BITS=0 switches it off: object models carry a validity bitmask of their model maps for the tracker's early reject

@@ -1,4 +1,4 @@
-// mf_kernels.h -- host-callable launchers of the sm_100a kernels and the device-side
+// mf_kernels.h -- host-callable launchers of the sm_90a kernels and the device-side
 // structures they share with the host classes (mf_host.cu).
 #pragma once
 #include <cuda_runtime.h>
@@ -138,6 +138,7 @@ struct TrackJob {
 };
 
 void set_num_sms(int n);
+int num_sms();
 // in-stream stage timer hook (mf_host.cu): records a CUDA event on `s`; the time until the next mark is attributed to `name`
 void prof_mark(cudaStream_t s, const char* name);
 

@@ -1,4 +1,4 @@
-// mf_seg.cu -- geometric depth-edge segmentation kernels (sm_100a)
+// mf_seg.cu -- geometric depth-edge segmentation kernels (sm_90a)
 //   edge-ness (concavity + distance) <- computeGeometricSegmentation_Kernel, Core/Cuda/segmentation.cu:122-177
 //   threshold / invert               <- segmentation.cu:257-269
 //   binary close                     <- dilate_Kernel / erode_Kernel, segmentation.cu:217-255, host :334-354
@@ -171,7 +171,7 @@ __global__ void k_cc_merge(const uint8_t* __restrict__ img, int W, int H, int* L
     if (x > 0 && img[i - 1]) ccUnion(L, i, i - 1);
     if (y > 0 && img[i - W]) ccUnion(L, i, i - W);
 }
-// Two-level union-find (the single global pass over all pixels took 300 us: every pixel hooked roots through L2 atomics, ncu r01i):
+// Two-level union-find (a single global pass over all pixels hooks every root through L2 atomics):
 //   k_cc_tile   : one 32x16 tile per CTA, union-find in SHARED memory over the tile's pixels (left / up neighbours inside the tile);
 //                 every pixel leaves with the GLOBAL index of its tile-local root (roots are the smallest index, and local raster order is
 //                 global raster order inside a tile, so the invariant "root = smallest pixel index of the set" holds for the global pass)
@@ -228,8 +228,8 @@ __global__ void k_cc_number(int* __restrict__ L, int P, int* __restrict__ dense,
     }
 }
 // Integer histogram update with one atomic per distinct bin per warp: neighbouring pixels mostly hit the same bin (one component /
-// one model covers most of the image), and 300 k atomics on ONE address serialise (k_seg_hist, k_mask_overlap and this kernel took
-// 200-300 us each, ncu r01i).  key < 0: this lane adds nothing.  All 32 lanes must call.  Sums of integers: order-free, results identical.
+// one model covers most of the image), and 300 k atomics on ONE address serialise (k_seg_hist, k_mask_overlap and this kernel were
+// bound by them).  key < 0: this lane adds nothing.  All 32 lanes must call.  Sums of integers: order-free, results identical.
 MF_D void warpAggAdd(int* __restrict__ bins, int key)
 {
     const unsigned peers = __match_any_sync(0xffffffffu, key);
@@ -283,7 +283,7 @@ __global__ void k_seg_hist(const int* __restrict__ lab, const uint8_t* __restric
     if (nMasks) warpAggAdd(compMask, in ? c * nMasks + (int)mask[i] : -1);
 }
 // the two component histograms are sized for the worst case (P/2 + 2 components x 64 models / 256 masks: memory is not the
-// constraint on a 180 GB part); only the rows this frame uses are cleared, the counts come from the device
+// constraint: 0.6 GB at 1280x720 on an 80 GB part); only the rows this frame uses are cleared, the counts come from the device
 __global__ void k_clear_hist(const uint32_t* __restrict__ ccCounter, const FrameHdr* __restrict__ hdr, int nModels, int* __restrict__ compModel, int* __restrict__ compMask)
 {
     const size_t nC = (size_t)*ccCounter + 1, nA = nC * nModels, nB = nC * hdr->nMasks;
@@ -437,12 +437,12 @@ void launch_seg_hist(const int* lab, const uint8_t* projID, const uint8_t* mask,
 }
 void launch_clear_hist(const uint32_t* ccCounter, const FrameHdr* hdr, int nModels, int* compModel, int* compMask, cudaStream_t s)
 {
-    prof_mark(s, "k_clear_hist"); k_clear_hist<<<148, 256, 0, s>>>(ccCounter, hdr, nModels, compModel, compMask);
+    prof_mark(s, "k_clear_hist"); k_clear_hist<<<num_sms(), 256, 0, s>>>(ccCounter, hdr, nModels, compModel, compMask);
 }
 void launch_component_map(const uint32_t* ccCounter, const int* area, const int* compModel, const int* compMask, int nModels, const FrameHdr* hdr,
                           const uint8_t* indexToId, int minMapped, int* mapToMask, int* absorb, int* maskPixels, cudaStream_t s)
 {
-    prof_mark(s, "k_component_map"); k_component_map<<<148, 128, 0, s>>>(ccCounter, area, compModel, compMask, nModels, hdr, indexToId, minMapped, mapToMask, absorb, maskPixels);
+    prof_mark(s, "k_component_map"); k_component_map<<<num_sms(), 128, 0, s>>>(ccCounter, area, compModel, compMask, nModels, hdr, indexToId, minMapped, mapToMask, absorb, maskPixels);
 }
 void launch_vote(const FrameHdr* hdr, const VoteParams& vp, const int* maskPixels, const unsigned* maskOverlap, const uint32_t* ccCounter,
                  uint8_t* maskToID, FrameResult* res, cudaStream_t s)

@@ -1,4 +1,4 @@
-// mf_surfel.cu -- surfel-map kernels (sm_100a).  These replace the reference's OpenGL
+// mf_surfel.cu -- surfel-map kernels (sm_90a).  These replace the reference's OpenGL
 // passes; there is no rasteriser here.
 //   predictIndices  <- index_map.vert/.frag,            ModelProjection.cpp:100-152
 //   associate       <- data.vert/.geom/.frag,           Model.cpp:466-581
@@ -236,7 +236,7 @@ struct CleanParams {
 // ---- clean, restructured for dense execution -------------------------------------------------
 // Only surfels that project into the image need the index-map window and they are scattered through
 // the store: evaluated inline per thread the window code ran with ~9 of 32 lanes active, and a
-// warp-cooperative variant was instruction bound (ncu, profiles/).  So each block (1) projects its
+// warp-cooperative variant was instruction bound.  So each block (1) projects its
 // 512 surfels, (2) compacts the ones that need a window into shared memory, (3) runs the window code
 // densely, one compacted entry per thread, (4) hands the counts back to the owning threads.
 struct CleanEntry { float xn, yn, lx, ly, lz, init, rad, lnz; };
@@ -281,7 +281,7 @@ MF_D void cleanWindow(const CleanEntry& e, const CleanParams& P, const CleanTexe
     }
     // The tap coordinates are monotone and span two texels: at most three DISTINCT columns / rows, equal ones adjacent.
     // Compact them (texel, multiplicity) so that the loads of a whole window row can be issued together: walked one texel at a
-    // time every tap paid a full L2 round trip before the next address was even formed (54 % of this kernel, ncu r01g).
+    // time every tap paid a full L2 round trip before the next address was even formed.
     int ux[3] = {0, 0, 0}, wx[3] = {0, 0, 0}, uy[3] = {0, 0, 0}, wy[3] = {0, 0, 0};
     int nux = 0, nuy = 0;
 #pragma unroll
@@ -385,10 +385,10 @@ __global__ void __launch_bounds__(256, 8) k_clean_p1(float4* __restrict__ pos, f
     // resolved after this kernel and read by pass 2 only.  A surfel that is drawn into the index map but needs no window (x or y exactly
     // 0, time gate at equality) is finished by pass 2 as well (flag bit 31): its confidence must not change before the resolve reads it.
     // candidates are staged per block in shared memory and flushed in chunks: one device-wide atomic per ~2k candidates
-    // (a warp-aggregated global append put ~130k returning atomics on ONE L2 address: 62 % busy slice, ncu r01b)
+    // (a warp-aggregated global append put ~130k returning atomics on ONE L2 address)
     // ... and, round 2, per WARP: a warp owns CAND_BUF / 8 slots, appends with a ballot and flushes on its own (one device-wide atomic
-    // per ~220 candidates, coalesced 128-byte copies): no block barrier in the streaming loop (two per round cost 45 % issue-active at
-    // 26 % of the DRAM peak when every surfel of a dense map is a candidate).  The order of the list is irrelevant to pass 2.
+    // per ~220 candidates, coalesced 128-byte copies): no block barrier in the streaming loop (two per round stall it
+    // when every surfel of a dense map is a candidate).  The order of the list is irrelevant to pass 2.
     __shared__ uint32_t sBuf[8][CAND_BUF / 8];
     P.tinv = dpose->tinv;
     const uint32_t count = *countPtr;
@@ -405,7 +405,7 @@ __global__ void __launch_bounds__(256, 8) k_clean_p1(float4* __restrict__ pos, f
         staged = 0;
     };
     // the next round's two planes stream in behind this round's arithmetic and block-wide staging (two barriers per round exposed the
-    // full DRAM latency of every round otherwise: 45 % issue-active at 26 % of the DRAM peak, ncu r02)
+    // full DRAM latency of every round otherwise)
     const uint32_t stride = gridDim.x * blockDim.x;
     float4 vpN = make_float4(0, 0, 0, 0), vcN = vpN;
     { const uint32_t e0 = blockIdx.x * blockDim.x + threadIdx.x; if (e0 < count) { vpN = pos[e0]; vcN = col[e0]; } }
@@ -486,7 +486,7 @@ __global__ void __launch_bounds__(256, 4) k_clean_p2(float4* __restrict__ pos, f
 }
 
 // per-512-element keep counts for the ordered compaction: one WARP per sub-block (16 flag bytes per lane, no block barriers;
-// the block-per-sub-block version spent 14 us in two barriers and a serial 16-term sum per 512 flags)
+// the block-per-sub-block version paid two barriers and a serial 16-term sum per 512 flags)
 __global__ void __launch_bounds__(256) k_keep_block_sums(const uint8_t* __restrict__ keep, const uint32_t* __restrict__ countPtr, int Ppix,
                                                          uint32_t* __restrict__ blockSums, uint32_t* __restrict__ candCount, uint32_t* __restrict__ ticket)
 {
@@ -737,8 +737,8 @@ __global__ void __launch_bounds__(SPLAT_BS, SPLAT_MIN_BLOCKS) k_splat_project(co
     // numbered by an exclusive prefix sum and walked by all threads, unit u belonging to the entry found by binary search.
     // Balanced whatever the mix of far (1 px) and near (large) surfels, and the per-fragment work is the ray/disc test alone:
     // the search and the unit -> (row, x range) arithmetic are paid once per SPLAT_SEG fragments, the pixel ray comes from the
-    // table.  (One search + one integer division + one ray normalisation per FRAGMENT made this kernel instruction bound:
-    // 139 M warp instructions, ncu r01e; a per-thread pixel loop before that ran with ~5 of 32 lanes active.)
+    // table.  (One search + one integer division + one ray normalisation per FRAGMENT made this kernel instruction bound;
+    // a per-thread pixel loop before that ran with ~5 of 32 lanes active.)
     struct Entry { float px, py, pz, nx, ny, nz, rad; int x0, y0, w; uint32_t id; };
     constexpr int NW = SPLAT_BS / 32;
     __shared__ Entry ent[SPLAT_BS];
@@ -791,7 +791,7 @@ __global__ void __launch_bounds__(SPLAT_BS, SPLAT_MIN_BLOCKS) k_splat_project(co
         if (threadIdx.x == 0) offs[nent] = total;
         __syncthreads();
         // gridDim.y > 1 (small stores): the blocks of a column redo the (cheap) vertex stage of the same 128 surfels and share their units --
-        // an object model has ~50 blocks' worth of surfels, and the units of a few large sprites kept one SM busy for 40 us while 100 idled
+        // an object model has ~50 blocks' worth of surfels, and the units of a few large sprites kept one SM busy while the others idled
         for (int u = threadIdx.x + blockIdx.y * blockDim.x; u < total; u += blockDim.x * gridDim.y) {
             int lo = 0, hi = nent - 1;                       // last entry with offs[e] <= u
             while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (offs[mid] <= u) lo = mid; else hi = mid - 1; }
@@ -1017,9 +1017,14 @@ __global__ void k_aos_to_planes(const float4* __restrict__ in, uint32_t n, float
 }
 
 // ------------------------------ host launchers ----------------------------------------
-static int g_numSMs = 148;
-void set_num_sms(int n) { g_numSMs = n > 0 ? n : 148; }
-static inline int persistentBlocks(int perSM) { return g_numSMs * perSM; }
+static int g_numSMs = 0;                 // set by the context; a standalone backbone reads the current device
+void set_num_sms(int n) { g_numSMs = n > 0 ? n : 132; }
+int num_sms()
+{
+    if (!g_numSMs) { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); set_num_sms(n); }
+    return g_numSMs;
+}
+static inline int persistentBlocks(int perSM) { return num_sms() * perSM; }
 
 // host-driven pose (constructor, overridePose, updateStaticPose, C-ABI set_pose) -> device-resident DevPose; matrices by value
 struct Pose2 { float p[16], l[16]; };

@@ -1,4 +1,4 @@
-// mf_track.cu -- dense RGB-D odometry on the device (sm_100a).
+// mf_track.cu -- dense RGB-D odometry on the device (sm_90a).
 //   ICP point-to-plane JtJ/Jtr   <- icpKernel / ICPReduction,        Core/Cuda/reduce.cu:259-444
 //   photometric correspondences  <- residualKernel / RGBResidual,   reduce.cu:774-997
 //   photometric JtJ/Jtr          <- rgbKernel / RGBReduction,        reduce.cu:529-713
@@ -300,7 +300,7 @@ MF_D void blockReduceStore(double* acc, double* partialOut)
 // Sum the per-block partials (rows of 32 doubles, N used) with the WHOLE last block: warp w takes blocks
 // w, w+8, ...; lanes take columns lane and lane+32 (coalesced 128-byte rows, independent loads), doubles
 // throughout; the 8 warp sums are combined in fixed order.  Deterministic for a fixed launch shape.
-// (A single thread per column walking all partials serially cost ~10 us of exposed L2 latency per step.)
+// (A single thread per column walking all partials serially exposes the L2 latency of every partial.)
 template <int N>
 MF_D void sumPartials(const double* __restrict__ partial, unsigned nblocks, double* tot /* shared, >= N */)
 {
@@ -392,8 +392,7 @@ __global__ void __launch_bounds__(TRK_THREADS) k_icp_only(const float4* __restri
 // The whole Gauss-Newton schedule of a frame as ONE cooperative kernel.
 //
 // The reference returns to the host after each of its <= 67 reductions per model per frame; a launch-per-iteration
-// device port (round 1, first version) still paid ~10-45 us of launch + tail latency 38 times per frame, 40 % of the
-// frame.  Here a persistent grid (1 CTA per SM, split between the tracked models along blockIdx.y) walks the schedule
+// device port pays launch + tail latency 38 times per frame.  Here a persistent grid (1 CTA per SM, split between the tracked models along blockIdx.y) walks the schedule
 //     SO(3) pre-alignment (<= 10 its) -> level 2 (4) -> level 1 (5) -> level 0 (10)
 // with one software grid barrier per reduction.  The solver state is REPLICATED: after a barrier every CTA sums the
 // same per-CTA partial rows in the same order and runs the same 6x6 solve, so all CTAs hold bit-identical poses and
@@ -535,7 +534,7 @@ MF_D void sumRows(const double* __restrict__ rows, unsigned R, double (*ws)[ROWF
 // A row travels as 32 x 16 bytes {value.lo, flag, value.hi, flag}: every 8-byte half carries the flag of THIS reduction, 8-byte stores
 // are single transactions, so a reader that finds both flags holds the value -- no release fence on the producer, no arrival counter,
 // no second round trip for the data: the consumers poll the rows themselves.  The software barrier cost one fence + one atomic + one
-// polled counter + one row read per reduction (~2.6-3.5 us of L2 latency, 48 reductions per frame); this costs the row read alone.
+// polled counter + one row read per reduction (48 reductions per frame); this costs the row read alone.
 // Flags are unique per reduction and launch (llBase advances by 64 per launch, 0 is never used), rows ping-pong between two buffers:
 // a CTA writes reduction g + 2 only after it has consumed g + 1 from every peer, which every peer produced after consuming g.
 MF_D void llStore(uint4* p, double v, unsigned flag)
@@ -620,8 +619,8 @@ MF_D void reduceStep(const double* acc, int e0, int e1, bool active, RedCtx& rc,
             uint4* rows = reinterpret_cast<uint4*>(rc.rowsBuf[0]) + (size_t)(rc.gen & 1) * rc.G * ROWF;
             ++rc.gen;
             const unsigned flag = rc.llBase + rc.gen;
-            // (an out-of-line routine shared by the three reductions shrank the loop by 1700 instructions but cost more than it saved: the 32
-            // values travel through local memory: 412 -> 493 us, profiles/r02e_track_timing_outlined_exchange.json)
+            // (an out-of-line routine shared by the three reductions shrank the loop but cost more than it saved: the 32 values travel
+            // through local memory)
             if (active) ctaReduceStoreLL<N>(acc, red, rows + (size_t)rc.bx * ROWF, flag, e0, e1);
             sumRowsLL(rows, rc.Gact, flag, ws, tot);
         } else {
@@ -643,7 +642,7 @@ MF_D void gradU8(const uint8_t* __restrict__ img, int W, int x, int y, float& gx
 
 
 // entry e = (r, c) of the inverse of a 3x3: cofactor(c, r) / det with cyclic indices (no sign bookkeeping, no divergent
-// switch: a 9-way switch serialised the nine lanes, ncu r01d).  Products and differences are the ones inv3d forms.
+// switch: a 9-way switch serialised the nine lanes).  Products and differences are the ones inv3d forms.
 // M is read in place with row stride LD (3 for a 3x3, 4 for the rotation block of a 4x4): no local copies.
 template <int LD>
 MF_D double inv3dEntry(const double* M, int e)
@@ -879,8 +878,8 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     // Pose-independent inputs of this thread's pixels (frame vertex / normal, depth of the photometric pyramid, intensity, validity, image
     // gradient, pixel coordinates) are the same in every iteration of a level: they are read from global memory ONCE per level into
     // shared memory (slot = round * PT_THREADS + thread, structure of arrays: conflict-free 16-byte accesses) and the Gauss-Newton
-    // iterations re-read them from there.  Phase A then issues only its pose-dependent gathers: one L2 round trip instead of two, ~40 %
-    // fewer instructions per pixel (stage clock, profiles/r02_track_timing*.json).  Rounds beyond tp.cacheRounds (720p level 0) use global memory.
+    // iterations re-read them from there.  Phase A then issues only its pose-dependent gathers: one L2 round trip instead of two, fewer
+    // instructions per pixel.  Rounds beyond tp.cacheRounds (720p level 0) use global memory.
     const int cacheSlots = tp.cacheRounds * PT_THREADS;
     unsigned char* const cacheBase = reinterpret_cast<unsigned char*>(corrShared) + (((size_t)tp.corrSlots * sizeof(int2) + 15) & ~(size_t)15);
     float4* const vcS = reinterpret_cast<float4*>(cacheBase);
@@ -1086,8 +1085,8 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
         };
         // (Tried: source pixels whose model-side depth is exactly 0 -- 95 % of an object model's image -- all warp to ONE target pixel, so
         // whether they can correspond is decidable once per iteration and they could skip the photometric projection.  Exact, but the two
-        // dependent loads of that decision sat on the critical path of every iteration: tracker 390 -> 402 us on the single-model replay,
-        // 8 / 3 objects 308 / 580 -> 304 / 567 frames/s.  Removed.)
+        // dependent loads of that decision sat on the critical path of every iteration and made the
+        // tracker slower.  Removed.)
         // addresses of both gathers under the current estimate
         auto stage1 = [&](PixA& p, int k, const float3 tprev) {
             p.rOK = false; p.iOK = false; p.jr = 0; p.ji = 0; p.u0 = 0; p.v0 = 0; p.td1 = 0.f;
@@ -1344,9 +1343,8 @@ static int trackBlocks(int N, int numSMs)
 }
 
 // CTAs of the persistent tracking grid per model (host logic, exported as mf_track_shares for the CPU tests).  A light model (bit set in
-// lightMask: an object model with a validity bitmask) gets one share, a heavy one (full-frame maps) `ratio` shares; measured, frames/s of the
-// 8-object / 3-object scenes: equal shares 251 / 474; ratio 2: 307 / 576; ratio 3: 297 / 557; ratio 5: 297 / 516.  Without both kinds in the
-// batch, or when the grid is too small for 4 CTAs per light model, the shares are equal.
+// lightMask: an object model with a validity bitmask) gets one share, a heavy one (full-frame maps) `ratio` shares (2 by default, the fastest of
+// 1, 2, 3 and 5 on the 8- and 3-object scenes).  Without both kinds in the batch, or when the grid is too small for 4 CTAs per light model, the shares are equal.
 void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* G)
 {
     if (nJobs < 1) return;

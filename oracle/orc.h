@@ -15,7 +15,7 @@
  * PARITY PINNING: the reference ships no tests, golden vectors or fixtures
  * (SURVEY.md section 4).  The CUDA half of the oracle (maps, pyramids, ICP / RGB /
  * SO3 reductions, edge-ness) is pinned against the reference's own kernels
- * recompiled for sm_100 (oracle/_ref, built by oracle/Makefile.ref) on the GPU
+ * recompiled for sm_90a (oracle/_ref, built by oracle/Makefile.ref) on the GPU
  * box; the GLSL half cannot be executed anywhere in this environment (no
  * OpenGL) => "parity unpinned" for those passes; their semantics are fixed in
  * writing in DESIGN.md (rules N1..N14 of SURVEY.md Appendix A).

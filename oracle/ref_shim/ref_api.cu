@@ -3,7 +3,7 @@
 // segmentation.cuh:28-52), compiled from the sources where they lie under /root/reference
 // by oracle/Makefile.ref into oracle/_ref/libmf_ref.so.  Host arrays in, host arrays out
 // (planar 3*rows x cols maps, exactly the reference's DeviceArray2D contents).  Used by
-// tests/test_gpu_ref.py to pin the CPU oracle against the reference's kernels on the B200.
+// tests/test_gpu_ref.py to pin the CPU oracle against the reference's kernels on the GPU.
 #include "cudafuncs.cuh"
 #include "segmentation.cuh"
 #include <cstring>

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Backbone (ResNet-101-FPN, 1024x1024, synthetic weights) timing: tensor-pipe utilisation of the tcgen05 GEMMs.
-Prints one JSON object; used by bench.py (key "backbone") and by the ncu captures."""
+"""Backbone (ResNet-101-FPN, 1024x1024, synthetic weights) timing: tensor-pipe utilisation of the wgmma GEMMs.
+Prints one JSON object; used by bench.py (key "backbone")."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -21,7 +21,7 @@ def run(S=1024, iters=10, warm=3, per_layer=False):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / iters
     fl = bb.flops()
-    peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) else {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+    peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) else {"bf16_tflops": 989.0}      # H100 SXM data sheet, dense BF16, 700 W part
     out = {"input": S, "gemms": bb.numGemms(), "gflop": round(fl / 1e9, 2), "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 2),
            "peak_tflops_burst": peaks["bf16_tflops"], "frac_of_burst_peak": round(fl / ms / 1e9 / peaks["bf16_tflops"], 4)}
     # cuDNN/torch bf16 channels_last conv forward of the same layer stack = library comparison point (BASELINE.md B-cnn)

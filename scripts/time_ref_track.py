@@ -47,7 +47,7 @@ def run(reps=10):
     return {"ref_cuda_us_per_model_frame": round(float(ms[0]) * 1e3, 1),
             "parts_us": {"model_maps": round(float(ms[1]) * 1e3, 1), "rgb_pyramids": round(float(ms[2]) * 1e3, 1),
                          "so3_10_iterations": round(float(ms[3]) * 1e3, 1), "levels_4_5_10": round(float(ms[4]) * 1e3, 1)},
-            "what": "reference reduce.cu/cudafuncs.cu (unmodified, sm_100a, its own flags and launch shapes) in the calling pattern of "
+            "what": "reference reduce.cu/cudafuncs.cu (unmodified, sm_90a, its own flags and launch shapes) in the calling pattern of "
                     "RGBDOdometry.cpp:153-476 on a VGA frame; host Eigen solves and the GL surfel passes not included", "reps": int(reps)}
 
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM + ResNet-101-FPN backbone (csrc/mf_cnn.cu) against a plain PyTorch fp32 reference of the
+"""wgmma GEMM + ResNet-101-FPN backbone (csrc/mf_cnn.cu) against a plain PyTorch fp32 reference of the
 same ops with the same (seeded, bf16-representable) weights.  The reference's real network lives in an
 un-vendored third party (matterport Mask_RCNN + COCO weights + TF 1.8: "parity unpinned", SURVEY 8c), so
 parity here = agreement with the PyTorch restatement of the published architecture.
@@ -38,7 +38,8 @@ def _gemm(mfb, torch, M, N, K, relu, use_res, seed):
 
 
 @pytest.mark.parametrize("M,N,K,relu,res", [(128, 64, 64, 0, 0), (256, 128, 64, 0, 0), (1024, 64, 192, 1, 0), (4096, 256, 576, 1, 1),
-                                            (65536, 64, 64, 1, 0), (1024, 2048, 512, 1, 1), (200, 128, 128, 0, 1)])
+                                            (65536, 64, 64, 1, 0), (1024, 2048, 512, 1, 1), (200, 128, 128, 0, 1),
+                                            (32768, 256, 128, 1, 1)])                  # >= 132 tiles of 128 columns: BN = 128
 def test_gemm_matches_torch(M, N, K, relu, res):
     import torch
     import maskfusion_b200 as mfb
@@ -47,7 +48,8 @@ def test_gemm_matches_torch(M, N, K, relu, res):
     assert err <= 2.0 ** -7 * max(scale, 1.0), (err, scale)       # one bf16 rounding of the output (fp32 accumulate on both sides)
 
 
-@pytest.mark.parametrize("H,W,Cin,Cout", [(256, 256, 64, 64), (128, 128, 128, 128), (64, 64, 256, 256), (32, 32, 512, 512), (16, 16, 256, 256)])
+@pytest.mark.parametrize("H,W,Cin,Cout", [(256, 256, 64, 64), (128, 128, 128, 128), (64, 64, 256, 256), (32, 32, 512, 512), (16, 16, 256, 256),
+                                         (256, 256, 64, 128)])                         # 512 M tiles x 1: BN = 128
 def test_implicit_conv3x3_matches_torch(H, W, Cin, Cout):
     """3x3/s1/p1 convolution through the 3-D TMA map (zero fill == padding), tiles of 128 / (64x2) / (32x4) / (16x8) pixels"""
     import torch

@@ -201,11 +201,10 @@ def test_table_scene_eight_tracked_objects():
         json.dump({"frames": n, "ate_rmse_m": ate, "models": log[-1]["n_c"]}, f)
 
 
-@pytest.mark.skipif(os.environ.get("MF_LONG") != "1", reason="BASELINE configs[4] scene: ~10 s of CPU oracle per frame; run with MF_LONG=1")
 def test_table_scene_720p_sixteen_objects():
     """BASELINE configs[4] shape on one GPU: 1280x720 (the -cal intrinsics 792/792/640/360), sixteen objects on three rows, every model
-    tracked; one spawn per frame.  Same exactness contract as the VGA scene."""
-    log = run(26, track_all=True, tag="_table16_720p", n_objects=16, layout="table", size=(1280, 720), icpWeight=20.0, modelSpawnOffset=1,
+    tracked; a spawn every frame at most (the oracle holds 12 models from frame 38 on).  Same exactness contract as the VGA scene."""
+    log = run(40, track_all=True, tag="_table16_720p", n_objects=16, layout="table", size=(1280, 720), icpWeight=20.0, modelSpawnOffset=1,
               fx=792.0, fy=792.0, cx=640.0, cy=360.0, capacityGlobal=2200000, capacityObject=262144)
     assert log[-1]["n_c"] >= 12, log[-1]["n_c"]          # the partly occluded back-row objects stay below minRelSizeNew (1.5 % of the image)
     check_exact(log, 12)

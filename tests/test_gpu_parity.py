@@ -1,7 +1,7 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on the same
 seeded synthetic inputs.  Integer / index / per-element fp32 outputs must be BIT-EXACT;
 Gauss-Newton reductions (summation order differs) are checked to the tolerances written
-next to each assertion.  Run on the B200 box: pytest -m gpu."""
+next to each assertion.  Run on an H100: pytest -m gpu."""
 from __future__ import annotations
 
 import json
