@@ -8,6 +8,7 @@
 // 3*rows x cols, NaN in the x plane); all loads are 16-byte, coalesced along rows.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "mf_host.h"
 
 namespace mfb {
 
@@ -20,19 +21,17 @@ __global__ void k_unpack_rgb(const uint8_t* __restrict__ rgb3, uchar4* __restric
 
 // 13x13 bilateral, one thread per pixel, (32+12)x(8+12) depth tile staged in shared memory.
 // Accumulation order (cy outer, cx inner, ascending) is part of the parity contract.
-#ifndef MFB200_DEFAULT_BILATERAL_BULK
-#define MFB200_DEFAULT_BILATERAL_BULK 1      // bit-exact with the staging loop (tests/test_gpu_parity.py)
-#endif
 #define BIL_R 6
 #define BIL_BX 32
 #define BIL_BY 8
-// the filter of one pixel from a staged tile: tile[ty][XOFF + tx] holds depth(x0 + tx, y0 + ty), zero outside the image
-template <int PITCH, int XOFF>
-MF_D void bilateralPixel(const float (*tile)[PITCH], float* __restrict__ out, int W, int H, int x0, int y0)
+#define BIL_BW (BIL_BX + 16)             // 48 floats per staged row
+#define BIL_XO 2                         // the halo's first column sits at index 2 of the staged row (x0 = 32 bx - 6 = (32 bx - 8) + 2)
+// the filter of one pixel from the staged tile: tile[ty][BIL_XO + tx] holds depth(x0 + tx, y0 + ty), zero outside the image
+MF_D void bilateralPixel(const float (*tile)[BIL_BW], float* __restrict__ out, int W, int H, int x0, int y0)
 {
     const int x = blockIdx.x * BIL_BX + threadIdx.x, y = blockIdx.y * BIL_BY + threadIdx.y;
     if (x >= W || y >= H) return;
-    const float value = tile[threadIdx.y + BIL_R][XOFF + threadIdx.x + BIL_R];
+    const float value = tile[threadIdx.y + BIL_R][BIL_XO + threadIdx.x + BIL_R];
     if (value <= 0.03f) { out[y * W + x] = 0.0f; return; }
     const float sigma_space2_inv_half = 0.024691358f, sigma_color2_inv_half = 555.556f;
     const int D = 2 * BIL_R + 1;
@@ -45,7 +44,7 @@ MF_D void bilateralPixel(const float (*tile)[PITCH], float* __restrict__ out, in
         for (int iy = 0; iy < D; ++iy) {
             const float dy = (float)(BIL_R - iy);
             const float dy2 = dy * dy;
-            const float* row = &tile[threadIdx.y + iy][XOFF + threadIdx.x];
+            const float* row = &tile[threadIdx.y + iy][BIL_XO + threadIdx.x];
 #pragma unroll
             for (int ix = 0; ix < D; ++ix) {
                 const float tmp = row[ix];
@@ -63,7 +62,7 @@ MF_D void bilateralPixel(const float (*tile)[PITCH], float* __restrict__ out, in
     }
     for (int cy = max(y - D / 2, 0); cy < ty; ++cy) {
         const float dy = (float)y - (float)cy;
-        const float* row = tile[cy - y0] + XOFF;
+        const float* row = tile[cy - y0] + BIL_XO;
         for (int cx = max(x - D / 2, 0); cx < tx; ++cx) {
             float tmp = row[cx - x0];
             float dx = (float)x - (float)cx;
@@ -78,29 +77,13 @@ MF_D void bilateralPixel(const float (*tile)[PITCH], float* __restrict__ out, in
     out[y * W + x] = sum1 / sum2;
 }
 
-__global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral(const float* __restrict__ depth, float* __restrict__ out, int W, int H)
-{
-    __shared__ float tile[BIL_BY + 2 * BIL_R][BIL_BX + 2 * BIL_R + 1];
-    const int x0 = blockIdx.x * BIL_BX - BIL_R, y0 = blockIdx.y * BIL_BY - BIL_R;
-    for (int t = threadIdx.y * BIL_BX + threadIdx.x; t < (BIL_BY + 2 * BIL_R) * (BIL_BX + 2 * BIL_R); t += BIL_BX * BIL_BY) {
-        int ty = t / (BIL_BX + 2 * BIL_R), tx = t - ty * (BIL_BX + 2 * BIL_R);
-        int gx = x0 + tx, gy = y0 + ty;
-        tile[ty][tx] = (gx >= 0 && gx < W && gy >= 0 && gy < H) ? depth[gy * W + gx] : 0.0f;
-    }
-    __syncthreads();
-    bilateralPixel<BIL_BX + 2 * BIL_R + 1, 0>(tile, out, W, H, x0, y0);
-}
-
-// ---- the same filter with the halo tile staged by the bulk-copy engine (north_star: "depth tiles staged through TMA into shared memory") ----
-// One cp.async.bulk (global -> shared, completion on an mbarrier) per tile ROW: 20 rows of 48 floats, the 16-byte aligned superset
+// The halo tile is staged by the bulk-copy engine.  One cp.async.bulk (global -> shared, completion on an mbarrier) per tile ROW: 20 rows of 48 floats, the 16-byte aligned superset
 // [32 bx - 8, 32 bx + 40) of the 44 columns the filter reads (bulk copies need 16-byte aligned source, destination and size; the halo
 // starts 6 pixels left of the block).  Rows above / below the image and the column ranges left / right of it are zero-filled by the
 // threads themselves (disjoint shared-memory words: no proxy ordering needed); everything else arrives without a single load instruction
 // or bounds branch in the kernel.  The descriptor-based 2-D tensor copy of round 2a (zero fill by the copy engine) trapped in this kernel;
-// the descriptor-free form does the same job.  Arithmetic: bilateralPixel, the same bits out.
-#define BIL_BW (BIL_BX + 16)             // 48 floats per staged row
-#define BIL_XO 2                         // the halo's first column sits at index 2 of the staged row (x0 = 32 bx - 6 = (32 bx - 8) + 2)
-__global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral_bulk(const float* __restrict__ depth, float* __restrict__ out, int W, int H)
+// the descriptor-free form does the same job.  Needs 16-byte aligned rows: W % 4 == 0 and a 16-byte aligned image (launch_bilateral checks).
+__global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral(const float* __restrict__ depth, float* __restrict__ out, int W, int H)
 {
     __shared__ __align__(128) float tile[BIL_BY + 2 * BIL_R][BIL_BW];
     __shared__ __align__(8) unsigned long long bar;
@@ -141,7 +124,7 @@ __global__ void __launch_bounds__(BIL_BX* BIL_BY) k_bilateral_bulk(const float* 
         "bra BILB_WAIT;\n\t"
         "BILB_DONE:\n\t}" ::"r"(barAddr) : "memory");
     __syncthreads();                                               // the zero fill of the other threads
-    bilateralPixel<BIL_BW, BIL_XO>(tile, out, W, H, x0, y0);
+    bilateralPixel(tile, out, W, H, x0, y0);
 }
 
 __constant__ float c_gauss5[25] = {1, 4, 6, 4, 1, 4, 16, 24, 16, 4, 6, 24, 36, 24, 6, 4, 16, 24, 16, 4, 1, 4, 6, 4, 1};
@@ -438,11 +421,9 @@ static inline dim3 grid2(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x
 void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, cudaStream_t s) { k_unpack_rgb<<<(P + 255) / 256, 256, 0, s>>>(rgb3, out, P); }
 void launch_bilateral(const float* depth, float* out, int W, int H, cudaStream_t s)
 {
+    // the bulk copies need 16-byte aligned rows (MaskFusion rejects W % 4 != 0; the raw depth sits 16-byte aligned in its frame buffer)
+    if (W % 4 != 0 || ((uintptr_t)depth & 15) != 0) throw CudaError{"bilateral filter: depth rows must be 16-byte aligned (W % 4 == 0, aligned image)"};
     dim3 b(BIL_BX, BIL_BY);
-    // halo tile staged by cp.async.bulk + mbarrier (default; MFB200_BILATERAL_BULK=0: hand-rolled staging loop) (needs 16-byte aligned rows: W % 4 == 0, cudaMalloc'ed image)
-    static int bulk = -1;
-    if (bulk < 0) { const char* e = getenv("MFB200_BILATERAL_BULK"); bulk = e ? (e[0] != '0') : MFB200_DEFAULT_BILATERAL_BULK; }
-    if (bulk && W % 4 == 0 && ((uintptr_t)depth & 15) == 0) { prof_mark(s, "k_bilateral"); k_bilateral_bulk<<<grid2(W, H, b), b, 0, s>>>(depth, out, W, H); return; }
     prof_mark(s, "k_bilateral"); k_bilateral<<<grid2(W, H, b), b, 0, s>>>(depth, out, W, H);
 }
 void launch_pyrdown2_f(const float* src, int sw, int sh, float* dst1, float* dst2, cudaStream_t s)

@@ -123,8 +123,8 @@ Model::Model(MaskFusion* o, unsigned char id_, float conf, bool enableFillIn, in
     const int W = o->W, H = o->H, P = o->P;
     cudaStream_t s = o->stream;
     if (ghost) return;
-    // in-place clean (default): ONE copy of the store; the ping-pong pair only for the A/B path MFB200_CLEAN_INPLACE=0
-    for (int b = 0; b < (o->cleanInPlace ? 1 : 2); ++b) { pos[b].alloc(capacity); col[b].alloc(capacity); nrm[b].alloc(capacity); }
+    // in-place clean: ONE copy of the store; Model::clean allocates the second plane set when it first needs the copy
+    pos[0].alloc(capacity); col[0].alloc(capacity); nrm[0].alloc(capacity);
     count.alloc(2); count.zero(s);
     cudaCheck(cudaMallocHost((void**)&hCount, 2 * sizeof(uint32_t)), "cudaMallocHost"); hCount[0] = hCount[1] = 0;
     cudaCheck(cudaMallocHost((void**)&hTrackOut, 40 * sizeof(float)), "cudaMallocHost");
@@ -141,10 +141,8 @@ Model::Model(MaskFusion* o, unsigned char id_, float conf, bool enableFillIn, in
     keep.alloc((size_t)capacity + P);
     size_t nblk = ((size_t)capacity + P + 511) / 512 + 1;
     blockSums.alloc(nblk); blockSums2.alloc(nblk);
-    if (o->cleanInPlace) {
-        cleanTicket.alloc(4); cleanTicket.zero(s); cleanLoaded.alloc(nblk); cleanLoaded.zero(s);
-        cudaCheck(cudaMallocHost((void**)&hCleanStat, 2 * sizeof(uint32_t)), "cudaMallocHost"); hCleanStat[0] = hCleanStat[1] = 0;
-    }
+    cleanTicket.alloc(4); cleanTicket.zero(s); cleanLoaded.alloc(nblk); cleanLoaded.zero(s);
+    cudaCheck(cudaMallocHost((void**)&hCleanStat, 2 * sizeof(uint32_t)), "cudaMallocHost"); hCleanStat[0] = hCleanStat[1] = 0;
     cand.alloc((size_t)capacity + P); candCount.alloc(1); candCount.zero(s);
     for (int l = 0; l < 3; ++l) {
         size_t Pl = (size_t)(W >> l) * (H >> l);
@@ -203,7 +201,7 @@ void Model::prepareTracking()
     launch_model_maps(splatVertex, splatNormal, fillIn ? fillVertex.p : splatVertex.p, fillIn ? fillNormal.p : splatNormal.p, nb, denom, W, H,
                       dpose, 6.0f /* maxDepthRGB, RGBDOdometry.cpp:34 */, v, n, lastDepth[0], s);
     o->launches += 1;
-    if (validBits[0].p && o->trackValidBits) {
+    if (validBits[0].p) {
         uint32_t* b3[3] = {validBits[0].p, validBits[1].p, validBits[2].p};
         launch_valid_bits3(n, W, H, b3, s);
         o->launches += 1;
@@ -237,7 +235,7 @@ float Model::computeFusionWeight(float weightMultiplier) const
 void Model::predictIndices(int time, float depthCutoff, int timeDelta, bool forClean)
 {
     MaskFusion* o = owner;
-    if (forClean && o->fuseIndexIntoClean) {                          // lazily: see idxDeferred
+    if (forClean) {                                                   // lazily: see idxDeferred
         idxDeferred = true; idxTime = time; idxDelta = timeDelta; idxDepth = depthCutoff;
         return;
     }
@@ -274,19 +272,18 @@ void Model::clean(int time, int timeDelta, float /*depthCutoff*/)
 {
     MaskFusion* o = owner;
     float4* m[3] = {meas[0].p, meas[1].p, meas[2].p};
-    const bool inPlace = o->cleanInPlace;
     // In-place compaction moves only the surfels behind the first removal, cheap when removals sit in the young tail of the store (the
     // steady state), but its ticketed hand-over is slower than the copy when most of a large store moves (a removal near the front:
     // e.g. the first frames after a map upload).  Both produce the same store, so the choice is free: a large store uses the copy into
     // a second plane set (allocated on first need) for the frame that FOLLOWS one in which more than 40 % of it moved -- the statistic
     // comes back with an asynchronous 8-byte copy and is read without waiting (a stale value only delays the switch).
     bool pingPong = false;
-    if (inPlace && capacity >= (1u << 20) && hCleanStat && hCleanStat[1] > 0) {
+    if (capacity >= (1u << 20) && hCleanStat[1] > 0) {
         const uint32_t first = hCleanStat[0], nb = hCleanStat[1];
         pingPong = first < nb && (uint64_t)(nb - first) * 10 > (uint64_t)nb * 4;
     }
     if (pingPong && !pos[1 - target].p) { pos[1 - target].alloc(capacity); col[1 - target].alloc(capacity); nrm[1 - target].alloc(capacity); }
-    int other = (inPlace && !pingPong) ? target : 1 - target, otherCount = 1 - countSel;
+    int other = pingPong ? 1 - target : target, otherCount = 1 - countSel;
     // the pending index projection rides in pass 1 when it uses this call's time gate (always, in the frame schedule)
     const bool fused = idxDeferred && idxTime == time && idxDelta == timeDelta && (size_t)capacity + (size_t)o->P < 0x80000000ull;   // bit 31 of a candidate entry is a flag
     if (!fused) flushIndex();
@@ -300,8 +297,8 @@ void Model::clean(int time, int timeDelta, float /*depthCutoff*/)
     CleanInPlace ip{cleanTicket.p, cleanLoaded.p, cleanTicket.p + 1, cleanEpoch, pingPong};
     launch_clean(planes(target), planes(other), dCount(), count.p + otherCount, capacity, aflag, m, dpose, o->cam, o->W, o->H,
                  time, timeDelta, confidenceThreshold, o->cfg.outlierCoeff, id, win, o->depthFilt, o->mask, keep, blockSums,
-                 cand, candCount, o->stream, fused ? &f : nullptr, inPlace ? &ip : nullptr);
-    if (inPlace && capacity >= (1u << 20))
+                 cand, candCount, o->stream, ip, fused ? &f : nullptr);
+    if (capacity >= (1u << 20))
         cudaCheck(cudaMemcpyAsync(hCleanStat, cleanTicket.p + 1, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, o->stream), "clean statistic D2H");
     target = other; countSel = otherCount;
     o->launches += fused ? 6 : 5;
@@ -326,9 +323,6 @@ MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), d
     cudaCheck(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
     numSMs = prop.multiProcessorCount;
     set_num_sms(numSMs);
-    if (const char* env = getenv("MFB200_FUSE_INDEX")) fuseIndexIntoClean = env[0] != '0';
-    if (const char* env = getenv("MFB200_TRACK_BITS")) trackValidBits = env[0] != '0';
-    if (const char* env = getenv("MFB200_CLEAN_INPLACE")) cleanInPlace = env[0] != '0';
     W = c.width; H = c.height; P = W * H;
     if (W % 4 || H % 4) throw CudaError{"width and height must be multiples of 4 (3-level pyramid)"};
     cam = Cam{c.fx, c.fy, c.cx, c.cy};
@@ -343,15 +337,13 @@ MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), d
     cudaCheck(cudaEventCreateWithFlags(&inputsCopied, cudaEventDisableTiming), "cudaEventCreate");
     cudaCheck(cudaEventCreateWithFlags(&evMain, cudaEventDisableTiming), "cudaEventCreate");
     cudaCheck(cudaEventCreateWithFlags(&evComm, cudaEventDisableTiming), "cudaEventCreate");
-    multiOverlap = true;             // validated bit-exact (single process and 2-rank NCCL); MFB200_MULTI_OVERLAP=0 keeps everything on one stream (A/B)
-    if (const char* env = getenv("MFB200_MULTI_OVERLAP")) multiOverlap = env[0] != '0';
     for (int l = 0; l < 3; ++l) {
         size_t Pl = (size_t)(W >> l) * (H >> l);
         if (l > 0) depthPyr[l].alloc(Pl);
         vmap[l].alloc(Pl); nmap[l].alloc(Pl); nextImage[l].alloc(Pl); nextGrad[l].alloc(Pl); rgbValid[l].alloc(Pl);
     }
     edgeMap.alloc(P); edgeBinary.alloc(P); edgeBuf.alloc(P); edgeInv.alloc(P);
-    dJobs.alloc(TRACK_MAX_JOBS); trackBars.alloc(TRACK_MAX_JOBS * 32);
+    dJobs.alloc(TRACK_MAX_JOBS);
     cudaCheck(cudaMallocHost((void**)&hJobs, TRACK_MAX_JOBS * sizeof(TrackJob)), "cudaMallocHost");
     initFlagR.alloc(P); initFlagF.alloc(P);
     scratch.alloc((size_t)P * 4);
@@ -508,9 +500,9 @@ void MaskFusion::trackModels(const std::vector<Model*>& ms, bool viaResult)
             J.vmapG[l] = m->vmapG[l]; J.nmapG[l] = m->nmapG[l]; J.lastDepth[l] = m->lastDepth[l]; J.lastImage[l] = m->lastImage[l];
             J.cloud[l] = m->cloud[l]; J.corres[l] = m->corres[l];
         }
-        J.lastNextImage2 = m->lastNextImage2; J.st = m->trackState; J.partial = m->partial; J.bar = trackBars.p + j * 32;
+        J.lastNextImage2 = m->lastNextImage2; J.st = m->trackState; J.partial = m->partial;
         J.dpose = m->dpose;
-        for (int l = 0; l < 3; ++l) J.validBits[l] = (m->validBits[l].p && trackValidBits) ? m->validBits[l].p : nullptr;
+        for (int l = 0; l < 3; ++l) J.validBits[l] = m->validBits[l].p;
         if (J.validBits[0] != nullptr) lightMask |= 1u << j;
     }
     if (preWaitPending) {            // the frame's preprocessing ran on preStream: the tracker is the first consumer on the main stream
@@ -521,7 +513,7 @@ void MaskFusion::trackModels(const std::vector<Model*>& ms, bool viaResult)
     // hJobs is reused every frame: the next frameBegin first waits (finalisePending) for an event recorded behind this copy
     cudaCheck(cudaMemcpyAsync(dJobs, hJobs, ms.size() * sizeof(TrackJob), cudaMemcpyHostToDevice, stream), "jobs upload");
     launches += launch_tracking(dJobs, (int)ms.size(), W, H, cam, cfg.rgbOnly != 0, cfg.icpWeight, cfg.pyramid != 0, cfg.fastOdom != 0,
-                                cfg.so3 != 0, numSMs, trackBars, stream, lightMask);
+                                cfg.so3 != 0, numSMs, stream, lightMask);
     prof_mark(stream, "copy_pose_d2h");
     for (Model* m : ms) {
         if (!viaResult)
@@ -804,10 +796,10 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
     // previous frame's images; the copy engine and the issue-bound bilateral overlap well with the HBM-bound clean/scatter).
     // Safe without further events: finalisePending() above has waited for the previous frame's tracker, the last reader of the maps.
     const bool overlap = !multi && world == 1 && tracking && !prof.on;
-    // multi-model frames (MFB200_MULTI_OVERLAP=1): the same idea -- the frame's inputs and preprocessing run on preStream next to the
+    // multi-model frames: the same idea -- the frame's inputs and preprocessing run on preStream next to the
     // previous frame's fusion / clean / prediction tail.  With a communicator ALL collectives are issued on preStream (one stream per
     // communicator: their order is the same on every rank by construction) and tied to the main stream by events.
-    const bool moverlap = multi && multiOverlap && tracking && !prof.on && (world == 1 || shardNccl);
+    const bool moverlap = multi && tracking && !prof.on && (world == 1 || shardNccl);
     if (overlap) {
         selectSet(curSet ^ 1);
         uploadInputs(rgbIn, depthIn, nullptr, timestamp, onDevice, preStream);

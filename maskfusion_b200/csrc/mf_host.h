@@ -185,8 +185,8 @@ public:
     void* backbone = nullptr; int backboneEvery = 0; cudaEvent_t bbFrameReady = nullptr, bbMoldDone = nullptr; bool bbMoldPending = false;
     void attachBackbone(void* bb, int everyK);
     void runBackbone(cudaStream_t producer = nullptr);
-    // multi-model frames with the inputs / preprocessing (and, sharded, every collective) on preStream: MFB200_MULTI_OVERLAP=1
-    bool multiOverlap = false, spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
+    // multi-model frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
+    bool spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
     FrameResult* hRes = nullptr; DevBuf<FrameResult> dRes; cudaEvent_t resEvt = nullptr; bool pendingResult = false;
     DevBuf<float> poseTable, gathered;
     float fWeight = 1.f; int fTick = 0; bool fTracked = false;
@@ -199,9 +199,6 @@ public:
 
     mf_config cfg; Cam cam; int W, H, P; int device; cudaStream_t stream; bool ownStream;
     int numSMs = 132;
-    bool fuseIndexIntoClean = true;         // Model::predictIndices rides inside the following Model::clean (one stream over the store); MFB200_FUSE_INDEX=0: two passes (A/B)
-    bool cleanInPlace = true;               // Model::clean compacts the store in place, touching only the tail behind the first removal; MFB200_CLEAN_INPLACE=0: ping-pong copy of the whole store (A/B)
-    bool trackValidBits = true;             // MFB200_TRACK_BITS=0 switches it off: object models carry a validity bitmask of their model maps for the tracker's early reject
     int tick = 1;
     int64_t launches = 0;
     std::vector<std::unique_ptr<Model>> models;
@@ -227,7 +224,7 @@ public:
     DevBuf<float> depthPyr[3]; DevBuf<float4> vmap[3], nmap[3];
     DevBuf<uint8_t> nextImage[3]; DevBuf<short2> nextGrad[3]; DevBuf<uint8_t> rgbValid[3];
     DevBuf<float> edgeMap; DevBuf<uint8_t> edgeBinary, edgeBuf, edgeInv;
-    DevBuf<TrackJob> dJobs; TrackJob* hJobs = nullptr; DevBuf<unsigned> trackBars;
+    DevBuf<TrackJob> dJobs; TrackJob* hJobs = nullptr;
     DevBuf<uint8_t> initFlagR, initFlagF;
     DevBuf<float> scratch;                  // read-back staging
     DevBuf<float4> rayTab;                  // viewing ray of every pixel centre (camera constant): read by the splat rasteriser

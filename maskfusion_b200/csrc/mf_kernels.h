@@ -133,7 +133,6 @@ struct TrackJob {
     DevPose* dpose;       // initial pose in, tracked pose + derived quantities out
     TrackState* st;
     float* partial;       // 2 x (TRACK_MAX_BLOCKS / 2) rows of 32 x 16 bytes: per-CTA partial sums (fp64 value + flags), ping-pong between reductions
-    unsigned* bar;        // grid barrier counter of this job (own 128-byte line)
     const uint32_t* validBits[3];   // object models: one bit per model-map pixel, set where the model normal is valid (nullptr: not used)
 };
 
@@ -184,7 +183,7 @@ void launch_clean(const SurfelPlanes& src, const SurfelPlanes& dst, const uint32
                   const uint8_t* aflag, float4* const* meas, const DevPose* dpose, Cam cam, int W, int H, int time, int timeDelta, float confThreshold,
                   float outlierCoeff, uint8_t maskID, const CleanWindowImages& win,
                   const float* depthFilt, const uint8_t* mask, uint8_t* keep, uint32_t* blockSums, uint32_t* cand, uint32_t* candCount, cudaStream_t s,
-                  const IndexFused* fused = nullptr, const CleanInPlace* inplace = nullptr);
+                  const CleanInPlace& inplace, const IndexFused* fused = nullptr);
 void launch_combined_predict(const SurfelPlanes& sp, const uint32_t* count, const DevPose* dpose, Cam cam, int W, int H, float maxDepth,
                              float confThreshold, int time, int maxTime, int timeDelta, const float4* rayTab, uint64_t* key, uchar4* image, float4* vertexConf,
                              float4* normalRad, uint16_t* timeTex, int doFill, const float* depthFilt, const uchar4* rgb, int ptVN, int ptImg,
@@ -199,7 +198,7 @@ void launch_aos_to_planes(const float4* in, uint32_t n, const SurfelPlanes& sp, 
 // ---- mf_track.cu ----
 void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* G);   // CTAs per model of the persistent tracking grid
 int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
-                    bool pyramid, bool fastOdom, bool so3, int numSMs, unsigned* bars, cudaStream_t s, unsigned lightMask = false);
+                    bool pyramid, bool fastOdom, bool so3, int numSMs, cudaStream_t s, unsigned lightMask = false);
 int debug_track_timing(long long* out, int cap);
 void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
                      const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, int numSMs, cudaStream_t s);

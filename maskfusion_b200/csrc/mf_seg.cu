@@ -153,24 +153,6 @@ MF_D void ccUnion(int* L, int a, int b)
         a = old;
     }
 }
-// single-pass variant (round 1; kept for A/B runs: MFB200_CC_TILE=0): every pixel hooks roots through L2 atomics
-__global__ void k_cc_init(const uint8_t* __restrict__ img, int P, int* __restrict__ L, int* __restrict__ area, uint32_t* counter)
-{
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i == 0) *counter = 0;
-    if (i >= P) return;
-    L[i] = img[i] ? i : -1;
-    area[i] = 0;
-}
-__global__ void k_cc_merge(const uint8_t* __restrict__ img, int W, int H, int* L)
-{
-    int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= W || y >= H) return;
-    int i = y * W + x;
-    if (!img[i]) return;
-    if (x > 0 && img[i - 1]) ccUnion(L, i, i - 1);
-    if (y > 0 && img[i - W]) ccUnion(L, i, i - W);
-}
 // Two-level union-find (a single global pass over all pixels hooks every root through L2 atomics):
 //   k_cc_tile   : one 32x16 tile per CTA, union-find in SHARED memory over the tile's pixels (left / up neighbours inside the tile);
 //                 every pixel leaves with the GLOBAL index of its tile-local root (roots are the smallest index, and local raster order is
@@ -408,18 +390,10 @@ __global__ void k_proj_resolve(unsigned long long* __restrict__ key, int P, cons
 void launch_cc(const uint8_t* img, int W, int H, int* L, int* dense, int* lab, int* area, int* box, uint32_t* counter, cudaStream_t s)
 {
     int P = W * H;
-    static int tiled = -1;
-    if (tiled < 0) { const char* e = getenv("MFB200_CC_TILE"); tiled = e ? (e[0] != '0') : 1; }
-    if (tiled) {
-        dim3 gt((W + CC_TW - 1) / CC_TW, (H + CC_TH - 1) / CC_TH);
-        prof_mark(s, "k_cc_tile"); k_cc_tile<<<gt, CC_TW * CC_TH, 0, s>>>(img, W, H, L, area, counter);
-        const int nEdge = ((W - 1) / CC_TW) * H + ((H - 1) / CC_TH) * W;
-        if (nEdge > 0) { prof_mark(s, "k_cc_border"); k_cc_border<<<(nEdge + 255) / 256, 256, 0, s>>>(img, W, H, L); }
-    } else {
-        dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
-        prof_mark(s, "k_cc_init"); k_cc_init<<<(P + 255) / 256, 256, 0, s>>>(img, P, L, area, counter);
-        prof_mark(s, "k_cc_merge"); k_cc_merge<<<g, b, 0, s>>>(img, W, H, L);
-    }
+    dim3 gt((W + CC_TW - 1) / CC_TW, (H + CC_TH - 1) / CC_TH);
+    prof_mark(s, "k_cc_tile"); k_cc_tile<<<gt, CC_TW * CC_TH, 0, s>>>(img, W, H, L, area, counter);
+    const int nEdge = ((W - 1) / CC_TW) * H + ((H - 1) / CC_TH) * W;
+    if (nEdge > 0) { prof_mark(s, "k_cc_border"); k_cc_border<<<(nEdge + 255) / 256, 256, 0, s>>>(img, W, H, L); }
     prof_mark(s, "k_cc_number"); k_cc_number<<<(P + 255) / 256, 256, 0, s>>>(L, P, dense, counter, box);
     prof_mark(s, "k_cc_relabel"); k_cc_relabel<<<(P + 255) / 256, 256, 0, s>>>(L, dense, P, W, lab, area, box);
 }

@@ -492,7 +492,7 @@ __global__ void __launch_bounds__(256) k_keep_block_sums(const uint8_t* __restri
 {
     const uint32_t total = *countPtr + (uint32_t)Ppix;
     const uint32_t nblk = (total + SCAN_BLOCK - 1) / SCAN_BLOCK;
-    if (blockIdx.x == 0 && threadIdx.x == 0) { *candCount = 0; if (ticket) *ticket = 0; }       // self-cleaning: ready for the next clean / the compaction below
+    if (blockIdx.x == 0 && threadIdx.x == 0) { *candCount = 0; *ticket = 0; }       // self-cleaning: ready for the next clean / the compaction below
     const uint32_t lane = threadIdx.x & 31, gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t blk = gw; blk < nblk; blk += nw) {
         const uint32_t e0 = blk * SCAN_BLOCK + lane * 16;
@@ -544,7 +544,7 @@ __global__ void __launch_bounds__(1024) k_scan_block_sums(uint32_t* __restrict__
     __syncthreads();
     uint32_t offs = wtot[warp] + incl - run;
     for (uint32_t i = b0; i < b1; ++i) { const uint32_t v = blockSums[i]; blockSums[i] = offs; offs += v; }
-    if (threadIdx.x == 0 && firstMoved) { firstMoved[0] = sFirst; firstMoved[1] = nblk; }      // [1]: read back by the host for its in-place / ping-pong choice
+    if (threadIdx.x == 0) { firstMoved[0] = sFirst; firstMoved[1] = nblk; }      // [1]: read back by the host for its in-place / ping-pong choice
 }
 
 // pass 3: ordered scatter of the survivors (old surfels in buffer order, then new vertices
@@ -1071,7 +1071,7 @@ void launch_clean(const SurfelPlanes& src, const SurfelPlanes& dst, const uint32
                   const uint8_t* aflag, float4* const* meas, const DevPose* tinv, Cam cam, int W, int H, int time, int timeDelta, float confThreshold,
                   float outlierCoeff, uint8_t maskID, const CleanWindowImages& win,
                   const float* depthFilt, const uint8_t* mask, uint8_t* keep, uint32_t* blockSums, uint32_t* cand, uint32_t* candCount, cudaStream_t s,
-                  const IndexFused* fused, const CleanInPlace* inplace)
+                  const CleanInPlace& inplace, const IndexFused* fused)
 {
     const CleanTexels texels{win.packed, win.vertConf, win.colorTime, win.idx};
     CleanParams P;
@@ -1089,11 +1089,11 @@ void launch_clean(const SurfelPlanes& src, const SurfelPlanes& dst, const uint32
     prof_mark(s, "k_clean_p2");
     if (texels.packed) k_clean_p2<true><<<persistentBlocks(8), 256, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], P, tinv, texels, depthFilt, mask, keep, cand, candCount);
     else k_clean_p2<false><<<persistentBlocks(8), 256, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], P, tinv, texels, depthFilt, mask, keep, cand, candCount);
-    prof_mark(s, "k_keep_block_sums"); k_keep_block_sums<<<persistentBlocks(8), 256, 0, s>>>(keep, count, Ppix, blockSums, candCount, inplace ? inplace->ticket : nullptr);
-    prof_mark(s, "k_scan_block_sums"); k_scan_block_sums<<<1, 1024, 0, s>>>(blockSums, count, Ppix, capacity, newCount, inplace ? inplace->firstMoved : nullptr);
-    if (inplace && !inplace->pingPong) {
+    prof_mark(s, "k_keep_block_sums"); k_keep_block_sums<<<persistentBlocks(8), 256, 0, s>>>(keep, count, Ppix, blockSums, candCount, inplace.ticket);
+    prof_mark(s, "k_scan_block_sums"); k_scan_block_sums<<<1, 1024, 0, s>>>(blockSums, count, Ppix, capacity, newCount, inplace.firstMoved);
+    if (!inplace.pingPong) {
         prof_mark(s, "k_clean_compact"); k_clean_compact<<<blocks, SCAN_BLOCK, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
-                                                      inplace->ticket, inplace->loaded, inplace->firstMoved, inplace->epoch);
+                                                      inplace.ticket, inplace.loaded, inplace.firstMoved, inplace.epoch);
     } else {
         prof_mark(s, "k_clean_scatter"); k_clean_scatter<<<blocks, SCAN_BLOCK, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
                                                       dst.pos, dst.col, dst.nrm);

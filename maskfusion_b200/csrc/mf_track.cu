@@ -7,32 +7,28 @@
 //                                   + OdometryProvider::{rodrigues,computeUpdateSE3}, OdometryProvider.h:32-90
 //
 // The reference returns to the host after every one of its <= 67 kernel pairs per model per
-// frame (cudaDeviceSynchronize + 116-byte D2H + Eigen LDLT).  Here the whole schedule is
-// enqueued once: each step kernel reduces with warp shuffles, writes one partial per block,
-// and the LAST block to finish (threadfence + ticket) sums the partials in double in fixed
-// order, solves the 6x6 system (pivoted LDLT, double) and updates the pose state in device
-// memory, which the next launch reads.  blockIdx.y indexes the tracked model, so N objects
-// on one GPU share every launch.  Results are deterministic for a fixed launch shape.
+// frame (cudaDeviceSynchronize + 116-byte D2H + Eigen LDLT).  Here the whole schedule of a
+// frame -- SO(3) pre-alignment, then pyramid levels 2, 1, 0 -- is ONE cooperative launch,
+// k_track_persistent: one CTA per SM, the CTAs split between the tracked models (a flat grid,
+// CTA ranges per model), so N objects on one GPU share the launch.  Every reduction exchanges
+// one fp64 partial row per CTA as flagged words; each CTA then sums all rows of its model in
+// fixed order and runs the same 6x6 solve (pivoted LDLT, double), so the solver state is
+// replicated bit for bit without a broadcast.  Results are deterministic for a fixed launch shape.
+// MFB200_TRACK_CACHE=1 keeps the pose-independent pixel inputs of a level in shared memory (same bits).
+// k_icp_only is a stand-alone ICP reduction at a given pose (last-block ticket) for the parity tests.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 #include "mf_host.h"
 #include <float.h>
 #include <algorithm>
 #include <stdlib.h>
-#include <string.h>
 #include <string>
 
 namespace mfb {
 
-// feature defaults (each has an A/B environment switch; see DESIGN.md 3a)
-#ifndef MFB200_DEFAULT_TRACK_CLUSTER
-#define MFB200_DEFAULT_TRACK_CLUSTER 0
-#endif
+// per-level shared-memory cache of the pose-independent pixel inputs (A/B environment switch MFB200_TRACK_CACHE; see launch_tracking)
 #ifndef MFB200_DEFAULT_TRACK_CACHE
 #define MFB200_DEFAULT_TRACK_CACHE 0
-#endif
-#ifndef MFB200_DEFAULT_TRACK_LL
-#define MFB200_DEFAULT_TRACK_LL 1
 #endif
 #define CACHE_BYTES_PER_SLOT 44        // float4 vertex + float4 normal + depth + packed (valid, intensity, x, y) + Sobel gradient
 #define TRK_THREADS 256
@@ -392,9 +388,9 @@ __global__ void __launch_bounds__(TRK_THREADS) k_icp_only(const float4* __restri
 // The whole Gauss-Newton schedule of a frame as ONE cooperative kernel.
 //
 // The reference returns to the host after each of its <= 67 reductions per model per frame; a launch-per-iteration
-// device port pays launch + tail latency 38 times per frame.  Here a persistent grid (1 CTA per SM, split between the tracked models along blockIdx.y) walks the schedule
+// device port pays launch + tail latency 38 times per frame.  Here a persistent grid (1 CTA per SM, CTA ranges per tracked model) walks the schedule
 //     SO(3) pre-alignment (<= 10 its) -> level 2 (4) -> level 1 (5) -> level 0 (10)
-// with one software grid barrier per reduction.  The solver state is REPLICATED: after a barrier every CTA sums the
+// with one flagged exchange of partial rows per reduction.  The solver state is REPLICATED: after an exchange every CTA sums the
 // same per-CTA partial rows in the same order and runs the same 6x6 solve, so all CTAs hold bit-identical poses and
 // take identical break decisions without a second barrier or a broadcast.  Per-pixel data that a later phase needs
 // (photometric correspondences, validity) is written and re-read by the same thread.
@@ -414,11 +410,9 @@ struct TrackParams {
     int corrSlots;                     // photometric correspondences kept per CTA in shared memory (0: global scratch instead)
     int bitWords;                      // shared-memory words reserved for the model-map validity bitmask of a level (0: none)
     int cacheRounds;                   // pixel rounds per thread whose pose-independent inputs are kept in shared memory across the iterations of a level
-    int phase;                         // 0: whole schedule in this launch; 1: SO(3) + level 2 only (cluster kernel); 2: resume at level 1
-    unsigned llBase;                   // != 0: the partial rows are exchanged as flagged words (flag = llBase + index of the reduction in the launch)
-    // flat grid (persistent kernel): CTA b belongs to the job j with jobStart[j] <= b < jobStart[j + 1] -- the models of a batch get
-    // DIFFERENT numbers of CTAs (a full-frame model walks 307 k live pixels per iteration, an object model rejects nearly all of them on its
-    // validity bitmask); nJobs == 0: the rectangular grid (blockIdx.y = job) of the cluster kernel
+    unsigned llBase;                   // flag of the partial rows of reduction g of this launch: llBase + g (never 0)
+    // flat grid: CTA b belongs to the job j with jobStart[j] <= b < jobStart[j + 1] -- the models of a batch get DIFFERENT numbers of
+    // CTAs (a full-frame model walks 307 k live pixels per iteration, an object model rejects nearly all of them on its validity bitmask)
     int nJobs; unsigned short jobStart[TRACK_MAX_JOBS + 1];
 };
 
@@ -444,92 +438,6 @@ MF_D void warpReduceHalving32(double* v)
     }
 }
 
-// CTA-wide fp64 sum of N (<= 29) accumulators -> one row of 32 doubles in global memory (row = this CTA's partial); two integer
-// counters ride in columns 29 and 30 (exact in fp64).  Accumulating the exact products of floats in fp64 makes the totals agree with
-// a sequential fp64 sum to ~1e-15 relative whatever the order: rounded to float (the reference's result record) they are the
-// oracle's values bit for bit, which is what keeps tracked trajectories identical instead of merely close (DESIGN.md section 4).
-template <int N>
-MF_D void ctaReduceStore(const double* acc, double (*red)[ROWF], double* __restrict__ rowOut, int extra0 = 0, int extra1 = 0)
-{
-    double v[32];
-#pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = k < N ? acc[k] : 0.0;
-    v[29] = (double)extra0; v[30] = (double)extra1;
-    warpReduceHalving32(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    red[warp][lane] = v[0];
-    __syncthreads();
-    if (threadIdx.x < ROWF) {
-        double s = 0;
-#pragma unroll
-        for (int w = 0; w < PT_WARPS; ++w) s += red[w][threadIdx.x];
-        rowOut[threadIdx.x] = s;
-    }
-}
-
-// all CTAs of one model: arrive (release: this CTA's partial row is visible first), then wait until `target` arrivals have been
-// counted since the launch (monotonic counter, acquire)
-MF_D void gridBarrier(unsigned* bar, unsigned target)
-{
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(bar) : "memory");
-        unsigned v;
-        do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while (v < target);
-    }
-    __syncthreads();
-}
-
-// ---- thread-block cluster primitives (sm_90+): hardware barrier over the CTAs of a cluster, loads from a peer CTA's shared memory ----
-MF_D void clusterSync()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-MF_D unsigned clusterSize() { unsigned r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
-MF_D double ldClusterF64(const double* localShared, unsigned rank)
-{
-    const unsigned a = (unsigned)__cvta_generic_to_shared(localShared);
-    unsigned ra; double v;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(a), "r"(rank));
-    asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(ra) : "memory");
-    return v;
-}
-
-// every CTA: sum the R partial rows (fixed order, fp64) -> tot[0..32); columns 29/30 carry the integer counters.
-// Warp w owns rows w, w+16, ...; the rows of a batch are all loaded before the first add (one L2 round trip for R <= 160).
-#define SUM_BATCH 10
-MF_D void sumRows(const double* __restrict__ rows, unsigned R, double (*ws)[ROWF], double* tot)
-{
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double a0 = 0;
-    for (unsigned base = warp; base < R; base += PT_WARPS * SUM_BATCH) {
-        double x[SUM_BATCH];
-#pragma unroll
-        for (int i = 0; i < SUM_BATCH; ++i) {
-            const unsigned b = base + (unsigned)i * PT_WARPS;
-            x[i] = b < R ? __ldcg(rows + (size_t)b * ROWF + lane) : 0.0;
-        }
-#pragma unroll
-        for (int i = 0; i < SUM_BATCH; ++i) a0 += x[i];
-    }
-    ws[warp][lane] = a0;
-    __syncthreads();
-    if (threadIdx.x < ROWF) {
-        double s2 = 0;
-#pragma unroll
-        for (int w = 0; w < PT_WARPS; ++w) s2 += ws[w][threadIdx.x];
-        tot[threadIdx.x] = s2;
-    }
-    __syncthreads();
-}
-
-// One reduction of the schedule: CTA partial -> exchange -> every CTA holds the same totals (replicated solver state, no broadcast).
-//   CL == false: partial rows in global memory + software grid barrier over the G CTAs of the model (any grid size)
-//   CL == true : the G CTAs of the model form ONE thread-block cluster: the partial row stays in the CTA's shared memory
-//                (double-buffered), barrier.cluster replaces the L2 round trips of the software barrier, the rows of the peers are read
-//                through distributed shared memory.  Used for SO(3) pre-alignment and level 2 (19 k pixels: 14 iterations whose cost
-//                is the reduction, not the pixels).
 // ---- flagged exchange of the partial rows (the LL scheme of collective libraries) ----
 // A row travels as 32 x 16 bytes {value.lo, flag, value.hi, flag}: every 8-byte half carries the flag of THIS reduction, 8-byte stores
 // are single transactions, so a reader that finds both flags holds the value -- no release fence on the producer, no arrival counter,
@@ -547,8 +455,13 @@ MF_D uint4 llLoad(const uint4* p)
     asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
     return r;
 }
+
+// CTA-wide fp64 sum of N (<= 29) accumulators -> one row of 32 flagged doubles in global memory (row = this CTA's partial); two integer
+// counters ride in columns 29 and 30 (exact in fp64).  Accumulating the exact products of floats in fp64 makes the totals agree with
+// a sequential fp64 sum to ~1e-15 relative whatever the order: rounded to float (the reference's result record) they are the
+// oracle's values bit for bit, which is what keeps tracked trajectories identical instead of merely close (DESIGN.md section 4).
 template <int N>
-MF_D void ctaReduceStoreLL(const double* acc, double (*red)[ROWF], uint4* __restrict__ rowOut, unsigned flag, int extra0, int extra1)
+MF_D void ctaReduceStore(const double* acc, double (*red)[ROWF], uint4* __restrict__ rowOut, unsigned flag, int extra0, int extra1)
 {
     double v[32];
 #pragma unroll
@@ -565,8 +478,11 @@ MF_D void ctaReduceStoreLL(const double* acc, double (*red)[ROWF], uint4* __rest
         llStore(rowOut + threadIdx.x, s, flag);
     }
 }
-// same summation order as sumRows (warp w: rows w, w + 16, ... ascending; then the 16 warp sums ascending)
-MF_D void sumRowsLL(const uint4* __restrict__ rows, unsigned R, unsigned flag, double (*ws)[ROWF], double* tot)
+// every CTA: sum the R partial rows (fixed order, fp64) -> tot[0..32); columns 29/30 carry the integer counters.  Summation order:
+// warp w adds rows w, w + 16, ... ascending, then the 16 warp sums are added ascending.  The rows of a batch are all polled until
+// their flags match before the first add (one L2 round trip for R <= 160).
+#define SUM_BATCH 10
+MF_D void sumRows(const uint4* __restrict__ rows, unsigned R, unsigned flag, double (*ws)[ROWF], double* tot)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     double a0 = 0;
@@ -584,7 +500,7 @@ MF_D void sumRowsLL(const uint4* __restrict__ rows, unsigned R, unsigned flag, d
                 if ((pending >> i) & 1u) { if (__all_sync(0xffffffffu, x[i].y == flag && x[i].w == flag)) pending &= ~(1u << i); }
         }
 #pragma unroll
-        for (int i = 0; i < SUM_BATCH; ++i) a0 += __hiloint2double((int)x[i].z, (int)x[i].x);      // rows beyond R contribute +0.0 as in sumRows
+        for (int i = 0; i < SUM_BATCH; ++i) a0 += __hiloint2double((int)x[i].z, (int)x[i].x);      // rows beyond R contribute +0.0
     }
     ws[warp][lane] = a0;
     __syncthreads();
@@ -597,39 +513,20 @@ MF_D void sumRowsLL(const uint4* __restrict__ rows, unsigned R, unsigned flag, d
     __syncthreads();
 }
 
-struct RedCtx { double* rowsBuf[2]; unsigned* bar; unsigned G, Gact, gen, llBase, bx; };
-template <bool CL, bool LL, int N>
-MF_D void reduceStep(const double* acc, int e0, int e1, bool active, RedCtx& rc, double (*red)[ROWF], double (*ws)[ROWF], double (*rowSh)[ROWF], double* tot)
+// One reduction of the schedule: CTA partial -> flagged exchange -> every CTA holds the same totals (replicated solver state, no
+// broadcast).  G CTAs of the model, the first Gact of them active.
+struct RedCtx { uint4* rows; unsigned G, Gact, gen, llBase, bx; };
+template <int N>
+MF_D void reduceStep(const double* acc, int e0, int e1, bool active, RedCtx& rc, double (*red)[ROWF], double (*ws)[ROWF], double* tot)
 {
-    if (CL) {
-        ctaReduceStore<N>(acc, red, rowSh[rc.gen & 1], e0, e1);
-        const double* mine = rowSh[rc.gen & 1];
-        ++rc.gen;
-        __syncthreads();
-        clusterSync();
-        if (threadIdx.x < ROWF) {
-            double s2 = 0;
-            for (unsigned r = 0; r < rc.G; ++r) s2 += ldClusterF64(mine + threadIdx.x, r);
-            tot[threadIdx.x] = s2;
-        }
-        __syncthreads();
-    } else {
-        if (LL) {
-            // 16 bytes per value: the two ping-pong buffers are 2 * G * ROWF doubles each
-            uint4* rows = reinterpret_cast<uint4*>(rc.rowsBuf[0]) + (size_t)(rc.gen & 1) * rc.G * ROWF;
-            ++rc.gen;
-            const unsigned flag = rc.llBase + rc.gen;
-            // (an out-of-line routine shared by the three reductions shrank the loop but cost more than it saved: the 32 values travel
-            // through local memory)
-            if (active) ctaReduceStoreLL<N>(acc, red, rows + (size_t)rc.bx * ROWF, flag, e0, e1);
-            sumRowsLL(rows, rc.Gact, flag, ws, tot);
-        } else {
-            double* rows = rc.rowsBuf[rc.gen & 1];
-            if (active) ctaReduceStore<N>(acc, red, rows + (size_t)rc.bx * ROWF, e0, e1);
-            ++rc.gen; gridBarrier(rc.bar, rc.gen * rc.G);
-            sumRows(rows, rc.Gact, ws, tot);
-        }
-    }
+    // 16 bytes per value: the two ping-pong buffers are G * ROWF values each
+    uint4* rows = rc.rows + (size_t)(rc.gen & 1) * rc.G * ROWF;
+    ++rc.gen;
+    const unsigned flag = rc.llBase + rc.gen;
+    // (an out-of-line routine shared by the three reductions shrank the loop but cost more than it saved: the 32 values travel
+    // through local memory)
+    if (active) ctaReduceStore<N>(acc, red, rows + (size_t)rc.bx * ROWF, flag, e0, e1);
+    sumRows(rows, rc.Gact, flag, ws, tot);
 }
 
 MF_D void gradU8(const uint8_t* __restrict__ img, int W, int x, int y, float& gx, float& gy)
@@ -661,7 +558,7 @@ MF_D double inv3dEntry(const double* M, int e)
 #ifdef MF_TRACK_TIMING
 __device__ long long g_trackTiming[8192];
 __device__ int g_trackTimingN;
-#define TT(tag) do { if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) { int q_ = g_trackTimingN; if (q_ + 2 <= 8192) { g_trackTiming[q_] = (tag); g_trackTiming[q_ + 1] = clock64(); g_trackTimingN = q_ + 2; } } } while (0)
+#define TT(tag) do { if (blockIdx.x == 0 && threadIdx.x == 0) { int q_ = g_trackTimingN; if (q_ + 2 <= 8192) { g_trackTiming[q_] = (tag); g_trackTiming[q_ + 1] = clock64(); g_trackTimingN = q_ + 2; } } } while (0)
 #else
 #define TT(tag) do { } while (0)
 #endif
@@ -811,11 +708,8 @@ struct PixA {
 
 extern __shared__ int2 corrShared[];
 
-
-// LL: the partial rows travel as flagged words (compile-time: the other exchange is not even instantiated -- the kernel's loop body
-// has to stay inside the instruction cache)
-template <bool CL, bool LL>
-MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
+// the whole schedule of a frame for every tracked model: cooperative launch, one CTA per SM
+__global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJob* __restrict__ jobs, TrackParams tp)
 {
     __shared__ TrackJob J;
     __shared__ TrackState S;
@@ -824,34 +718,25 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     __shared__ double ws[PT_WARPS][ROWF];
     __shared__ double tot[64];
     __shared__ double totR[ROWF];
-    __shared__ double rowSh[2][ROWF];                                  // cluster variant: this CTA's partial row, double buffered
     __shared__ float so3B[9], so3Kinv[9], so3Krlr[9];
     __shared__ double so3K[9], so3KinvD[9];
     __shared__ int flag;
-    unsigned bx = blockIdx.x, by = blockIdx.y, Gj = gridDim.x;         // CTA index within its model, model, CTAs of the model
-    if (!CL && tp.nJobs > 0) {
-        by = 0;
-        while ((int)by + 1 < tp.nJobs && blockIdx.x >= tp.jobStart[by + 1]) ++by;
-        bx = blockIdx.x - tp.jobStart[by]; Gj = (unsigned)tp.jobStart[by + 1] - tp.jobStart[by];
-    }
+    unsigned job = 0;                                                  // the model of this CTA
+    while ((int)job + 1 < tp.nJobs && blockIdx.x >= tp.jobStart[job + 1]) ++job;
+    const unsigned bx = blockIdx.x - tp.jobStart[job];                 // CTA index within its model
+    const unsigned G = (unsigned)tp.jobStart[job + 1] - tp.jobStart[job];      // CTAs of this model
     {   // job record -> shared memory (one coalesced read instead of dependent pointer chases in every phase)
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(jobs + by);
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(jobs + job);
         uint32_t* dst = reinterpret_cast<uint32_t*>(&J);
         for (int k = threadIdx.x; k < (int)(sizeof(TrackJob) / 4); k += PT_THREADS) dst[k] = src[k];
     }
     TrackState* st = &S;
 #ifdef MF_TRACK_TIMING
-    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) g_trackTimingN = 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) g_trackTimingN = 0;
 #endif
     TT(1);
-    const unsigned G = Gj;                                             // CTAs of this model (cluster variant: == cluster size)
     __syncthreads();
-    if (tp.phase == 2) {
-        // second launch of the frame: the replicated solver state as the cluster kernel left it
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(J.st);
-        uint32_t* dst = reinterpret_cast<uint32_t*>(&S);
-        for (int k = threadIdx.x; k < (int)(sizeof(TrackState) / 4); k += PT_THREADS) dst[k] = __ldcg(src + k);
-    } else if (threadIdx.x == 0) {
+    if (threadIdx.x == 0) {
         // RGBDOdometry.cpp:331-345 initial state; the model's pose is device resident (written by the previous frame's epilogue or k_set_pose)
         const float* P = J.dpose->pose.m;
         for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) st->Rprev[r * 3 + c] = P[r * 4 + c]; st->tprev[r] = P[r * 4 + 3]; }
@@ -869,8 +754,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     }
     __syncthreads();
     RedCtx rc;
-    rc.rowsBuf[0] = reinterpret_cast<double*>(J.partial); rc.rowsBuf[1] = reinterpret_cast<double*>(J.partial) + (size_t)G * ROWF;
-    rc.bar = J.bar; rc.G = G; rc.Gact = G; rc.gen = 0; rc.llBase = CL ? 0u : tp.llBase; rc.bx = bx;
+    rc.rows = reinterpret_cast<uint4*>(J.partial); rc.G = G; rc.Gact = G; rc.gen = 0; rc.llBase = tp.llBase; rc.bx = bx;
     // photometric correspondences of this thread's pixels, slot = round * PT_THREADS + thread: written in phase A, read in phase B
     // by the same thread.  Shared memory when the launch reserved enough, else a private stripe of the model's scratch buffer.
     const size_t corrNeed = (size_t)((tp.W * tp.H + G * PT_THREADS - 1) / (G * PT_THREADS)) * PT_THREADS;      // slots of this CTA at level 0 (depends on the model's share of the grid)
@@ -890,7 +774,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     uint32_t* const bitsS = gS + cacheSlots;                                       // validity bitmask of the model's normal map at this level
 
     // ---------------- SO(3) pre-alignment on level-2 intensities (RGBDOdometry.cpp:272-345) ----------------
-    if (tp.so3 && tp.phase != 2) {
+    if (tp.so3) {
         const int W = tp.W >> 2, H = tp.H >> 2, N = W * H;
         // CTAs beyond the pixel count only wait at the barriers: fewer partial rows to sum
         const unsigned Gact = min(G, (unsigned)((N + PT_THREADS - 1) / PT_THREADS));
@@ -956,7 +840,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
             }
             TT(12);
             rc.Gact = Gact;
-            reduceStep<CL, LL, 11>(acc, 0, 0, active, rc, red, ws, rowSh, tot);
+            reduceStep<11>(acc, 0, 0, active, rc, red, ws, tot);
             TT(15);
             if (threadIdx.x < 32) {
                 // host logic of RGBDOdometry.cpp:301-324 on warp 0: lane 0 takes the decisions, the 3x3 solve is warp-cooperative
@@ -1006,7 +890,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     }
 
     // ---------------- pyramid levels, coarse to fine (RGBDOdometry.cpp:347-476) ----------------
-    for (int level = (tp.phase == 2 ? 1 : 2); level >= (tp.phase == 1 ? 2 : 0); --level) {
+    for (int level = 2; level >= 0; --level) {
         if (tp.iterations[level] == 0) continue;
         const int W = tp.W >> level, H = tp.H >> level, N = W * H;
         const unsigned Gact = min(G, (unsigned)((N + PT_THREADS - 1) / PT_THREADS));
@@ -1051,7 +935,6 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
         }
         __syncthreads();
 
-        // pose-independent inputs of pixel k
         // object models: validity bitmask of this level's model maps -> shared memory (every CTA holds the whole level: gathers go anywhere)
         const bool useBits = tp.icp && tp.bitWords > 0 && J.validBits[level] != nullptr && (N + 31) / 32 <= tp.bitWords;
         if (useBits) {
@@ -1070,6 +953,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
             if (tp.icp) { vc = vmapC[k]; nc = nmapC[k]; }
             vcS[slot] = vc; ncS[slot] = nc; d1S[slot] = d1; pkS[slot] = pk; gS[slot] = g;
         }
+        // pose-independent inputs of pixel k (round r)
         auto stage0 = [&](PixA& p, int k, int r) {
             if (r < cRounds) {
                 const int slot = r * PT_THREADS + threadIdx.x;
@@ -1196,7 +1080,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
             rc.Gact = Gact;
             // phase B's first streaming inputs (pose independent) -> L1 while this CTA waits at the reduction
             if (tp.rgb && rounds > cRounds) { prefetchL1(grad + kOf(cRounds)); }
-            reduceStep<CL, LL, NACC_ICP>(acc, cnt, sig, active, rc, red, ws, rowSh, tot);
+            reduceStep<NACC_ICP>(acc, cnt, sig, active, rc, red, ws, tot);
             TT(5);
             if (tp.rgb) {
                 if (threadIdx.x == 0) {
@@ -1270,7 +1154,7 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
                         prefetchL1(nextDepth + kn);
                     }
                 // ICP totals stay in tot[0..28]; the photometric ones go behind them
-                reduceStep<CL, LL, NACC_RGB>(accR, 0, 0, active, rc, red, ws, rowSh, totR);
+                reduceStep<NACC_RGB>(accR, 0, 0, active, rc, red, ws, totR);
                 TT(9);
                 if (threadIdx.x < NACC_RGB) tot[NACC_ICP + threadIdx.x] = totR[threadIdx.x];
                 __syncthreads();
@@ -1283,18 +1167,6 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     }
 
     TT(99);
-    if (tp.phase == 1) {
-        // hand the replicated state to the second launch (every CTA holds the same bits: rank 0 writes); a CTA must not exit while a
-        // peer may still read its shared memory
-        __syncthreads();
-        if (bx == 0) {
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(&S);
-            uint32_t* dst = reinterpret_cast<uint32_t*>(J.st);
-            for (int k = threadIdx.x; k < (int)(sizeof(TrackState) / 4); k += PT_THREADS) dst[k] = src[k];
-        }
-        if (CL) clusterSync();
-        return;
-    }
     // ---------------- result (RGBDOdometry.cpp:478-497) ----------------
     if (bx == 0 && threadIdx.x == 0) {
         float dx = st->tcurr[0] - st->tprev[0], dy = st->tcurr[1] - st->tprev[1], dz = st->tcurr[2] - st->tprev[2];
@@ -1319,13 +1191,6 @@ MF_D void trackBody(const TrackJob* __restrict__ jobs, const TrackParams& tp)
     }
 }
 
-// whole schedule (phase 0) or levels 1..0 (phase 2): cooperative launch, one CTA per SM, software grid barrier
-__global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJob* __restrict__ jobs, TrackParams tp) { trackBody<false, true>(jobs, tp); }
-// the same with the counter barrier + plain rows (MFB200_TRACK_LL=0, A/B)
-__global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent_bar(const TrackJob* __restrict__ jobs, TrackParams tp) { trackBody<false, false>(jobs, tp); }
-// SO(3) pre-alignment + level 2 (phase 1): one thread-block cluster per tracked model
-__global__ void __launch_bounds__(PT_THREADS, 1) k_track_cluster(const TrackJob* __restrict__ jobs, TrackParams tp) { trackBody<true, false>(jobs, tp); }
-
 // ------------------------------ host launchers ----------------------------------------
 float track_min_scale(int level)
 {
@@ -1343,8 +1208,8 @@ static int trackBlocks(int N, int numSMs)
 }
 
 // CTAs of the persistent tracking grid per model (host logic, exported as mf_track_shares for the CPU tests).  A light model (bit set in
-// lightMask: an object model with a validity bitmask) gets one share, a heavy one (full-frame maps) `ratio` shares (2 by default, the fastest of
-// 1, 2, 3 and 5 on the 8- and 3-object scenes).  Without both kinds in the batch, or when the grid is too small for 4 CTAs per light model, the shares are equal.
+// lightMask: an object model with a validity bitmask) gets one share, a heavy one (full-frame maps) `ratio` shares (launch_tracking passes 2, the
+// fastest of 1, 2, 3 and 5 on the 8- and 3-object scenes).  Without both kinds in the batch, or when the grid is too small for 4 CTAs per light model, the shares are equal.
 void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* G)
 {
     if (nJobs < 1) return;
@@ -1364,12 +1229,12 @@ void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* 
 }
 
 int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
-                    bool pyramid, bool fastOdom, bool so3, int numSMs, unsigned* bars, cudaStream_t s, unsigned lightMask)
+                    bool pyramid, bool fastOdom, bool so3, int numSMs, cudaStream_t s, unsigned lightMask)
 {
     const bool anyValidBits = lightMask != 0;          // bit j: job j is an object model with a validity bitmask (nearly all of its pixels are rejected early)
     // per-device launch limits (several contexts on different GPUs may live in one process): occupancy and the opt-in
     // dynamic shared memory attribute are properties of (function, device)
-    static int coResidentDev[64]; static size_t dynMaxDev[64], dynMaxClDev[64]; static bool devInit[64]; static int clusterOkDev[64];
+    static int coResidentDev[64]; static size_t dynMaxDev[64]; static bool devInit[64];
     int dev = 0; cudaCheck(cudaGetDevice(&dev), "cudaGetDevice");
     if (dev < 0 || dev >= 64) throw CudaError{"device ordinal above 63"};
     if (!devInit[dev]) {
@@ -1381,15 +1246,6 @@ int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgb
         cudaFuncAttributes fa; cudaCheck(cudaFuncGetAttributes(&fa, k_track_persistent), "cudaFuncGetAttributes");
         dynMaxDev[dev] = (size_t)optin > fa.sharedSizeBytes + 2048 ? (size_t)optin - fa.sharedSizeBytes - 2048 : 0;
         cudaCheck(cudaFuncSetAttribute(k_track_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dynMaxDev[dev]), "cudaFuncSetAttribute");
-        cudaCheck(cudaFuncSetAttribute(k_track_persistent_bar, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dynMaxDev[dev]), "cudaFuncSetAttribute");
-        cudaCheck(cudaFuncGetAttributes(&fa, k_track_cluster), "cudaFuncGetAttributes");
-        dynMaxClDev[dev] = (size_t)optin > fa.sharedSizeBytes + 2048 ? (size_t)optin - fa.sharedSizeBytes - 2048 : 0;
-        // clusters of 16 CTAs are a non-portable size: opt in; if either attribute is refused the frame runs as one cooperative launch
-        clusterOkDev[dev] = 1;
-        if (cudaFuncSetAttribute(k_track_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dynMaxClDev[dev]) != cudaSuccess) clusterOkDev[dev] = 0;
-        if (cudaFuncSetAttribute(k_track_cluster, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) clusterOkDev[dev] = 0;
-        cudaGetLastError();
-        { const char* env = getenv("MFB200_TRACK_CLUSTER"); if (!(env ? env[0] != '0' : MFB200_DEFAULT_TRACK_CLUSTER)) clusterOkDev[dev] = 0; }
         devInit[dev] = true;
     }
     const int coResident = coResidentDev[dev];
@@ -1403,86 +1259,44 @@ int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgb
     tp.angleThres = (float)sin(20.f * 3.14159254f / 180.f);
     tp.distThres = 0.10f; tp.sobelScale = (float)(1.0 / 8.0); tp.maxDepthDelta = 0.07f;
     for (int l = 0; l < 3; ++l) tp.minScale[l] = track_min_scale(l);
-    tp.phase = 0; tp.cacheRounds = 0; tp.bitWords = 0; tp.llBase = 0;
-    static int llOn = -1;           // MFB200_TRACK_LL=0: counter barrier + plain rows instead of the flagged exchange (A/B)
-    if (llOn < 0) { const char* e = getenv("MFB200_TRACK_LL"); llOn = e ? (e[0] != '0') : MFB200_DEFAULT_TRACK_LL; }
     static unsigned llEpoch[64];    // per device; every launch owns 64 flag values
-    if (llOn) {
-        unsigned ep = ++llEpoch[dev];
-        if ((ep << 6) == 0u) ep = ++llEpoch[dev];           // flag 0 means "never written"
-        tp.llBase = ep << 6;
-    }
-    const bool bitsOn = anyValidBits;                 // shared-memory words for the bitmask of a level: only when a job carries one (object models)
-    static int cacheOn = -1;        // MFB200_TRACK_CACHE=0: every iteration re-reads its pose-independent inputs from global memory (A/B)
-    if (cacheOn < 0) { const char* e = getenv("MFB200_TRACK_CACHE"); cacheOn = e ? (e[0] != '0') : MFB200_DEFAULT_TRACK_CACHE; }
+    unsigned ep = ++llEpoch[dev];
+    if ((ep << 6) == 0u) ep = ++llEpoch[dev];           // flag 0 means "never written"
+    tp.llBase = ep << 6;
     int G = numSMs / nJobs;                      // one CTA per SM, the SMs split between the tracked models
     if (G * nJobs > coResident) G = coResident / nJobs;
     if (G > TRACK_MAX_BLOCKS / 2) G = TRACK_MAX_BLOCKS / 2;
     if (G < 1) throw CudaError{"too many tracked models for one cooperative launch"};
     // Per-model shares of the persistent grid.  A full-frame model (the background) pays the whole pixel phase for every live pixel; an
     // object model rejects nearly every pixel on its bitmask and is bound by the reduction / solve chain instead: with equal shares the
-    // background of the 8-object scene walked 37 pixels per thread while the objects' CTAs idled at their barriers.  Light models get a
+    // background of the 8-object scene walked 37 pixels per thread while the objects' CTAs idled at their exchanges.  Light models get a
     // small fixed share, the heavy ones split the rest.  (Sums are fp64 of exact products: the result does not depend on the shares.)
-    static int sharesOn = -1;       // MFB200_TRACK_SHARES=0: equal shares (A/B)
-    if (sharesOn < 0) { const char* e = getenv("MFB200_TRACK_SHARES"); sharesOn = e ? (e[0] != '0') : 1; }
     int Gof[TRACK_MAX_JOBS];
-    static int ratio = -1;          // MFB200_TRACK_HEAVY_RATIO (A/B)
-    if (ratio < 0) { const char* e = getenv("MFB200_TRACK_HEAVY_RATIO"); ratio = e ? std::max(1, atoi(e)) : 2; }
-    track_shares(nJobs, sharesOn ? lightMask : 0u, std::min(numSMs, coResident), ratio, Gof);
+    track_shares(nJobs, lightMask, std::min(numSMs, coResident), 2, Gof);
     int Gheavy = 0;                  // the largest share (sizes the shared-memory correspondences)
     for (int j = 0; j < nJobs; ++j) Gheavy = std::max(Gheavy, Gof[j]);
     tp.nJobs = nJobs; tp.jobStart[0] = 0;
     for (int j = 0; j < nJobs; ++j) tp.jobStart[j + 1] = (unsigned short)(tp.jobStart[j] + Gof[j]);
     const int gridCTAs = tp.jobStart[nJobs];
-    int launches = 0;
-    const TrackJob* jp = d_jobs;
-    // ---- SO(3) pre-alignment + level 2 on one thread-block cluster per model (hardware barrier + distributed shared memory) ----
-    bool clustered = false;
-    if (clusterOkDev[dev] && (tp.so3 || tp.iterations[2] > 0)) {
-        TrackParams t1 = tp; t1.phase = 1; t1.nJobs = 0;
-        const int N2 = (W >> 2) * (H >> 2);
-        for (int C = 16; C >= 8 && !clustered; C >>= 1) {
-            const int roundsC = (N2 + C * PT_THREADS - 1) / (C * PT_THREADS);
-            size_t dynC = (size_t)roundsC * PT_THREADS * sizeof(int2);
-            if (t1.rgb && dynC <= dynMaxClDev[dev]) t1.corrSlots = roundsC * PT_THREADS; else { t1.corrSlots = 0; dynC = 0; }
-            if (t1.rgb && t1.corrSlots == 0) break;             // the global scratch stripe is sized for the persistent grid only
-            dynC = (dynC + 15) & ~(size_t)15;
-            t1.bitWords = bitsOn ? (N2 + 31) / 32 : 0;
-            const size_t bitBytesC = ((size_t)t1.bitWords * 4 + 15) & ~(size_t)15;
-            if (dynC + bitBytesC > dynMaxClDev[dev]) { t1.bitWords = 0; }
-            t1.cacheRounds = cacheOn ? (int)std::min<size_t>((size_t)roundsC, (dynMaxClDev[dev] - dynC - (t1.bitWords ? bitBytesC : 0)) / ((size_t)PT_THREADS * CACHE_BYTES_PER_SLOT)) : 0;
-            dynC += (size_t)t1.cacheRounds * PT_THREADS * CACHE_BYTES_PER_SLOT + (t1.bitWords ? bitBytesC : 0);
-            cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-            cfg.gridDim = dim3(C, nJobs); cfg.blockDim = dim3(PT_THREADS); cfg.dynamicSmemBytes = dynC; cfg.stream = s;
-            cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            int maxClusters = 0;
-            if (cudaOccupancyMaxActiveClusters(&maxClusters, k_track_cluster, &cfg) != cudaSuccess || maxClusters < 1) { cudaGetLastError(); continue; }
-            if (maxClusters < nJobs && C > 8) continue;        // all models' clusters should be co-resident: try the smaller cluster
-            prof_mark(s, "k_track_cluster");
-            cudaError_t e = cudaLaunchKernelEx(&cfg, k_track_cluster, jp, t1);
-            if (e != cudaSuccess) { cudaGetLastError(); continue; }
-            clustered = true; ++launches;
-        }
-        if (!clustered) clusterOkDev[dev] = clusterOkDev[dev];  // keep trying on later frames: the failure may depend on nJobs
-    }
-    tp.phase = clustered ? 2 : 0;
     // photometric correspondences stay in shared memory when the per-CTA pixel share fits (8 B per pixel slot)
     // sized for the models with the largest share (the heavy ones); a CTA whose share needs more slots uses its model's global scratch stripe
     const int rounds0 = (W * H + Gheavy * PT_THREADS - 1) / (Gheavy * PT_THREADS);
     size_t dyn = (size_t)rounds0 * PT_THREADS * sizeof(int2);
     if (tp.rgb && dyn <= dynMaxDev[dev]) tp.corrSlots = rounds0 * PT_THREADS; else { tp.corrSlots = 0; dyn = 0; }
     dyn = (dyn + 15) & ~(size_t)15;
-    tp.bitWords = bitsOn ? (W * H + 31) / 32 : 0;
+    // shared-memory words for the bitmask of a level: only when a job carries one (object models) and it fits behind the correspondences
+    tp.bitWords = anyValidBits ? (W * H + 31) / 32 : 0;
     const size_t bitBytes = ((size_t)tp.bitWords * 4 + 15) & ~(size_t)15;
     if (dyn + bitBytes > dynMaxDev[dev]) tp.bitWords = 0;
+    static int cacheOn = -1;        // MFB200_TRACK_CACHE=0: every iteration re-reads its pose-independent inputs from global memory (A/B)
+    if (cacheOn < 0) { const char* e = getenv("MFB200_TRACK_CACHE"); cacheOn = e ? (e[0] != '0') : MFB200_DEFAULT_TRACK_CACHE; }
     tp.cacheRounds = cacheOn ? (int)std::min<size_t>((size_t)rounds0, (dynMaxDev[dev] - dyn - (tp.bitWords ? bitBytes : 0)) / ((size_t)PT_THREADS * CACHE_BYTES_PER_SLOT)) : 0;
     dyn += (size_t)tp.cacheRounds * PT_THREADS * CACHE_BYTES_PER_SLOT + (tp.bitWords ? bitBytes : 0);
-    cudaCheck(cudaMemsetAsync(bars, 0, TRACK_MAX_JOBS * 32 * sizeof(unsigned), s), "barrier reset");
     prof_mark(s, "k_track_persistent");
+    const TrackJob* jp = d_jobs;
     void* args[] = {(void*)&jp, (void*)&tp};
-    cudaCheck(cudaLaunchCooperativeKernel(llOn ? (const void*)k_track_persistent : (const void*)k_track_persistent_bar, dim3(gridCTAs), dim3(PT_THREADS), args, dyn, s), "cooperative launch (tracking)");
-    return launches + 1;
+    cudaCheck(cudaLaunchCooperativeKernel((const void*)k_track_persistent, dim3(gridCTAs), dim3(PT_THREADS), args, dyn, s), "cooperative launch (tracking)");
+    return 1;
 }
 
 // (tag, clock64) pairs of the last tracking launch (A/B build -DMF_TRACK_TIMING only); returns the number of int64 values written
