@@ -195,6 +195,33 @@ int mf_backbone_download(mf_backbone* h, int level, void* host_bf16);
 double mf_backbone_flops(mf_backbone* h);
 int mf_backbone_num_gemms(mf_backbone* h);
 
+/* ---- Mask R-CNN region proposals on the backbone's P2..P6 (matterport mrcnn rpn_graph + ProposalLayer + PyramidROIAlign, COCO
+ *      InferenceConfig; weights synthetic/seeded and owned by the handle, not by the backbone's layer table).  The handle reads the
+ *      backbone's outputs and enqueues on the backbone's stream; destroy it before the backbone.  Errors: mf_cnn_last_error().
+ *      Anchors: 3 per feature pixel (ratios 0.5, 1, 2), order (level P2..P6, y, x, ratio), normalised y1 x1 y2 x2; A anchors in all.
+ *      Boxes are normalised y1 x1 y2 x2 float; pooled features are [n][pool][pool][256] bf16. ---- */
+typedef struct mf_rpn mf_rpn;
+#define MF_RPN_CONV 1          /* shared 3x3 256->512 conv + ReLU on P2..P6 (wgmma GEMM) */
+#define MF_RPN_HEADS 2         /* 1x1 class-logit and box-delta heads as one GEMM with fp32 output -> logits [A][2], deltas [A][4] */
+#define MF_RPN_PROPOSALS 4     /* top 6000 by score, decode + clip, NMS 0.7 -> 1000 proposals (zero padded) and the kept count */
+#define MF_RPN_ROI_ALIGN 8     /* 7x7 ROI Align of the 1000 proposals */
+mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed);
+void mf_rpn_destroy(mf_rpn* h);
+int mf_rpn_forward(mf_rpn* h);                        /* all four stages, after mf_backbone_forward on the same stream */
+int mf_rpn_run(mf_rpn* h, int stages);                /* a subset of the stages (MF_RPN_* bits), in order */
+int mf_rpn_num_anchors(mf_rpn* h);
+/* the proposal stage of the forward on caller-supplied device arrays: logits [n][2], deltas [n][4], anchors [n][4] float, 1 <= n <= A */
+int mf_rpn_propose(mf_rpn* h, const float* d_logits, const float* d_deltas, const float* d_anchors, int n_anchors);
+/* pyramid ROI Align of n boxes (device, [n][4]) on bb's P2..P5 into d_out ([n][pool][pool][256] bf16, device), 2 <= pool <= 64; bb's stream */
+int mf_roi_align_bf16(mf_backbone* bb, const float* d_boxes, int n, int pool, void* d_out);
+/* read-back to host memory (each waits for the handle's stream); NULL skips an output */
+int mf_rpn_get_weights(mf_rpn* h, float* conv_w_512x2304, float* conv_b_512, float* head_w_18x512, float* head_b_18);   /* (ky,kx,cin) order; head rows 0..5 logits, 6..17 deltas */
+int mf_rpn_get_anchors(mf_rpn* h, float* anchors_Ax4);
+int mf_rpn_get_head_outputs(mf_rpn* h, float* logits_Ax2, float* deltas_Ax4);
+int mf_rpn_download_conv(mf_rpn* h, int level, void* host_bf16);                 /* level 0..4 = P2..P6: H x W x 512 bf16 */
+int mf_rpn_get_proposals(mf_rpn* h, float* rois_1000x4);                          /* returns the kept count */
+int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16_1000x7x7x256);
+
 /* ---- image-directory loader ("-dir", GUI/Tools/ImageLogReader.{h,cpp}; GUI/MainController.cpp:150-176) ----
  * colour .png/.ppm/.jpg, depth 16-bit .png (x 0.001), masks 8-bit .png/.pgm + "<mask>.txt" (class ids, boxes); .exr depth is refused
  * (no OpenEXR in this build).  hasMore() lets the last frame through (ImageLogReader.cpp:326), unlike the .klg reader. */

@@ -2,6 +2,8 @@
 pipeline behind the reference's MaskFusion::processFrame / Model::{performTracking,fuse,...}
 interface.  The product is the CUDA library (csrc/ -> libmaskfusion_b200.so, C ABI in
 include/maskfusion_b200.h); this package is the thin host-side mirror used by tests/bench."""
-from .api import (MaskFusion, Model, Config, KlgLogReader, ImageLogReader, MFError, default_config, load_library, write_klg, LIB_PATH, EXPORTS, Backbone)
+from .api import (MaskFusion, Model, Config, KlgLogReader, ImageLogReader, MFError, default_config, load_library, write_klg, LIB_PATH, EXPORTS, Backbone,
+                  RegionProposals, roi_align)
 
-__all__ = ["MaskFusion", "Model", "Config", "KlgLogReader", "ImageLogReader", "MFError", "default_config", "load_library", "write_klg", "LIB_PATH", "EXPORTS", "Backbone"]
+__all__ = ["MaskFusion", "Model", "Config", "KlgLogReader", "ImageLogReader", "MFError", "default_config", "load_library", "write_klg", "LIB_PATH", "EXPORTS", "Backbone",
+           "RegionProposals", "roi_align"]

@@ -53,6 +53,8 @@ EXPORTS = [
     "mf_dir_get_next", "mf_dir_close", "mf_decode_jpeg", "mf_decode_exr_depth", "mf_export_poses", "mf_generate_id_image", "mf_pre_segmentation", "mf_write_ply", "mf_cnn_last_error", "mf_gemm_bf16", "mf_conv3x3_bf16", "mf_backbone_create", "mf_backbone_destroy", "mf_backbone_num_layers",
     "mf_backbone_layer", "mf_backbone_get_weights", "mf_backbone_mold", "mf_backbone_input_buffer", "mf_backbone_forward", "mf_backbone_output",
     "mf_backbone_flops", "mf_backbone_num_gemms", "mf_backbone_download",
+    "mf_rpn_create", "mf_rpn_destroy", "mf_rpn_forward", "mf_rpn_run", "mf_rpn_num_anchors", "mf_rpn_propose", "mf_roi_align_bf16",
+    "mf_rpn_get_weights", "mf_rpn_get_anchors", "mf_rpn_get_head_outputs", "mf_rpn_download_conv", "mf_rpn_get_proposals", "mf_rpn_get_pooled",
     "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
     "mf_shard_projection_keys", "mf_shard_frame_end", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
 ]
@@ -147,6 +149,19 @@ def load_library():
     L.mf_backbone_flops.restype = C.c_double; L.mf_backbone_flops.argtypes = [C.c_void_p]
     L.mf_backbone_num_gemms.argtypes = [C.c_void_p]
     L.mf_backbone_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.mf_rpn_create.restype = C.c_void_p; L.mf_rpn_create.argtypes = [C.c_void_p, C.c_uint]
+    L.mf_rpn_destroy.restype = None; L.mf_rpn_destroy.argtypes = [C.c_void_p]
+    L.mf_rpn_forward.argtypes = [C.c_void_p]
+    L.mf_rpn_run.argtypes = [C.c_void_p, C.c_int]
+    L.mf_rpn_num_anchors.argtypes = [C.c_void_p]
+    L.mf_rpn_propose.argtypes = [C.c_void_p] * 4 + [C.c_int]
+    L.mf_roi_align_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    L.mf_rpn_get_weights.argtypes = [C.c_void_p] * 5
+    L.mf_rpn_get_anchors.argtypes = [C.c_void_p, C.c_void_p]
+    L.mf_rpn_get_head_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.mf_rpn_download_conv.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.mf_rpn_get_proposals.argtypes = [C.c_void_p, C.c_void_p]
+    L.mf_rpn_get_pooled.argtypes = [C.c_void_p, C.c_void_p]
     L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.mf_shard_frame_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
     L.mf_shard_unique_id.argtypes = [C.c_void_p]
@@ -634,3 +649,90 @@ class Backbone:
 
     def numGemms(self):
         return int(self.L.mf_backbone_num_gemms(self.h))
+
+
+def _bf16_to_f32(raw: np.ndarray) -> np.ndarray:
+    return (raw.astype(np.uint32) << 16).view(np.float32)
+
+
+class RegionProposals:
+    """Mask R-CNN RPN head + proposal layer + pyramid ROI Align on a Backbone's P2..P6 (csrc/mf_rpn.cu).  Weights are synthetic (seeded).
+    Runs on the backbone's stream; close it before the backbone."""
+
+    POST_NMS, POOL, CHANNELS = 1000, 7, 256
+    CONV, HEADS, PROPOSALS, ROI_ALIGN = 1, 2, 4, 8        # stage bits of run()
+
+    def __init__(self, backbone: Backbone, seed=1):
+        self.L = load_library()
+        self.backbone = backbone
+        self.S = backbone.S
+        self.h = self.L.mf_rpn_create(C.c_void_p(backbone.h), seed)
+        if not self.h:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+        self.A = int(self.L.mf_rpn_num_anchors(self.h))
+
+    def _ck(self, r):
+        if r < 0:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+        return r
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.mf_rpn_destroy(self.h); self.h = None
+
+    def forward(self):
+        """conv, heads, proposals and ROI Align of the backbone's last forward"""
+        self._ck(self.L.mf_rpn_forward(self.h))
+
+    def run(self, stages: int):
+        self._ck(self.L.mf_rpn_run(self.h, int(stages)))
+
+    def anchors(self) -> np.ndarray:
+        out = np.zeros((self.A, 4), np.float32)
+        self._ck(self.L.mf_rpn_get_anchors(self.h, _p(out)))
+        return out
+
+    def headOutputs(self):
+        """fp32 (logits [A, 2], deltas [A, 4])"""
+        lg = np.zeros((self.A, 2), np.float32); dl = np.zeros((self.A, 4), np.float32)
+        self._ck(self.L.mf_rpn_get_head_outputs(self.h, _p(lg), _p(dl)))
+        return lg, dl
+
+    def convOutput(self, level: int) -> np.ndarray:
+        """shared 3x3 conv output of P(level+2), level 0..4, as float32 (H, W, 512)"""
+        n = self.S >> (level + 2)
+        raw = np.zeros((n, n, 512), np.uint16)
+        self._ck(self.L.mf_rpn_download_conv(self.h, int(level), _p(raw)))
+        return _bf16_to_f32(raw)
+
+    def proposals(self):
+        """-> (kept count, rois [1000, 4] normalised y1 x1 y2 x2, zero rows past the count)"""
+        rois = np.zeros((self.POST_NMS, 4), np.float32)
+        n = self._ck(self.L.mf_rpn_get_proposals(self.h, _p(rois)))
+        return n, rois
+
+    def pooled(self, raw: bool = False) -> np.ndarray:
+        """ROI-aligned features [1000, 7, 7, 256]: bf16 bit patterns (uint16) if raw, else float32"""
+        out = np.zeros((self.POST_NMS, self.POOL, self.POOL, self.CHANNELS), np.uint16)
+        self._ck(self.L.mf_rpn_get_pooled(self.h, _p(out)))
+        return out if raw else _bf16_to_f32(out)
+
+    def weights(self):
+        """-> conv weights [512, 3, 3, 256], conv bias [512], head weights [18, 512] (rows 0..5 logits a*2+c, 6..17 deltas a*4+k),
+        head bias [18]; bf16-representable float32"""
+        cw = np.zeros((512, 3, 3, 256), np.float32); cb = np.zeros(512, np.float32)
+        hw = np.zeros((18, 512), np.float32); hb = np.zeros(18, np.float32)
+        self._ck(self.L.mf_rpn_get_weights(self.h, _p(cw), _p(cb), _p(hw), _p(hb)))
+        return cw, cb, hw, hb
+
+    def propose(self, logits_ptr: int, deltas_ptr: int, anchors_ptr: int, n: int):
+        """the proposal stage on caller-supplied device arrays (float32 [n, 2], [n, 4], [n, 4]); results through proposals()"""
+        self._ck(self.L.mf_rpn_propose(self.h, C.c_void_p(logits_ptr), C.c_void_p(deltas_ptr), C.c_void_p(anchors_ptr), int(n)))
+
+
+def roi_align(backbone: Backbone, boxes_ptr: int, n: int, pool: int, out_ptr: int):
+    """pyramid ROI Align of n normalised boxes (device float32 [n, 4]) on the backbone's P2..P5 into out (device bf16 [n, pool, pool, 256]),
+    enqueued on the backbone's stream"""
+    L = load_library()
+    if L.mf_roi_align_bf16(C.c_void_p(backbone.h), C.c_void_p(boxes_ptr) if n else None, int(n), int(pool), C.c_void_p(out_ptr) if n else None) != 0:
+        raise MFError(L.mf_cnn_last_error().decode())

@@ -40,6 +40,7 @@ SOURCES = {
     "mf_jpeg.cu": [],                     # host code only: baseline JPEG decode, libjpeg's default path restated
     "mf_loader.cu": [],                   # host code only: image-directory loader (PNG/PNM decode, zlib)
     "mf_cnn.cu": [],                      # tensor-core GEMMs: no bit-exactness contract, FMA contraction on
+    "mf_rpn.cu": ["-fmad=false"],         # proposal layer + ROI Align: bit-exact against the numpy restatement (the GEMMs live in mf_cnn.cu)
 }
 
 

@@ -28,6 +28,7 @@
 #include <string.h>
 #include <map>
 #include <array>
+#include <type_traits>
 
 namespace mfb {
 
@@ -104,10 +105,11 @@ constexpr int GEMM_BM = 128, GEMM_BK = 64, GEMM_STAGES = 4, GEMM_THREADS = 384; 
 // by (kx-1, ky-1) -- TMA zero-fills the out-of-image part, which IS the padding.  No im2col buffer.
 struct ConvGeom { int mode; int Wimg, Himg, Wbox, Hbox, cblocks; };
 
-template <int BN>
+// OutT = __nv_bfloat16 (every backbone layer) or float (the RPN's 1x1 heads, whose scores feed a top-k: no bf16 ties)
+template <int BN, typename OutT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_wgmma(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                                                                       const float* __restrict__ bias, const __nv_bfloat16* __restrict__ residual,
-                                                                      __nv_bfloat16* __restrict__ out, int M, int N, int K, int relu, ConvGeom geo)
+                                                                      OutT* __restrict__ out, int M, int N, int K, int relu, ConvGeom geo)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // carve: [stages x A tile 16 KB][stages x B tile BN*128 B][barriers]
@@ -174,7 +176,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_wgmma(const __gri
         const int rt = c * 64 + w * 16 + (lane >> 2) + 8 * h;
         const int row = geo.mode ? (py0 + rt / geo.Wbox) * geo.Wimg + px0 + rt % geo.Wbox : tile_m * GEMM_BM + rt;
         if (row >= M) continue;
-        __nv_bfloat16* optr = out + (size_t)row * N + tile_n * BN + 2 * (lane & 3);
+        OutT* optr = out + (size_t)row * N + tile_n * BN + 2 * (lane & 3);
         const __nv_bfloat16* rptr = residual ? residual + (size_t)row * N + tile_n * BN + 2 * (lane & 3) : nullptr;
         const float* bptr = bias + tile_n * BN + 2 * (lane & 3);
 #pragma unroll
@@ -183,7 +185,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_wgmma(const __gri
             float x0 = d[4 * j + 2 * h] + b2.x, x1 = d[4 * j + 2 * h + 1] + b2.y;
             if (rptr) { const __nv_bfloat162 r2 = *reinterpret_cast<const __nv_bfloat162*>(rptr + 8 * j); x0 += __low2float(r2); x1 += __high2float(r2); }
             if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-            *reinterpret_cast<__nv_bfloat162*>(optr + 8 * j) = __floats2bfloat162_rn(x0, x1);
+            if constexpr (std::is_same<OutT, float>::value) *reinterpret_cast<float2*>(optr + 8 * j) = make_float2(x0, x1);
+            else *reinterpret_cast<__nv_bfloat162*>(optr + 8 * j) = __floats2bfloat162_rn(x0, x1);
         }
     }
 }
@@ -355,12 +358,24 @@ template <int BN>
 static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 2 * GEMM_STAGES * 8 + 1024; }
 
 const char* cnn_last_error() { return g_cnn_err.c_str(); }
+void cnn_set_error(const char* msg) { g_cnn_err = msg; }
+
+template <int BN, typename OutT>
+static void launch_wgmma(dim3 grid, cudaStream_t s, const CUtensorMap& mA, const CUtensorMap& mB, const float* bias, const void* residual, void* out,
+                         int M, int N, int K, int relu, const ConvGeom& geo)
+{
+    static bool attr = false;
+    if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<BN>()); attr = true; }
+    k_gemm_bf16_wgmma<BN, OutT><<<grid, GEMM_THREADS, gemm_smem_bytes<BN>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (OutT*)out, M, N, K, relu, geo);
+}
 
 // D = relu?(A * B^T + bias + residual); all device pointers; K % 64 == 0, N % 64 == 0
 // conv3x3 != nullptr: A is an NHWC activation [Himg x Wimg x Cin] and the GEMM is the implicit 3x3/s1/p1 convolution (K = 9*Cin)
+// outF32: D is written as fp32 (residual must then be null), else as bf16
 int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
-                     const int* conv3x3 /* Wimg, Himg, Cin */ = nullptr)
+                     const int* conv3x3 /* Wimg, Himg, Cin */, bool outF32)
 {
+    if (outF32 && residual) { g_cnn_err = "gemm: the fp32 output takes no residual"; return -2; }
     if (!ensure_encode()) return -1;
     if (K % 64 || N % 64 || M <= 0) { g_cnn_err = "gemm: need K % 64 == 0 and N % 64 == 0"; return -2; }
     const int mtiles = (M + GEMM_BM - 1) / GEMM_BM;
@@ -376,15 +391,14 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
     } else if (!cached_map(&mA, A, (uint64_t)M, (uint64_t)K, GEMM_BM)) return -3;
     if (!cached_map(&mB, B, (uint64_t)N, (uint64_t)K, (uint32_t)BN)) return -3;
     dim3 grid(mtiles, N / BN);
-    prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128" : "k_gemm_bf16_wgmma_n64");
-    if (BN == 128) {
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<128>()); attr = true; }
-        k_gemm_bf16_wgmma<128><<<grid, GEMM_THREADS, gemm_smem_bytes<128>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
+    if (outF32) {
+        prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128_f32" : "k_gemm_bf16_wgmma_n64_f32");
+        if (BN == 128) launch_wgmma<128, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
+        else launch_wgmma<64, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
     } else {
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<64>()); attr = true; }
-        k_gemm_bf16_wgmma<64><<<grid, GEMM_THREADS, gemm_smem_bytes<64>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, M, N, K, relu, geo);
+        prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128" : "k_gemm_bf16_wgmma_n64");
+        if (BN == 128) launch_wgmma<128, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
+        else launch_wgmma<64, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { g_cnn_err = std::string("gemm launch: ") + cudaGetErrorString(e); return -4; }
@@ -427,40 +441,59 @@ static int add_conv(Backbone* b, int Cin, int Cout, int k, int stride, int pad, 
     return (int)b->layers.size() - 1;
 }
 
-// runs conv layer li on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]
+// geometry guard of the implicit 3x3 path: the 128-pixel TMA box must tile the image exactly
+bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win)
+{
+    const int wbox = Win >= 128 ? 128 : Win;
+    return k == 3 && stride == 1 && pad == 1 && (Cin % 64) == 0 && Win <= 128 * 1024 && (128 % wbox) == 0 && (Win % wbox) == 0 &&
+           (Hin % (128 / wbox)) == 0 && wbox >= 8;
+}
+
+// runs convolution L (weights W [Cout x Kpad], bias B) on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]; col: im2col scratch
+static int conv_layer(const ConvLayer& L, const __nv_bfloat16* W, const float* B, __nv_bfloat16* col, const __nv_bfloat16* in, int Hin, int Win,
+                      __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s, int* HoutP, int* WoutP)
+{
+    const int Hout = (Hin + 2 * L.pad - L.k) / L.stride + 1, Wout = (Win + 2 * L.pad - L.k) / L.stride + 1;
+    const int M = Hout * Wout;
+    const __nv_bfloat16* A = in;
+    if (HoutP) *HoutP = Hout;
+    if (WoutP) *WoutP = Wout;
+    if (cnn_conv_implicit(L.k, L.stride, L.pad, L.Cin, Hin, Win)) {
+        int g3[3] = {Win, Hin, L.Cin};
+        return launch_gemm_bf16(in, W, B, residual, out, M, L.Cout, L.Kpad, relu, s, g3);
+    }
+    if (!(L.k == 1 && L.stride == 1)) {
+        if (L.k == 1 && L.stride == 2 && (L.Cin % 8) == 0) {
+            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, col);
+        } else {
+            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, col);
+        }
+        A = col;
+    }
+    return launch_gemm_bf16(A, W, B, residual, out, M, L.Cout, L.Kpad, relu, s);
+}
+
+// runs backbone layer li on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]
 static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int Win, __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s,
                     int* HoutP = nullptr, int* WoutP = nullptr)
 {
     const ConvLayer& L = b->layers[li];
-    const int Hout = (Hin + 2 * L.pad - L.k) / L.stride + 1, Wout = (Win + 2 * L.pad - L.k) / L.stride + 1;
-    const int M = Hout * Wout;
-    const __nv_bfloat16* A = in;
-    const int wbox = Win >= 128 ? 128 : Win;
-    const bool implicit3 = L.k == 3 && L.stride == 1 && L.pad == 1 && (L.Cin % 64) == 0 && Win <= 128 * 1024 && (128 % wbox) == 0 && (Win % wbox) == 0 &&
-                           (Hin % (128 / wbox)) == 0 && wbox >= 8;
-    if (implicit3) {
-        int g3[3] = {Win, Hin, L.Cin};
-        int rc = launch_gemm_bf16(in, b->dW + L.wOff, b->dB + L.bOff, residual, out, M, L.Cout, L.Kpad, relu, s, g3);
-        b->flops += 2.0 * M * (double)L.Cout * (double)(9 * L.Cin);
-        b->gemms++;
-        if (HoutP) *HoutP = Hout;
-        if (WoutP) *WoutP = Wout;
-        return rc;
-    }
-    if (!(L.k == 1 && L.stride == 1)) {
-        if (L.k == 1 && L.stride == 2 && (L.Cin % 8) == 0) {
-            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, b->col);
-        } else {
-            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, b->col);
-        }
-        A = b->col;
-    }
-    int rc = launch_gemm_bf16(A, b->dW + L.wOff, b->dB + L.bOff, residual, out, M, L.Cout, L.Kpad, relu, s);
-    b->flops += 2.0 * M * (double)L.Cout * (double)(L.k * L.k * L.Cin);
+    int Hout, Wout;
+    const int rc = conv_layer(L, b->dW + L.wOff, b->dB + L.bOff, b->col, in, Hin, Win, out, residual, relu, s, &Hout, &Wout);
+    b->flops += 2.0 * Hout * Wout * (double)L.Cout * (double)(L.k * L.k * L.Cin);
     b->gemms++;
     if (HoutP) *HoutP = Hout;
     if (WoutP) *WoutP = Wout;
     return rc;
+}
+
+// a convolution whose weights are not in the backbone's table (the RPN's shared 3x3): the same path as the backbone's layers
+int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
+             cudaStream_t s)
+{
+    ConvLayer L; L.Cin = Cin; L.Cout = Cout; L.k = k; L.stride = stride; L.pad = pad; L.Kpad = (k * k * Cin + 63) / 64 * 64; L.wOff = L.bOff = 0;
+    return conv_layer(L, (const __nv_bfloat16*)W, B, (__nv_bfloat16*)col, (const __nv_bfloat16*)in, Hin, Win, (__nv_bfloat16*)out, nullptr, relu, s,
+                      nullptr, nullptr);
 }
 
 }  // namespace mfb

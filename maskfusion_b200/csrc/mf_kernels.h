@@ -141,6 +141,19 @@ int num_sms();
 // in-stream stage timer hook (mf_host.cu): records a CUDA event on `s`; the time until the next mark is attributed to `name`
 void prof_mark(cudaStream_t s, const char* name);
 
+// ---- mf_cnn.cu ----
+// D[M x N] = relu?(A[M x K] * B[N x K]^T + bias + residual), bf16 operands; conv3x3 = {Wimg, Himg, Cin}: A is an NHWC activation and the GEMM is
+// the implicit 3x3/s1/p1 convolution; outF32: D is fp32 (no residual), else bf16.  Returns 0 or < 0 with the text in cnn_last_error()
+int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
+                     const int* conv3x3 = nullptr, bool outF32 = false);
+// one convolution (NHWC bf16, weights [Cout][Kpad] in (ky, kx, cin) order) through the backbone's conv path: the implicit 3x3 GEMM where its
+// geometry guard admits the shape, else im2col into `col` (Hout*Wout*Kpad bf16) + GEMM
+int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
+             cudaStream_t s);
+bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win);     // does cnn_conv take the implicit path (no im2col)?
+const char* cnn_last_error();
+void cnn_set_error(const char* msg);
+
 // ---- mf_frame.cu ----
 void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, cudaStream_t s);
 void launch_bilateral(const float* depth, float* out, int W, int H, cudaStream_t s);
