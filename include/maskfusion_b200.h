@@ -222,6 +222,51 @@ int mf_rpn_download_conv(mf_rpn* h, int level, void* host_bf16);                
 int mf_rpn_get_proposals(mf_rpn* h, float* rois_1000x4);                          /* returns the kept count */
 int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16_1000x7x7x256);
 
+/* ---- Mask R-CNN detection heads on an mf_rpn's proposals (matterport mrcnn fpn_classifier_graph + DetectionLayer + build_fpn_mask_graph +
+ *      unmold_detections + generate_id_image, COCO InferenceConfig: 81 classes; weights synthetic/seeded and owned by the handle).  The handle
+ *      reads the RPN's proposals and pooled features and the backbone's P2..P5, and enqueues on the backbone's stream; destroy it before the
+ *      RPN.  Errors: mf_cnn_last_error().  Shapes are the upstream ones: 1000 ROIs, 100 detection rows.  Detections are [100][6] float
+ *      y1 x1 y2 x2 (normalised to the S x S network input, clipped to the letter-box window of the image) class score, zero rows after the
+ *      count; masks are [100][28][28] float (sigmoid of the detection's own class).  The image size (W x H, the letter-box window) is the one
+ *      given to the last mf_detector_forward / detect / paste; S x S after create. ---- */
+typedef struct mf_detector mf_detector;
+#define MF_DET_CLASSIFIER 1    /* FC1 (7x7 conv on the pooled ROIs), FC2, class logits + box deltas (one GEMM, fp32) */
+#define MF_DET_DETECTIONS 2    /* softmax, refinement, clip to the window, confidence 0.7, per-class NMS 0.3, top 100 -> detections + count */
+#define MF_DET_MASKS 4         /* 14x14 ROI Align of the detections, 4 x 3x3 conv, 2x2/s2 transposed conv, 1x1 logits, own-class sigmoid */
+#define MF_DET_ID_IMAGE 8      /* unmould to image pixels + generate_id_image (export rule of mf_detector_set_export) -> id image, ids, rois */
+mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed);
+void mf_detector_destroy(mf_detector* h);
+int mf_detector_run(mf_detector* h, int stages);                  /* a subset of the stages (MF_DET_* bits), in order */
+int mf_detector_forward(mf_detector* h, int image_w, int image_h); /* all stages after mf_rpn_forward, for an image of image_w x image_h */
+/* what MaskRCNN.execute() does: mould the W x H RGBA8 device image, backbone, RPN and all head stages, enqueued on one stream */
+int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int H);
+/* generate_id_image's min_score, class_filter and special_assignments (mf_generate_id_image's conventions, <= 128 entries each; NULL with
+ * count 0 for none).  Default: 0.55 and no lists. */
+int mf_detector_set_export(mf_detector* h, double min_score, const int32_t* class_filter, int n_filter, const int32_t* special_assignments,
+                           int n_special);
+/* the detection layer on caller-supplied device arrays: rois [n][4], logits [n][81], deltas [n][81][4] float, 1 <= n <= 1000; the window
+ * of the current image size */
+int mf_detector_refine(mf_detector* h, const float* d_rois, const float* d_logits, const float* d_deltas, int n);
+/* unmould + id image on caller-supplied device arrays: detections [100][6], masks [100][28][28] float, for a W x H image */
+int mf_detector_paste(mf_detector* h, const float* d_detections, const float* d_masks, int W, int H);
+/* read-back to host memory (each waits for the handle's stream); NULL skips an output */
+int mf_detector_num_layers(mf_detector* h);
+/* layer i: Cin, rows (GEMM N, zero rows included), k, stride, pad, K.  0 FC1, 1 FC2, 2 heads (rows 0..80 logits, 81 + 4c + k deltas of class
+ * c), 3..6 mask convs, 7 transposed conv (row (dy*2 + dx)*256 + cout), 8 mask logits */
+int mf_detector_layer(mf_detector* h, int i, int* cin_rows_k_stride_pad_K);
+int mf_detector_get_weights(mf_detector* h, int i, float* w_rows_K, float* bias_rows);   /* (ky,kx,cin) order along K */
+int mf_detector_get_fc(mf_detector* h, void* fc1_bf16_1000x1024, void* fc2_bf16_1000x1024);
+int mf_detector_get_head_outputs(mf_detector* h, float* logits_1000x81, float* deltas_1000x81x4);
+/* mask head layer i: 0 pooled 100x14x14x256, 1..4 conv outputs 100x14x14x256, 5 transposed conv 100x14x14x2x2x256 (bf16); 6 mask logits
+ * 100x14x14x2x2x81 (float) */
+int mf_detector_get_mask_layer(mf_detector* h, int i, void* host);
+int mf_detector_get_detections(mf_detector* h, float* detections_100x6);            /* returns the detection count */
+int mf_detector_get_masks(mf_detector* h, float* masks_100x28x28);
+/* the execute() outputs in mf_generate_id_image's layout: id image H x W uint8, exported class ids, rois y1 x1 y2 x2 int32 (each sized for
+ * 100); returns the exported count */
+int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32_t* class_ids, int32_t* rois);
+int mf_detector_image_size(mf_detector* h, int* w, int* hgt);
+
 /* ---- image-directory loader ("-dir", GUI/Tools/ImageLogReader.{h,cpp}; GUI/MainController.cpp:150-176) ----
  * colour .png/.ppm/.jpg, depth 16-bit .png (x 0.001), masks 8-bit .png/.pgm + "<mask>.txt" (class ids, boxes); .exr depth is refused
  * (no OpenEXR in this build).  hasMore() lets the last frame through (ImageLogReader.cpp:326), unlike the .klg reader. */

@@ -55,6 +55,10 @@ EXPORTS = [
     "mf_backbone_flops", "mf_backbone_num_gemms", "mf_backbone_download",
     "mf_rpn_create", "mf_rpn_destroy", "mf_rpn_forward", "mf_rpn_run", "mf_rpn_num_anchors", "mf_rpn_propose", "mf_roi_align_bf16",
     "mf_rpn_get_weights", "mf_rpn_get_anchors", "mf_rpn_get_head_outputs", "mf_rpn_download_conv", "mf_rpn_get_proposals", "mf_rpn_get_pooled",
+    "mf_detector_create", "mf_detector_destroy", "mf_detector_run", "mf_detector_forward", "mf_detector_detect", "mf_detector_set_export",
+    "mf_detector_refine", "mf_detector_paste", "mf_detector_num_layers", "mf_detector_layer", "mf_detector_get_weights", "mf_detector_get_fc",
+    "mf_detector_get_head_outputs", "mf_detector_get_mask_layer", "mf_detector_get_detections", "mf_detector_get_masks", "mf_detector_get_id_image",
+    "mf_detector_image_size",
     "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
     "mf_shard_projection_keys", "mf_shard_frame_end", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
 ]
@@ -162,6 +166,24 @@ def load_library():
     L.mf_rpn_download_conv.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.mf_rpn_get_proposals.argtypes = [C.c_void_p, C.c_void_p]
     L.mf_rpn_get_pooled.argtypes = [C.c_void_p, C.c_void_p]
+    L.mf_detector_create.restype = C.c_void_p; L.mf_detector_create.argtypes = [C.c_void_p, C.c_uint]
+    L.mf_detector_destroy.restype = None; L.mf_detector_destroy.argtypes = [C.c_void_p]
+    L.mf_detector_run.argtypes = [C.c_void_p, C.c_int]
+    L.mf_detector_forward.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    L.mf_detector_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    L.mf_detector_set_export.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    L.mf_detector_refine.argtypes = [C.c_void_p] * 4 + [C.c_int]
+    L.mf_detector_paste.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_int]
+    L.mf_detector_num_layers.argtypes = [C.c_void_p]
+    L.mf_detector_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.mf_detector_get_weights.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    L.mf_detector_get_fc.argtypes = [C.c_void_p] * 3
+    L.mf_detector_get_head_outputs.argtypes = [C.c_void_p] * 3
+    L.mf_detector_get_mask_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.mf_detector_get_detections.argtypes = [C.c_void_p, C.c_void_p]
+    L.mf_detector_get_masks.argtypes = [C.c_void_p, C.c_void_p]
+    L.mf_detector_get_id_image.argtypes = [C.c_void_p] * 4
+    L.mf_detector_image_size.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.mf_shard_frame_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
     L.mf_shard_unique_id.argtypes = [C.c_void_p]
@@ -736,3 +758,125 @@ def roi_align(backbone: Backbone, boxes_ptr: int, n: int, pool: int, out_ptr: in
     L = load_library()
     if L.mf_roi_align_bf16(C.c_void_p(backbone.h), C.c_void_p(boxes_ptr) if n else None, int(n), int(pool), C.c_void_p(out_ptr) if n else None) != 0:
         raise MFError(L.mf_cnn_last_error().decode())
+
+
+class Detector:
+    """Mask R-CNN detection heads on a RegionProposals' proposals (csrc/mf_heads.cu): classifier, detection layer, mask head, unmould and
+    generate_id_image.  Weights are synthetic (seeded).  Runs on the backbone's stream; close it before the RegionProposals."""
+
+    ROIS, MAX_DETECTIONS, NUM_CLASSES, MASK = 1000, 100, 81, 28
+    CLASSIFIER, DETECTIONS, MASKS, ID_IMAGE = 1, 2, 4, 8        # stage bits of run()
+
+    def __init__(self, rpn: RegionProposals, seed=1):
+        self.L = load_library()
+        self.rpn = rpn
+        self.h = self.L.mf_detector_create(C.c_void_p(rpn.h), seed)
+        if not self.h:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+
+    def _ck(self, r):
+        if r < 0:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+        return r
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.mf_detector_destroy(self.h); self.h = None
+
+    def run(self, stages: int):
+        self._ck(self.L.mf_detector_run(self.h, int(stages)))
+
+    def forward(self, image_w: int, image_h: int):
+        """every head stage on the RPN's last forward, for an original image of image_w x image_h"""
+        self._ck(self.L.mf_detector_forward(self.h, int(image_w), int(image_h)))
+
+    def detect(self, rgba_ptr: int, W: int, H: int):
+        """mould + backbone + RPN + heads of a W x H RGBA8 device image, enqueued on the backbone's stream"""
+        self._ck(self.L.mf_detector_detect(self.h, C.c_void_p(rgba_ptr), int(W), int(H)))
+
+    def set_export(self, min_score=0.55, class_filter=(), special_assignments=()):
+        """generate_id_image's arguments for the id-image stage"""
+        cf = np.ascontiguousarray(list(class_filter), np.int32); sa = np.ascontiguousarray(list(special_assignments), np.int32)
+        self._ck(self.L.mf_detector_set_export(self.h, float(min_score), _p(cf) if cf.size else None, int(cf.size), _p(sa) if sa.size else None,
+                                               int(sa.size)))
+
+    def refine(self, rois_ptr: int, logits_ptr: int, deltas_ptr: int, n: int):
+        """the detection layer on device arrays (float32 [n, 4], [n, 81], [n, 81, 4]); results through detections()"""
+        self._ck(self.L.mf_detector_refine(self.h, C.c_void_p(rois_ptr), C.c_void_p(logits_ptr), C.c_void_p(deltas_ptr), int(n)))
+
+    def paste(self, detections_ptr: int, masks_ptr: int, W: int, H: int):
+        """unmould + id image of device arrays (float32 [100, 6], [100, 28, 28]) for a W x H image; results through idImage()"""
+        self._ck(self.L.mf_detector_paste(self.h, C.c_void_p(detections_ptr), C.c_void_p(masks_ptr), int(W), int(H)))
+
+    def layers(self):
+        """(Cin, rows, k, stride, pad, K) per layer: FC1, FC2, heads, 4 mask convs, transposed conv, mask logits"""
+        out = []
+        for i in range(self.L.mf_detector_num_layers(self.h)):
+            d = np.zeros(6, np.int32)
+            self._ck(self.L.mf_detector_layer(self.h, i, _p(d)))
+            out.append(tuple(int(v) for v in d))
+        return out
+
+    def weights(self, i: int):
+        """-> weights [rows, K] ((ky, kx, cin) order along K), bias [rows]; bf16-representable float32"""
+        _, rows, _, _, _, K = self.layers()[i]
+        w = np.zeros((rows, K), np.float32); b = np.zeros(rows, np.float32)
+        self._ck(self.L.mf_detector_get_weights(self.h, int(i), _p(w), _p(b)))
+        return w, b
+
+    def fcOutputs(self):
+        """FC1 and FC2 outputs [1000, 1024] as float32 (bf16 values)"""
+        a = np.zeros((self.ROIS, 1024), np.uint16); b = np.zeros((self.ROIS, 1024), np.uint16)
+        self._ck(self.L.mf_detector_get_fc(self.h, _p(a), _p(b)))
+        return _bf16_to_f32(a), _bf16_to_f32(b)
+
+    def headOutputs(self):
+        """fp32 (logits [1000, 81], deltas [1000, 81, 4])"""
+        lg = np.zeros((self.ROIS, self.NUM_CLASSES), np.float32); dl = np.zeros((self.ROIS, self.NUM_CLASSES, 4), np.float32)
+        self._ck(self.L.mf_detector_get_head_outputs(self.h, _p(lg), _p(dl)))
+        return lg, dl
+
+    def maskLayer(self, i: int) -> np.ndarray:
+        """0 pooled [100, 14, 14, 256], 1..4 conv outputs [100, 14, 14, 256], 5 transposed conv [100, 14, 14, 2, 2, 256] (bf16 values as
+        float32); 6 mask logits [100, 14, 14, 2, 2, 81] float32"""
+        if i == 6:
+            out = np.zeros((self.MAX_DETECTIONS, 14, 14, 2, 2, self.NUM_CLASSES), np.float32)
+            self._ck(self.L.mf_detector_get_mask_layer(self.h, 6, _p(out)))
+            return out
+        raw = np.zeros((self.MAX_DETECTIONS, 14, 14, 2, 2, 256) if i == 5 else (self.MAX_DETECTIONS, 14, 14, 256), np.uint16)
+        self._ck(self.L.mf_detector_get_mask_layer(self.h, int(i), _p(raw)))
+        return _bf16_to_f32(raw)
+
+    def detections(self):
+        """-> (count, detections [100, 6] y1 x1 y2 x2 class score, zero rows past the count)"""
+        d = np.zeros((self.MAX_DETECTIONS, 6), np.float32)
+        n = self._ck(self.L.mf_detector_get_detections(self.h, _p(d)))
+        return n, d
+
+    def masks(self) -> np.ndarray:
+        m = np.zeros((self.MAX_DETECTIONS, self.MASK, self.MASK), np.float32)
+        self._ck(self.L.mf_detector_get_masks(self.h, _p(m)))
+        return m
+
+    def idImage(self):
+        """-> (id_image H x W uint8, class ids, rois), the types of generate_id_image"""
+        w, hh = C.c_int(0), C.c_int(0)
+        self._ck(self.L.mf_detector_image_size(self.h, C.byref(w), C.byref(hh)))
+        img = np.zeros((hh.value, w.value), np.uint8); ec = np.zeros(self.MAX_DETECTIONS, np.int32)
+        er = np.zeros((self.MAX_DETECTIONS, 4), np.int32)
+        n = self._ck(self.L.mf_detector_get_id_image(self.h, _p(img), _p(ec), _p(er)))
+        return img, ec[:n].tolist(), er[:n].tolist()
+
+    def execute(self, rgb: np.ndarray):
+        """MaskRCNN.execute(): H x W x 3 uint8 RGB -> (id_image H x W uint8, class ids, rois), as generate_id_image returns them"""
+        import torch
+        a = np.ascontiguousarray(rgb, np.uint8)
+        if a.ndim != 3 or a.shape[2] != 3:
+            raise MFError("rgb must be HxWx3 uint8")
+        H, W = a.shape[:2]
+        rgba = torch.from_numpy(np.concatenate([a, np.full((H, W, 1), 255, np.uint8)], axis=2)).cuda()
+        torch.cuda.current_stream().synchronize()          # the upload is complete before the detector's stream reads it
+        self.detect(rgba.data_ptr(), W, H)
+        out = self.idImage()                      # waits for the stream, so the upload outlives its use
+        del rgba
+        return out

@@ -41,6 +41,7 @@ SOURCES = {
     "mf_loader.cu": [],                   # host code only: image-directory loader (PNG/PNM decode, zlib)
     "mf_cnn.cu": [],                      # tensor-core GEMMs: no bit-exactness contract, FMA contraction on
     "mf_rpn.cu": ["-fmad=false"],         # proposal layer + ROI Align: bit-exact against the numpy restatement (the GEMMs live in mf_cnn.cu)
+    "mf_heads.cu": ["-fmad=false"],       # detection layer, mask select, unmould + id image: bit-exact against the numpy restatement
 }
 
 

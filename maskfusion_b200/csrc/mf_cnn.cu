@@ -195,15 +195,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_bf16_wgmma(const __gri
 // data-movement kernels around the GEMMs (NHWC bf16)
 // ------------------------------------------------------------------------------------------
 // im2col: A[m][(ky*kw + kx)*Cin + c], K padded with zeros to Kpad; 8 channels (16 B) per thread when Cin % 8 == 0
-__global__ void k_im2col(const __nv_bfloat16* __restrict__ in, int Hin, int Win, int Cin, int Hout, int Wout, int kh, int kw, int stride,
+// nimg images stacked (the mask head's ROIs): row m = (img, oy, ox), each image padded on its own
+__global__ void k_im2col(const __nv_bfloat16* __restrict__ in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int kh, int kw, int stride,
                          int pad, int Kpad, __nv_bfloat16* __restrict__ A)
 {
     const int K = kh * kw * Cin;
-    const size_t total8 = (size_t)Hout * Wout * (Kpad / 8);
+    const size_t total8 = (size_t)nimg * Hout * Wout * (Kpad / 8);
     for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total8; t += (size_t)gridDim.x * blockDim.x) {
         const int k8 = (int)(t % (Kpad / 8));
         const size_t m = t / (Kpad / 8);
-        const int ox = (int)(m % Wout), oy = (int)(m / Wout);
+        const int ox = (int)(m % Wout), oy = (int)((m / Wout) % Hout);
+        const __nv_bfloat16* img = in + (m / ((size_t)Wout * Hout)) * Hin * Win * Cin;
         uint4 v = make_uint4(0, 0, 0, 0);
         const int k0 = k8 * 8;
         if ((Cin & 7) == 0) {
@@ -211,7 +213,7 @@ __global__ void k_im2col(const __nv_bfloat16* __restrict__ in, int Hin, int Win,
                 const int tap = k0 / Cin, c = k0 - tap * Cin;
                 const int ky = tap / kw, kx = tap - ky * kw;
                 const int iy = oy * stride - pad + ky, ix = ox * stride - pad + kx;
-                if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) v = *reinterpret_cast<const uint4*>(in + ((size_t)iy * Win + ix) * Cin + c);
+                if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) v = *reinterpret_cast<const uint4*>(img + ((size_t)iy * Win + ix) * Cin + c);
             }
         } else {
             __nv_bfloat16* e = reinterpret_cast<__nv_bfloat16*>(&v);
@@ -221,7 +223,7 @@ __global__ void k_im2col(const __nv_bfloat16* __restrict__ in, int Hin, int Win,
                     const int tap = k / Cin, c = k - tap * Cin;
                     const int ky = tap / kw, kx = tap - ky * kw;
                     const int iy = oy * stride - pad + ky, ix = ox * stride - pad + kx;
-                    if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) e[j] = in[((size_t)iy * Win + ix) * Cin + c];
+                    if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) e[j] = img[((size_t)iy * Win + ix) * Cin + c];
                 }
             }
         }
@@ -466,7 +468,7 @@ static int conv_layer(const ConvLayer& L, const __nv_bfloat16* W, const float* B
         if (L.k == 1 && L.stride == 2 && (L.Cin % 8) == 0) {
             prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, col);
         } else {
-            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, col);
+            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, col);
         }
         A = col;
     }
@@ -485,6 +487,22 @@ static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int W
     if (HoutP) *HoutP = Hout;
     if (WoutP) *WoutP = Wout;
     return rc;
+}
+
+void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int k, int stride, int pad, int Kpad, void* col, cudaStream_t s)
+{
+    prof_mark(s, "k_im2col");
+    k_im2col<<<8 * num_sms(), 256, 0, s>>>((const __nv_bfloat16*)in, nimg, Hin, Win, Cin, Hout, Wout, k, k, stride, pad, Kpad, (__nv_bfloat16*)col);
+}
+
+// mould_image's letter box as mf_backbone_mold applies it (the detection heads map boxes back through the same geometry)
+MoldGeom cnn_mold_geometry(int S, int W, int H)
+{
+    MoldGeom g;
+    g.scale = fminf((float)S / (float)W, (float)S / (float)H);
+    g.newW = (int)lroundf(W * g.scale); g.newH = (int)lroundf(H * g.scale);
+    g.offx = (S - g.newW) / 2; g.offy = (S - g.newH) / 2;
+    return g;
 }
 
 // a convolution whose weights are not in the backbone's table (the RPN's shared 3x3): the same path as the backbone's layers
@@ -678,10 +696,8 @@ extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H
 {
     if (!h) return -1;
     Backbone* b = &h->b; const int S = b->S;
-    float scale = fminf((float)S / (float)W, (float)S / (float)H);
-    int newW = (int)lroundf(W * scale), newH = (int)lroundf(H * scale);
-    int offx = (S - newW) / 2, offy = (S - newH) / 2;
+    const MoldGeom g = cnn_mold_geometry(S, W, H);
     prof_mark(h->stream, "k_mold_input");
-    k_mold_input<<<8 * num_sms(), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, scale, offx, offy, newW, newH, b->input);
+    k_mold_input<<<8 * num_sms(), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, g.scale, g.offx, g.offy, g.newW, g.newH, b->input);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }

@@ -1,0 +1,519 @@
+// mf_heads.cu -- Mask R-CNN detection heads on the RPN's proposals (sm_90a): classifier, detection layer, mask head, unmould + id image.
+//
+// matterport mrcnn's inference graph with the COCO InferenceConfig (NUM_CLASSES 81), written from upstream memory (the source is not
+// vendored; DESIGN §3c, rules R-SOFTMAX / R-DETNMS / R-UNMOLD / R-RESIZE / R-SIGMOID in §4):
+//   fpn_classifier_graph   7x7 valid conv 256->1024 + ReLU ("FC1": one GEMM on the RPN's pooled [1000][7][7][256] in place, K = 12 544),
+//                          1x1 conv 1024->1024 + ReLU ("FC2"), class logits (81) + box deltas (81 x 4) as ONE GEMM: 405 rows zero-padded
+//                          to 448, fp32 epilogue.  BatchNorm is in inference mode and folded into the seeded weights, as in the backbone.
+//   DetectionLayer         softmax, argmax class, class-specific deltas x BBOX_STD_DEV, apply_box_deltas_graph, clip to the letter-box
+//                          window, keep class > 0 and score >= 0.7, per-class greedy NMS at IoU 0.3 (<= 100 per class), top 100 by score
+//                          -> [100][6] y1 x1 y2 x2 class score, zero padded, and the count (on the device)
+//   build_fpn_mask_graph   ROI Align at 14 on the 100 detection rows, 4 x (3x3 conv 256->256 + ReLU) as im2col + GEMM (the implicit 3x3
+//                          path refuses 14-wide images), 2x2/s2 transposed conv as a GEMM with N = 4 x 256 (rows [roi][y][x][dy][dx][c]),
+//                          1x1 conv 256->81 (padded to 128, fp32) on those rows in place, then each detection's own class + sigmoid
+//                          -> [100][28][28] fp32
+//   unmold_detections +    k_unmold (one thread) maps the detections to integer boxes of the original image and applies
+//   generate_id_image      generate_id_image's export rule; k_paste (one thread per pixel) walks the exported detections from last to first
+//                          and writes the first whose resized mask is >= 0.5 there -- no H x W x N mask stack
+// Every stage is enqueued on the backbone's stream and runs on the fixed upstream shapes (1000 ROIs, 100 detection rows); nothing waits
+// for the host.  Everything after the GEMMs is IEEE fp32 (fp64 where R-UNMOLD / R-RESIZE say so) in a fixed operation order (this file is
+// compiled -fmad=false) and is reproduced bit for bit by the numpy restatement in tests/heads_ref.py.
+#include "mf_common.cuh"
+#include "mf_boxes.cuh"
+#include "mf_kernels.h"
+#include "../../include/maskfusion_b200.h"
+#include <cuda_bf16.h>
+#include <algorithm>
+#include <math.h>
+#include <string.h>
+#include <string>
+#include <vector>
+
+namespace mfb {
+
+constexpr int DET_ROIS = 1000, DET_MAX = 100, NCLS = 81, FC_N = 1024, POOL = 7, CH = 256, HEAD_N = 448;
+constexpr int MPOOL = 14, MPIX = MPOOL * MPOOL, MASK = 28, MLOG_N = 128, MCONV_K = 9 * CH, SEL_N = 1024, EXPORT_CAP = 128;
+constexpr float DET_MIN_CONFIDENCE = 0.7f, DET_NMS_THRESHOLD = 0.3f;
+constexpr float HEAD_LOGIT_GAIN = 1e-3f, HEAD_DELTA_GAIN = 2e-5f, MASK_LOGIT_GAIN = 1e-3f;     // see mf_detector_create
+
+// layer table: FC1, FC2, heads, 4 mask convs, transposed conv, mask logits; rows = GEMM N (zero rows included)
+enum { L_FC1, L_FC2, L_HEAD, L_M1, L_M2, L_M3, L_M4, L_DECONV, L_MLOG, N_LAYERS };
+struct LayerDef { int cin, cout, k, stride, pad, K, rows; };
+static const LayerDef LAYERS[N_LAYERS] = {
+    {CH, FC_N, POOL, 1, 0, POOL * POOL * CH, FC_N}, {FC_N, FC_N, 1, 1, 0, FC_N, FC_N}, {FC_N, NCLS * 5, 1, 1, 0, FC_N, HEAD_N},
+    {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH},
+    {CH, CH, 2, 2, 0, CH, 4 * CH}, {CH, NCLS, 1, 1, 0, CH, MLOG_N}};
+
+struct ExportParams { double min_score; int n_filter, n_special; int filter[EXPORT_CAP], special[EXPORT_CAP]; };
+
+// R-SOFTMAX + argmax + class-specific refinement of one ROI per thread -> candidate key (class, ~ord(score), roi) or ~0, refined box, score
+__global__ void k_det_refine(const float4* __restrict__ rois, const float* __restrict__ logits, int lstride, const float* __restrict__ deltas,
+                             int dstride, int n, float4 win, unsigned long long* __restrict__ keys, float4* __restrict__ boxes, float* __restrict__ scores)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float* l = logits + (size_t)i * lstride;
+    float m = l[0];
+    for (int c = 1; c < NCLS; ++c) m = l[c] > m ? l[c] : m;
+    float sum = 0.0f;
+    for (int c = 0; c < NCLS; ++c) sum = sum + det_expf(l[c] - m);
+    int best = 0;
+    float pbest = det_expf(l[0] - m) / sum;
+    for (int c = 1; c < NCLS; ++c) {
+        const float p = det_expf(l[c] - m) / sum;
+        if (p > pbest) { best = c; pbest = p; }
+    }
+    const float* d = deltas + (size_t)i * dstride + 4 * best;
+    const float4 b = decode_box(rois[i], make_float4(d[0], d[1], d[2], d[3]), win);
+    const bool keep = best > 0 && pbest >= DET_MIN_CONFIDENCE;
+    keys[i] = keep ? ((unsigned long long)best << 42) | ((unsigned long long)(~score_ord(pbest)) << 10) | (unsigned)i : ~0ull;
+    boxes[i] = b;
+    scores[i] = pbest;
+}
+
+// one CTA of 1024: sort the candidates on (class, ~ord(score), roi), per-class greedy NMS (warp w: classes w + 1, w + 33, ...), sort the
+// survivors on (~ord(score), roi), write the first 100 as detections (zero padded), their boxes for the mask head's ROI Align, the count
+__global__ void __launch_bounds__(SEL_N) k_det_select(const unsigned long long* __restrict__ keys, int n, const float4* __restrict__ boxes,
+                                                      const float* __restrict__ scores, float* __restrict__ dets, float4* __restrict__ dboxes,
+                                                      int* __restrict__ count)
+{
+    __shared__ unsigned long long sk[SEL_N];
+    __shared__ int segStart[NCLS], segEnd[NCLS];
+    __shared__ unsigned char supp[SEL_N], kept[SEL_N];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    sk[t] = t < n ? keys[t] : ~0ull;
+    supp[t] = 0; kept[t] = 0;
+    if (t < NCLS) { segStart[t] = 0; segEnd[t] = 0; }
+    __syncthreads();
+    cta_bitonic_sort(sk, SEL_N);
+    const int cls = sk[t] == ~0ull ? -1 : (int)(sk[t] >> 42);
+    if (cls > 0) {
+        if (t == 0 || (int)(sk[t - 1] >> 42) != cls) segStart[cls] = t;
+        if (t == SEL_N - 1 || sk[t + 1] == ~0ull || (int)(sk[t + 1] >> 42) != cls) segEnd[cls] = t + 1;
+    }
+    __syncthreads();
+    for (int c = 1 + warp; c < NCLS; c += SEL_N / 32) {
+        const int st = segStart[c], en = segEnd[c];
+        int nk = 0;
+        for (int i = st; i < en && nk < DET_MAX; ++i) {
+            __syncwarp();
+            if (supp[i]) continue;
+            ++nk;
+            if (lane == 0) kept[i] = 1;
+            const float4 bi = boxes[sk[i] & 1023];
+            for (int j = i + 1 + lane; j < en; j += 32)
+                if (iou_tf(bi, boxes[sk[j] & 1023]) > DET_NMS_THRESHOLD) supp[j] = 1;
+        }
+    }
+    __syncthreads();
+    unsigned long long k2 = ~0ull;
+    if (kept[t]) {
+        const unsigned roi = (unsigned)(sk[t] & 1023);
+        k2 = ((unsigned long long)(~score_ord(scores[roi])) << 32) | roi;
+    }
+    const int nkept = __syncthreads_count(kept[t]);
+    sk[t] = k2;
+    __syncthreads();
+    cta_bitonic_sort(sk, SEL_N);
+    if (t < DET_MAX) {
+        float* o = dets + t * 6;
+        float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (t < nkept) {
+            const unsigned roi = (unsigned)(sk[t] & 0xFFFFFFFFull);
+            b = boxes[roi];
+            o[4] = (float)(keys[roi] >> 42);
+            o[5] = scores[roi];
+        } else { o[4] = 0.f; o[5] = 0.f; }
+        o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w;
+        dboxes[t] = b;
+    }
+    if (t == 0) *count = nkept < DET_MAX ? nkept : DET_MAX;
+}
+
+// R-SIGMOID of each detection's own class: mask logits rows [det][y][x][dy][dx] x 128 -> masks [det][2y + dy][2x + dx]
+__global__ void k_mask_select(const float* __restrict__ mlog, const float* __restrict__ dets, float* __restrict__ masks)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= DET_MAX * MASK * MASK) return;
+    const int d = t / (MASK * MASK), Y = (t / MASK) % MASK, X = t % MASK;
+    const int cls = (int)dets[d * 6 + 4];
+    const size_t row = (((size_t)d * MPOOL + (Y >> 1)) * MPOOL + (X >> 1)) * 4 + (Y & 1) * 2 + (X & 1);
+    masks[t] = 1.0f / (1.0f + det_expf(-mlog[row * MLOG_N + cls]));
+}
+
+// R-UNMOLD + the export rule, one thread: detections (window-normalised) -> exported boxes in image pixels, ids, class ids, rois
+// einfo = {exported count, error (special assignment out of range)}; ebox = y1 x1 y2 x2 detection-row per exported detection
+__global__ void k_unmold(const float* __restrict__ dets, float4 win, int W, int H, ExportParams ep, int* __restrict__ ebox, uint8_t* __restrict__ eid,
+                         int* __restrict__ ecls, int* __restrict__ erois, int* __restrict__ einfo)
+{
+    int N = DET_MAX;
+    for (int d = 0; d < DET_MAX; ++d)
+        if (dets[d * 6 + 4] == 0.0f) { N = d; break; }
+    const float wh = win.z - win.x, ww = win.w - win.y;
+    int n = 0, err = 0;
+    for (int d = 0; d < N; ++d) {
+        const float* r = dets + d * 6;
+        const float ny1 = (r[0] - win.x) / wh, nx1 = (r[1] - win.y) / ww, ny2 = (r[2] - win.x) / wh, nx2 = (r[3] - win.y) / ww;
+        const int y1 = (int)rint((double)ny1 * (double)(H - 1) + 0.0), x1 = (int)rint((double)nx1 * (double)(W - 1) + 0.0);
+        const int y2 = (int)rint((double)ny2 * (double)(H - 1) + 1.0), x2 = (int)rint((double)nx2 * (double)(W - 1) + 1.0);
+        if ((y2 - y1) * (x2 - x1) <= 0) continue;
+        const int cid = (int)r[4];
+        uint8_t id = 0;
+        const int e = id_export(cid, r[5], ep.min_score, ep.filter, ep.n_filter, ep.special, ep.n_special, n, &id);
+        if (e < 0) { err = 1; break; }
+        if (e == 0) continue;
+        ebox[n * 5 + 0] = y1; ebox[n * 5 + 1] = x1; ebox[n * 5 + 2] = y2; ebox[n * 5 + 3] = x2; ebox[n * 5 + 4] = d;
+        eid[n] = id;
+        ecls[n] = cid;
+        erois[n * 4 + 0] = y1; erois[n * 4 + 1] = x1; erois[n * 4 + 2] = y2; erois[n * 4 + 3] = x2;
+        ++n;
+    }
+    einfo[0] = err ? 0 : n;
+    einfo[1] = err;
+}
+
+// R-RESIZE value of a 28x28 mask resized to h x w at output pixel (r, c): fp64 bilinear with zero outside the grid, rounded to fp32
+MF_D float resized_mask(const float* __restrict__ m, int h, int w, int r, int c)
+{
+    const double cy = ((double)r + 0.5) * (28.0 / (double)h) - 0.5, cx = ((double)c + 0.5) * (28.0 / (double)w) - 0.5;
+    const double fy0 = floor(cy), fx0 = floor(cx);
+    const int iy = (int)fy0, ix = (int)fx0;
+    const double fy = cy - fy0, fx = cx - fx0;
+    const bool y0 = iy >= 0 && iy < MASK, y1 = iy + 1 >= 0 && iy + 1 < MASK, x0 = ix >= 0 && ix < MASK, x1 = ix + 1 >= 0 && ix + 1 < MASK;
+    const double v00 = y0 && x0 ? (double)m[iy * MASK + ix] : 0.0, v01 = y0 && x1 ? (double)m[iy * MASK + ix + 1] : 0.0;
+    const double v10 = y1 && x0 ? (double)m[(iy + 1) * MASK + ix] : 0.0, v11 = y1 && x1 ? (double)m[(iy + 1) * MASK + ix + 1] : 0.0;
+    const double top = (1.0 - fx) * v00 + fx * v01, bot = (1.0 - fx) * v10 + fx * v11;
+    return (float)((1.0 - fy) * top + fy * bot);
+}
+
+// one thread per image pixel: the last exported detection whose box holds the pixel and whose resized mask is >= 0.5 there gives the id
+__global__ void k_paste(const float* __restrict__ masks, const int* __restrict__ ebox, const uint8_t* __restrict__ eid, const int* __restrict__ einfo,
+                        int W, int H, uint8_t* __restrict__ out)
+{
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= W * H) return;
+    const int y = p / W, x = p - (p / W) * W;
+    uint8_t v = 0;
+    for (int e = einfo[0] - 1; e >= 0; --e) {
+        const int* b = ebox + e * 5;
+        if (y < b[0] || y >= b[2] || x < b[1] || x >= b[3]) continue;
+        if (resized_mask(masks + (size_t)b[4] * MASK * MASK, b[2] - b[0], b[3] - b[1], y - b[0], x - b[1]) >= 0.5f) { v = eid[e]; break; }
+    }
+    out[p] = v;
+}
+
+static int det_fail(const std::string& msg) { cnn_set_error(msg.c_str()); return -1; }
+
+static int check_launch(const char* what)
+{
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return det_fail(std::string(what) + ": " + cudaGetErrorString(e));
+    return 0;
+}
+
+}  // namespace mfb
+
+using namespace mfb;
+
+struct mf_detector {
+    mf_rpn* rpn = nullptr;
+    mf_backbone* bb = nullptr;
+    cudaStream_t s = nullptr;
+    int S = 0, imgW = 0, imgH = 0;
+    float4 win = make_float4(0.f, 0.f, 1.f, 1.f);             // letter-box window of the current image, normalised (norm_boxes)
+    ExportParams ep;
+    std::vector<float> hW[N_LAYERS], hB[N_LAYERS];           // fp32 master copies [rows x K] (bf16-representable), biases [rows]
+    __nv_bfloat16* dW[N_LAYERS] = {};
+    float* dB[N_LAYERS] = {};
+    __nv_bfloat16 *fc1 = nullptr, *fc2 = nullptr, *mpool = nullptr, *col = nullptr, *mconv[4] = {}, *dec = nullptr;
+    float *head = nullptr, *mlog = nullptr, *masks = nullptr, *dets = nullptr, *scores = nullptr;
+    float4 *boxes = nullptr, *dboxes = nullptr;
+    unsigned long long* keys = nullptr;
+    int *count = nullptr, *ebox = nullptr, *ecls = nullptr, *erois = nullptr, *einfo = nullptr;
+    uint8_t *eid = nullptr, *idimg = nullptr;
+    size_t idcap = 0;
+};
+
+// the image geometry: the letter-box window of a W x H image in the S x S input, normalised as norm_boxes does (float64 divide, float32)
+static int set_image(mf_detector* h, int W, int H)
+{
+    if (W < 1 || H < 1 || W > 16384 || H > 16384) return det_fail("detector: image size " + std::to_string(W) + "x" + std::to_string(H) + " outside [1, 16384]");
+    if ((size_t)W * H > h->idcap) {
+        if (h->idimg && (cudaStreamSynchronize(h->s) != cudaSuccess || cudaFree(h->idimg) != cudaSuccess)) return det_fail("detector: id image free failed");
+        h->idimg = nullptr; h->idcap = 0;
+        if (cudaMalloc(&h->idimg, (size_t)W * H) != cudaSuccess) return det_fail("detector: id image cudaMalloc failed");
+        h->idcap = (size_t)W * H;
+    }
+    const MoldGeom g = cnn_mold_geometry(h->S, W, H);
+    const double s1 = (double)(h->S - 1);
+    h->win = make_float4((float)(g.offy / s1), (float)(g.offx / s1), (float)((g.offy + g.newH - 1) / s1), (float)((g.offx + g.newW - 1) / s1));
+    h->imgW = W; h->imgH = H;
+    return 0;
+}
+
+static int gemm(mf_detector* h, int layer, const void* A, void* out, int M, int relu, bool f32)
+{
+    const LayerDef& L = LAYERS[layer];
+    return launch_gemm_bf16(A, h->dW[layer], h->dB[layer], nullptr, out, M, L.rows, L.K, relu, h->s, nullptr, f32) ? -2 : 0;
+}
+
+static int refine(mf_detector* h, const float* rois, const float* logits, int lstride, const float* deltas, int dstride, int n)
+{
+    prof_mark(h->s, "k_det_refine");
+    k_det_refine<<<(n + 127) / 128, 128, 0, h->s>>>((const float4*)rois, logits, lstride, deltas, dstride, n, h->win, h->keys, h->boxes, h->scores);
+    prof_mark(h->s, "k_det_select");
+    k_det_select<<<1, SEL_N, 0, h->s>>>(h->keys, n, h->boxes, h->scores, h->dets, h->dboxes, h->count);
+    return check_launch("detection layer") ? -3 : 0;
+}
+
+static int paste(mf_detector* h, const float* dets, const float* masks)
+{
+    prof_mark(h->s, "k_unmold");
+    k_unmold<<<1, 1, 0, h->s>>>(dets, h->win, h->imgW, h->imgH, h->ep, h->ebox, h->eid, h->ecls, h->erois, h->einfo);
+    prof_mark(h->s, "k_paste");
+    k_paste<<<(h->imgW * h->imgH + 255) / 256, 256, 0, h->s>>>(masks, h->ebox, h->eid, h->einfo, h->imgW, h->imgH, h->idimg);
+    return check_launch("id image") ? -3 : 0;
+}
+
+// ==========================================================================================
+// C ABI (declared in include/maskfusion_b200.h)
+// ==========================================================================================
+extern "C" void mf_detector_destroy(mf_detector* h)
+{
+    if (!h) return;
+    for (int i = 0; i < N_LAYERS; ++i) { if (h->dW[i]) cudaFree(h->dW[i]); if (h->dB[i]) cudaFree(h->dB[i]); }
+    void* ptrs[] = {h->fc1, h->fc2, h->mpool, h->col, h->mconv[0], h->mconv[1], h->mconv[2], h->mconv[3], h->dec, h->head, h->mlog, h->masks,
+                    h->dets, h->scores, h->boxes, h->dboxes, h->keys, h->count, h->ebox, h->ecls, h->erois, h->einfo, h->eid, h->idimg};
+    for (void* p : ptrs) if (p) cudaFree(p);
+    delete h;
+}
+
+extern "C" mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed)
+{
+    if (!rpn) { det_fail("detector: no region-proposal handle"); return nullptr; }
+    mf_detector* h = new mf_detector;
+    h->rpn = rpn;
+    h->bb = rpn_backbone(rpn);
+    h->s = (cudaStream_t)mf_backbone_stream(h->bb);
+    int d[3];
+    mf_backbone_output(h->bb, 4, d);
+    h->S = d[0] * 4;
+    memset(&h->ep, 0, sizeof h->ep);
+    h->ep.min_score = 0.55;
+    // weights: FC1, FC2, the mask convs and the transposed conv at gain 1 (He-style, the backbone's scheme).  Their synthetic outputs are
+    // O(1000) (the pooled features carry the pixel-unit scale of the moulded input), so the output layers are damped: class logits of a
+    // few units (at gain 1 every softmax saturates; far below, the 81-way softmax stays near uniform and no ROI reaches the 0.7
+    // confidence), |delta| ~ 0.15 (refined boxes stay near their proposals), mask logits of a few units (mask pixels on both sides of 0.5).
+    uint32_t sd = seed ? seed : 1u;
+    for (int i = 0; i < N_LAYERS; ++i) {
+        const LayerDef& L = LAYERS[i];
+        h->hW[i].assign((size_t)L.rows * L.K, 0.f);
+        h->hB[i].assign(L.rows, 0.f);
+        if (i == L_HEAD) {
+            synth_weights(h->hW[i].data(), h->hB[i].data(), NCLS, L.K, HEAD_LOGIT_GAIN, sd);
+            synth_weights(h->hW[i].data() + (size_t)NCLS * L.K, h->hB[i].data() + NCLS, 4 * NCLS, L.K, HEAD_DELTA_GAIN, sd);
+        } else if (i == L_MLOG) {
+            synth_weights(h->hW[i].data(), h->hB[i].data(), NCLS, L.K, MASK_LOGIT_GAIN, sd);
+        } else if (i == L_DECONV) {
+            // conv-transpose kernel [dy][dx][cout][cin] as GEMM rows (dy * 2 + dx) * 256 + cout; one bias per output channel
+            synth_weights(h->hW[i].data(), h->hB[i].data(), L.rows, L.K, 1.0f, sd);
+            for (int r = CH; r < L.rows; ++r) h->hB[i][r] = h->hB[i][r % CH];
+        } else
+            synth_weights(h->hW[i].data(), h->hB[i].data(), L.rows, L.K, 1.0f, sd);
+    }
+    bool ok = true;
+    for (int i = 0; i < N_LAYERS && ok; ++i)
+        ok = cudaMalloc(&h->dW[i], h->hW[i].size() * 2) == cudaSuccess && cudaMalloc(&h->dB[i], h->hB[i].size() * 4) == cudaSuccess;
+    const size_t mrows = (size_t)DET_MAX * MPIX;
+    ok = ok && cudaMalloc(&h->fc1, (size_t)DET_ROIS * FC_N * 2) == cudaSuccess && cudaMalloc(&h->fc2, (size_t)DET_ROIS * FC_N * 2) == cudaSuccess &&
+         cudaMalloc(&h->head, (size_t)DET_ROIS * HEAD_N * 4) == cudaSuccess && cudaMalloc(&h->keys, DET_ROIS * 8) == cudaSuccess &&
+         cudaMalloc(&h->boxes, DET_ROIS * 16) == cudaSuccess && cudaMalloc(&h->scores, DET_ROIS * 4) == cudaSuccess &&
+         cudaMalloc(&h->dets, DET_MAX * 6 * 4) == cudaSuccess && cudaMalloc(&h->dboxes, DET_MAX * 16) == cudaSuccess &&
+         cudaMalloc(&h->count, 4) == cudaSuccess && cudaMalloc(&h->mpool, mrows * CH * 2) == cudaSuccess &&
+         cudaMalloc(&h->col, mrows * MCONV_K * 2) == cudaSuccess && cudaMalloc(&h->dec, mrows * 4 * CH * 2) == cudaSuccess &&
+         cudaMalloc(&h->mlog, mrows * 4 * MLOG_N * 4) == cudaSuccess && cudaMalloc(&h->masks, DET_MAX * MASK * MASK * 4) == cudaSuccess &&
+         cudaMalloc(&h->ebox, DET_MAX * 5 * 4) == cudaSuccess && cudaMalloc(&h->ecls, DET_MAX * 4) == cudaSuccess &&
+         cudaMalloc(&h->erois, DET_MAX * 16) == cudaSuccess && cudaMalloc(&h->einfo, 8) == cudaSuccess && cudaMalloc(&h->eid, DET_MAX) == cudaSuccess;
+    for (int i = 0; i < 4 && ok; ++i) ok = cudaMalloc(&h->mconv[i], mrows * CH * 2) == cudaSuccess;
+    if (!ok) { det_fail("detector: cudaMalloc failed"); mf_detector_destroy(h); return nullptr; }
+    for (int i = 0; i < N_LAYERS && ok; ++i) {
+        std::vector<__nv_bfloat16> w(h->hW[i].size());
+        for (size_t k = 0; k < w.size(); ++k) w[k] = __float2bfloat16(h->hW[i][k]);
+        ok = cudaMemcpy(h->dW[i], w.data(), w.size() * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
+             cudaMemcpy(h->dB[i], h->hB[i].data(), h->hB[i].size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+    }
+    ok = ok && cudaMemset(h->dets, 0, DET_MAX * 6 * 4) == cudaSuccess && cudaMemset(h->count, 0, 4) == cudaSuccess &&
+         cudaMemset(h->masks, 0, DET_MAX * MASK * MASK * 4) == cudaSuccess && cudaMemset(h->einfo, 0, 8) == cudaSuccess;
+    if (!ok || set_image(h, h->S, h->S)) { det_fail("detector: upload failed"); mf_detector_destroy(h); return nullptr; }
+    return h;
+}
+
+extern "C" int mf_detector_run(mf_detector* h, int stages)
+{
+    if (!h) return det_fail("detector: null handle");
+    const cudaStream_t s = h->s;
+    if (stages & MF_DET_CLASSIFIER) {
+        if (gemm(h, L_FC1, rpn_pooled(h->rpn), h->fc1, DET_ROIS, 1, false) || gemm(h, L_FC2, h->fc1, h->fc2, DET_ROIS, 1, false) ||
+            gemm(h, L_HEAD, h->fc2, h->head, DET_ROIS, 0, true)) return -2;
+    }
+    if ((stages & MF_DET_DETECTIONS) && refine(h, rpn_rois(h->rpn), h->head, HEAD_N, h->head + NCLS, HEAD_N, DET_ROIS)) return -3;
+    if (stages & MF_DET_MASKS) {
+        if (mf_roi_align_bf16(h->bb, (const float*)h->dboxes, DET_MAX, MPOOL, h->mpool)) return -3;
+        const __nv_bfloat16* x = h->mpool;
+        for (int i = 0; i < 4; ++i) {
+            launch_im2col(x, DET_MAX, MPOOL, MPOOL, CH, MPOOL, MPOOL, 3, 1, 1, MCONV_K, h->col, s);
+            if (gemm(h, L_M1 + i, h->col, h->mconv[i], DET_MAX * MPIX, 1, false)) return -2;
+            x = h->mconv[i];
+        }
+        if (gemm(h, L_DECONV, x, h->dec, DET_MAX * MPIX, 1, false) || gemm(h, L_MLOG, h->dec, h->mlog, DET_MAX * MPIX * 4, 0, true)) return -2;
+        prof_mark(s, "k_mask_select");
+        k_mask_select<<<(DET_MAX * MASK * MASK + 255) / 256, 256, 0, s>>>(h->mlog, h->dets, h->masks);
+        if (check_launch("k_mask_select")) return -3;
+    }
+    if ((stages & MF_DET_ID_IMAGE) && paste(h, h->dets, h->masks)) return -3;
+    return 0;
+}
+
+extern "C" int mf_detector_forward(mf_detector* h, int image_w, int image_h)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (set_image(h, image_w, image_h)) return -1;
+    return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+}
+
+extern "C" int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int H)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (!d_rgba || ((uintptr_t)d_rgba & 3)) return det_fail("detector: the image needs a 4-byte aligned device pointer");
+    if (set_image(h, W, H)) return -1;
+    if (mf_backbone_mold(h->bb, d_rgba, W, H) || mf_backbone_forward(h->bb, mf_backbone_input_buffer(h->bb)))
+        return det_fail(std::string("detector: backbone: ") + cnn_last_error());
+    if (mf_rpn_forward(h->rpn)) return -3;
+    return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+}
+
+extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const int32_t* class_filter, int n_filter, const int32_t* special_assignments,
+                                      int n_special)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (n_filter < 0 || n_special < 0 || n_filter > EXPORT_CAP || n_special > EXPORT_CAP || (n_filter && !class_filter) || (n_special && !special_assignments))
+        return det_fail("detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries");
+    ExportParams ep;
+    memset(&ep, 0, sizeof ep);
+    ep.min_score = min_score; ep.n_filter = n_filter; ep.n_special = n_special;
+    for (int i = 0; i < n_filter; ++i) ep.filter[i] = class_filter[i];
+    for (int i = 0; i < n_special; ++i) ep.special[i] = special_assignments[i];
+    h->ep = ep;
+    return 0;
+}
+
+extern "C" int mf_detector_refine(mf_detector* h, const float* d_rois, const float* d_logits, const float* d_deltas, int n)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (n < 1 || n > DET_ROIS) return det_fail("detector_refine: n = " + std::to_string(n) + " outside [1, 1000]");
+    if (!d_rois || !d_logits || !d_deltas || ((uintptr_t)d_rois & 15) || ((uintptr_t)d_logits & 3) || ((uintptr_t)d_deltas & 3))
+        return det_fail("detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer");
+    return refine(h, d_rois, d_logits, NCLS, d_deltas, 4 * NCLS, n);
+}
+
+extern "C" int mf_detector_paste(mf_detector* h, const float* d_detections, const float* d_masks, int W, int H)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (!d_detections || !d_masks || ((uintptr_t)d_detections & 3) || ((uintptr_t)d_masks & 3))
+        return det_fail("detector_paste: detections and masks need 4-byte aligned device pointers");
+    if (set_image(h, W, H)) return -1;
+    return paste(h, d_detections, d_masks);
+}
+
+extern "C" int mf_detector_num_layers(mf_detector* h) { return h ? N_LAYERS : -1; }
+
+extern "C" int mf_detector_layer(mf_detector* h, int i, int* out6)
+{
+    if (!h || i < 0 || i >= N_LAYERS || !out6) return det_fail("detector: bad layer index");
+    const LayerDef& L = LAYERS[i];
+    out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
+    return 0;
+}
+
+extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* bias)
+{
+    if (!h || i < 0 || i >= N_LAYERS) return det_fail("detector: bad layer index");
+    if (w) memcpy(w, h->hW[i].data(), h->hW[i].size() * 4);
+    if (bias) memcpy(bias, h->hB[i].data(), h->hB[i].size() * 4);
+    return 0;
+}
+
+static int download(mf_detector* h, void* dst, const void* src, size_t bytes)
+{
+    if (!dst) return 0;
+    if (cudaStreamSynchronize(h->s) != cudaSuccess || cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return det_fail(std::string("detector download: ") + cudaGetErrorString(cudaGetLastError()));
+    return 0;
+}
+
+extern "C" int mf_detector_get_fc(mf_detector* h, void* fc1_bf16, void* fc2_bf16)
+{
+    if (!h) return det_fail("detector: null handle");
+    return download(h, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2) || download(h, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2) ? -1 : 0;
+}
+
+extern "C" int mf_detector_get_head_outputs(mf_detector* h, float* logits, float* deltas)
+{
+    if (!h) return det_fail("detector: null handle");
+    std::vector<float> head((size_t)DET_ROIS * HEAD_N);
+    if (download(h, head.data(), h->head, head.size() * 4)) return -1;
+    for (int r = 0; r < DET_ROIS; ++r) {
+        if (logits) memcpy(logits + (size_t)r * NCLS, &head[(size_t)r * HEAD_N], NCLS * 4);
+        if (deltas) memcpy(deltas + (size_t)r * NCLS * 4, &head[(size_t)r * HEAD_N + NCLS], NCLS * 16);
+    }
+    return 0;
+}
+
+extern "C" int mf_detector_get_mask_layer(mf_detector* h, int i, void* host)
+{
+    if (!h) return det_fail("detector: null handle");
+    const size_t px = (size_t)DET_MAX * MPIX;
+    switch (i) {
+    case 0: return download(h, host, h->mpool, px * CH * 2);
+    case 1: case 2: case 3: case 4: return download(h, host, h->mconv[i - 1], px * CH * 2);
+    case 5: return download(h, host, h->dec, px * 4 * CH * 2);
+    case 6: {
+        std::vector<float> m(px * 4 * MLOG_N);
+        if (download(h, m.data(), h->mlog, m.size() * 4)) return -1;
+        for (size_t r = 0; r < px * 4; ++r) memcpy((float*)host + r * NCLS, &m[r * MLOG_N], NCLS * 4);
+        return 0;
+    }
+    default: return det_fail("detector: mask layer must be 0..6");
+    }
+}
+
+extern "C" int mf_detector_get_detections(mf_detector* h, float* detections)
+{
+    int n = 0;
+    if (!h) return det_fail("detector: null handle");
+    if (download(h, detections, h->dets, DET_MAX * 6 * 4) || download(h, &n, h->count, 4)) return -1;
+    return n;
+}
+
+extern "C" int mf_detector_get_masks(mf_detector* h, float* masks)
+{
+    return h ? download(h, masks, h->masks, DET_MAX * MASK * MASK * 4) : det_fail("detector: null handle");
+}
+
+extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32_t* class_ids, int32_t* rois)
+{
+    if (!h) return det_fail("detector: null handle");
+    int info[2];
+    if (download(h, info, h->einfo, 8)) return -1;
+    if (info[1]) return det_fail("generate_id_image: special_assignments[class_id] out of range");
+    if (download(h, id_image, h->idimg, (size_t)h->imgW * h->imgH) || download(h, class_ids, h->ecls, (size_t)info[0] * 4) ||
+        download(h, rois, h->erois, (size_t)info[0] * 16)) return -1;
+    return info[0];
+}
+
+extern "C" int mf_detector_image_size(mf_detector* h, int* w, int* hgt)
+{
+    if (!h) return det_fail("detector: null handle");
+    *w = h->imgW; *hgt = h->imgH;
+    return 0;
+}

@@ -5,6 +5,9 @@
 #include <stdint.h>
 #include "mf_common.cuh"
 
+struct mf_backbone;
+struct mf_rpn;
+
 namespace mfb {
 
 struct SurfelPlanes { float4* pos; float4* col; float4* nrm; };
@@ -151,8 +154,20 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
 int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
              cudaStream_t s);
 bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win);     // does cnn_conv take the implicit path (no im2col)?
+// im2col of `nimg` stacked NHWC images (each padded on its own): A[(img, oy, ox)][(ky, kx, cin)], K zero-padded to Kpad
+void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int k, int stride, int pad, int Kpad, void* col, cudaStream_t s);
+// the letter-box rule of mf_backbone_mold (mould_image): a W x H image is resized by `scale` to newW x newH and placed at (offx, offy) of S x S
+struct MoldGeom { float scale; int newW, newH, offx, offy; };
+MoldGeom cnn_mold_geometry(int S, int W, int H);
 const char* cnn_last_error();
 void cnn_set_error(const char* msg);
+
+// ---- mf_rpn.cu: what the detection heads read of the RPN handle ----
+mf_backbone* rpn_backbone(mf_rpn* h);
+const float* rpn_rois(mf_rpn* h);                 // [1000][4] proposals, zero padded
+const void* rpn_pooled(mf_rpn* h);                // [1000][7][7][256] bf16
+// seeded He-style weights [rows x K] (bf16-representable) and biases, the backbone's scheme (mf_cnn.cu add_conv)
+void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed);
 
 // ---- mf_frame.cu ----
 void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, cudaStream_t s);

@@ -11,6 +11,7 @@
 // Unlike KlgLogReader, hasMore() lets the LAST frame through (currentFrame starts at -1, :145,:326).
 // The reference's background buffering thread (:203-220) is an I/O detail and is not reproduced: frames are decoded on demand.
 #include "../../include/maskfusion_b200.h"
+#include "mf_boxes.cuh"
 #include <dirent.h>
 #include <stdio.h>
 #include <stdint.h>
@@ -545,17 +546,10 @@ extern "C" int mf_generate_id_image(const uint8_t* masks, int H, int W, int N, c
     int n = 0;
     for (int m = 0; m < N; ++m) {
         const int cid = class_ids[m];
-        bool pass = n_filter == 0;
-        for (int k = 0; k < n_filter && !pass; ++k) pass = class_filter[k] == cid;
-        if (!pass || !((double)scores[m] >= min_score)) continue;      // the float32 score against a double, as NumPy 1.x (the reference's TF-1.8-era environment) compares them
-        int val = n + 1;
-        bool special = false;
-        for (int k = 0; k < n_special && !special; ++k) special = special_assignments[k] == cid;   // "class_id in special_assignments"
-        if (special) {
-            if (cid < 0 || cid >= n_special) { mf_set_error("generate_id_image: special_assignments[class_id] out of range"); return -3; }   // Python: IndexError
-            val = special_assignments[cid];
-        }
-        const uint8_t v = (uint8_t)val;                                                 // numpy assignment into a uint8 image wraps
+        uint8_t v = 0;
+        const int e = mfb::id_export(cid, scores[m], min_score, class_filter, n_filter, special_assignments, n_special, n, &v);
+        if (e < 0) { mf_set_error("generate_id_image: special_assignments[class_id] out of range"); return -3; }   // Python: IndexError
+        if (e == 0) continue;
         for (size_t p = 0; p < P; ++p) if (masks[p * N + m] == 1) id_image[p] = v;
         if (exported_class_ids) exported_class_ids[n] = cid;
         if (exported_rois) for (int k = 0; k < 4; ++k) exported_rois[n * 4 + k] = rois[m * 4 + k];

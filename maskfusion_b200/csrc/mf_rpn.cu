@@ -20,6 +20,7 @@
 //   k_nms_mask      IoU > 0.7 bitmask: candidate i x 64-candidate words (upper triangle only)
 //   k_nms_scan      one warp: the greedy scan over the bitmask, stop at 1000 kept, zero padding
 #include "mf_common.cuh"
+#include "mf_boxes.cuh"
 #include "mf_kernels.h"
 #include "../../include/maskfusion_b200.h"
 #include <cuda_bf16.h>
@@ -37,15 +38,6 @@ constexpr int SORT_CAP = 8192;                              // bitonic sort size
 constexpr float RPN_NMS_THRESHOLD = 0.7f;
 
 struct SelState { unsigned long long prefix, mask; unsigned krem, nsel; unsigned hist[256]; };
-
-// order-preserving map of a float to uint32 (ascending); -0 is +0, NaN -> 0 (below -inf, so ~ord puts it last)
-MF_D uint32_t score_ord(float s)
-{
-    if (s != s) return 0u;
-    if (s == 0.0f) s = 0.0f;
-    const uint32_t u = __float_as_uint(s);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // softmax over the two logits (Keras: exp(x - max) / sum) -> foreground score -> R-TOPK key; block 0 resets the selection state
 __global__ void k_rpn_keys(const float2* __restrict__ logits, int n, int k, unsigned long long* __restrict__ keys, SelState* st)
@@ -110,21 +102,6 @@ __global__ void k_sel_compact(const unsigned long long* __restrict__ keys, int n
     }
 }
 
-// apply_box_deltas_graph (upstream operation order) + clip_boxes_graph to the window [0, 0, 1, 1]; box = y1 x1 y2 x2
-MF_D float4 decode_box(float4 a, float4 d)
-{
-    d.x = d.x * 0.1f; d.y = d.y * 0.1f; d.z = d.z * 0.2f; d.w = d.w * 0.2f;          // RPN_BBOX_STD_DEV
-    float h = a.z - a.x, w = a.w - a.y;
-    float cy = a.x + 0.5f * h, cx = a.y + 0.5f * w;
-    cy = cy + d.x * h;
-    cx = cx + d.y * w;
-    h = h * det_expf(d.z);
-    w = w * det_expf(d.w);
-    const float y1 = cy - 0.5f * h, x1 = cx - 0.5f * w;
-    const float y2 = y1 + h, x2 = x1 + w;
-    return make_float4(fmaxf(fminf(y1, 1.0f), 0.0f), fmaxf(fminf(x1, 1.0f), 0.0f), fmaxf(fminf(y2, 1.0f), 0.0f), fmaxf(fminf(x2, 1.0f), 0.0f));
-}
-
 // one CTA: bitonic sort of the k selected keys (padded with ~0 to a power of two), then the boxes in R-TOPK order
 __global__ void __launch_bounds__(1024) k_sort_decode(const unsigned long long* __restrict__ sel, int k, const float4* __restrict__ deltas,
                                                       const float4* __restrict__ anchors, float4* __restrict__ boxes)
@@ -134,36 +111,11 @@ __global__ void __launch_bounds__(1024) k_sort_decode(const unsigned long long* 
     while (P < k) P <<= 1;
     for (int i = threadIdx.x; i < P; i += blockDim.x) sk[i] = i < k ? sel[i] : ~0ull;
     __syncthreads();
-    for (int size = 2; size <= P; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int i = threadIdx.x; i < P / 2; i += blockDim.x) {
-                const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                const bool asc = (lo & size) == 0;
-                const unsigned long long a = sk[lo], b = sk[hi];
-                if ((a > b) == asc) { sk[lo] = b; sk[hi] = a; }
-            }
-            __syncthreads();
-        }
+    cta_bitonic_sort(sk, P);
     for (int i = threadIdx.x; i < k; i += blockDim.x) {
         const unsigned idx = (unsigned)(sk[i] & 0xFFFFFFFFull);
-        boxes[i] = decode_box(anchors[idx], deltas[idx]);
+        boxes[i] = decode_box(anchors[idx], deltas[idx], make_float4(0.f, 0.f, 1.f, 1.f));
     }
-}
-
-// TensorFlow's NMS IoU: corners min/max-normalised, an empty box overlaps nothing
-MF_D float lesser(float a, float b) { return b < a ? b : a; }       // std::min
-MF_D float greater(float a, float b) { return a < b ? b : a; }      // std::max
-MF_D float iou_tf(float4 i, float4 j)
-{
-    const float ymin_i = lesser(i.x, i.z), xmin_i = lesser(i.y, i.w), ymax_i = greater(i.x, i.z), xmax_i = greater(i.y, i.w);
-    const float ymin_j = lesser(j.x, j.z), xmin_j = lesser(j.y, j.w), ymax_j = greater(j.x, j.z), xmax_j = greater(j.y, j.w);
-    const float area_i = (ymax_i - ymin_i) * (xmax_i - xmin_i);
-    const float area_j = (ymax_j - ymin_j) * (xmax_j - xmin_j);
-    if (area_i <= 0.0f || area_j <= 0.0f) return 0.0f;
-    const float iymin = greater(ymin_i, ymin_j), ixmin = greater(xmin_i, xmin_j);
-    const float iymax = lesser(ymax_i, ymax_j), ixmax = lesser(xmax_i, xmax_j);
-    const float inter = greater(iymax - iymin, 0.0f) * greater(ixmax - ixmin, 0.0f);
-    return inter / ((area_i + area_j) - inter);
 }
 
 // bit j of word (i, c) set <=> candidate 64c + j comes after i and IoU(i, 64c + j) > 0.7; words left of the diagonal are not written
@@ -269,8 +221,7 @@ static uint32_t lcg(uint32_t& s) { s = s * 1664525u + 1013904223u; return s; }
 static float urand(uint32_t& s) { return (float)(lcg(s) >> 8) * (1.0f / 16777216.0f) * 2.f - 1.f; }
 static float bf16_round(float f) { return __bfloat162float(__float2bfloat16(f)); }
 
-// seeded He-style weights [rows x K] (bf16-representable) and biases, the backbone's scheme (mf_cnn.cu add_conv)
-static void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed)
+void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed)
 {
     const float sc = gain * sqrtf(2.0f / (float)K);
     for (int o = 0; o < rows; ++o)
@@ -535,3 +486,8 @@ extern "C" int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16)
 {
     return h ? download(h, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) : rpn_fail("rpn: null handle");
 }
+
+// ---- what the detection heads (mf_heads.cu) read of the handle ----
+mf_backbone* mfb::rpn_backbone(mf_rpn* h) { return h->bb; }
+const float* mfb::rpn_rois(mf_rpn* h) { return h->rois; }
+const void* mfb::rpn_pooled(mf_rpn* h) { return h->pooled; }
