@@ -120,6 +120,26 @@ int mf_download_edge_map(mf_context* ctx, float* edge, uint8_t* binary);        
  * processFrame letter-boxes the frame's RGB image into `backbone`'s input (mf_backbone_mold) and enqueues its forward on the backbone's
  * own stream, concurrently with the dense pipeline on the same GPU.  backbone = handle of mf_backbone_create; NULL detaches. */
 int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k);
+/* Mask R-CNN detector on the frame path: MfSegmentation::performSegmentation calls MaskRCNN::executeSequential when the frame has no mask
+ * (MfSegmentation.cpp:128-131), which fills FrameData::mask with the id image and FrameData::classIDs with [0] followed by the exported class
+ * ids (MaskRCNN.cpp:98-151).  With a detector attached (handle of mf_detector_create), a frame runs it when the context is multi-model,
+ * the caller passed NO mask, the frame runs segmentation (tick > 1 and not an in_pose frame) and mf_tick() % every_k == 0 before the call.
+ * Detection (mould, backbone, RPN, heads at the context's W x H) and the hand-off into the frame's mask and class list are enqueued on the
+ * detector's stream behind the frame's preprocessing; the context's stream waits for them only where segmentation first reads the mask,
+ * so tracking and the ID projection overlap the detector.  Nothing in the frame waits for the host.
+ *   - A frame skipped by every_k carries no masks (as with mask = NULL and no detector).  A frame given a mask uses it and the classes of
+ *     mf_set_frame_classes; the detector does not run.
+ *   - A failing export rule (special_assignments[class_id] out of range, an IndexError upstream) leaves that frame without masks, and the
+ *     NEXT call on the context returns non-zero with the message.
+ *   - Refused: a -static context, world > 1, a backbone attached (and mf_attach_backbone while a detector is attached); mf_shard_configure
+ *     and mf_shard_comm_init refuse a context with a detector attached.
+ *   - NULL detaches; detaching and mf_destroy first wait for the last hand-off.  The context never destroys the detector: detach (or destroy
+ *     the context) before destroying it.  Detector launches are not counted in mf_kernel_launches. */
+struct mf_detector;
+int mf_attach_detector(mf_context* ctx, struct mf_detector* detector, int every_k);
+/* FrameData::mask (W x H) and classIDs (n_masks entries of class_ids_256) that segmentation read on the last frame; mask is all zero when
+ * n_masks is 0 (the frame carried no masks).  NULL skips an output.  Multi-model contexts only. */
+int mf_download_frame_masks(mf_context* ctx, uint8_t* mask, int32_t* class_ids_256, int* n_masks);
 int mf_debug_track_timing(int64_t* out, int cap);   /* profiling builds only (-DMF_TRACK_TIMING): (tag, SM clock) pairs of the last tracking launch; else 0 */
 int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int iterations, int ellipse, uint8_t* inverted);
 

@@ -58,7 +58,7 @@ EXPORTS = [
     "mf_detector_create", "mf_detector_destroy", "mf_detector_run", "mf_detector_forward", "mf_detector_detect", "mf_detector_set_export",
     "mf_detector_refine", "mf_detector_paste", "mf_detector_num_layers", "mf_detector_layer", "mf_detector_get_weights", "mf_detector_get_fc",
     "mf_detector_get_head_outputs", "mf_detector_get_mask_layer", "mf_detector_get_detections", "mf_detector_get_masks", "mf_detector_get_id_image",
-    "mf_detector_image_size",
+    "mf_detector_image_size", "mf_attach_detector", "mf_download_frame_masks",
     "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
     "mf_shard_projection_keys", "mf_shard_frame_end", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
 ]
@@ -184,6 +184,8 @@ def load_library():
     L.mf_detector_get_masks.argtypes = [C.c_void_p, C.c_void_p]
     L.mf_detector_get_id_image.argtypes = [C.c_void_p] * 4
     L.mf_detector_image_size.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.mf_attach_detector.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    L.mf_download_frame_masks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
     L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.mf_shard_frame_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
     L.mf_shard_unique_id.argtypes = [C.c_void_p]
@@ -395,6 +397,18 @@ class MaskFusion:
     def attachBackbone(self, backbone, every_k: int = 5):
         """Mask R-CNN backbone on the frame path: every k-th processFrame enqueues mold + forward on the backbone's stream"""
         self._ck(self.L.mf_attach_backbone(self.h, C.c_void_p(backbone.h) if backbone is not None else None, int(every_k)))
+
+    def attachDetector(self, detector, every_k: int = 1):
+        """Mask R-CNN detector on the frame path (mf_attach_detector): segmentation frames given no mask take the detector's id image
+        and class ids every k-th tick; None detaches.  The context does not own the detector: detach before closing it."""
+        self._ck(self.L.mf_attach_detector(self.h, C.c_void_p(detector.h) if detector is not None else None, int(every_k)))
+
+    def frameMasks(self):
+        """-> (mask H x W uint8, class ids) that segmentation read on the last frame (FrameData::mask / classIDs); ([all zero], [])
+        when the frame carried no masks"""
+        m = np.zeros((self.H, self.W), np.uint8); c = np.zeros(256, np.int32); n = C.c_int(0)
+        self._ck(self.L.mf_download_frame_masks(self.h, _p(m), _p(c), C.byref(n)))
+        return m, c[:n.value].tolist()
 
     def setFrameClasses(self, classIDs):
         c = np.ascontiguousarray(classIDs, np.int32)

@@ -363,6 +363,31 @@ extern "C" int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k)
     MF_CATCH(-1)
 }
 
+// Mask R-CNN detector on the frame path (MfSegmentation.cpp:128-131, MaskRCNN.cpp:98-151): the masks of segmentation frames that the caller
+// gives none come from `detector` every k-th tick.  NULL detaches (after the last hand-off has landed).
+extern "C" int mf_attach_detector(mf_context* ctx, mf_detector* detector, int every_k)
+{
+    MF_TRY MF_NEED(ctx)
+    ctx->mf->attachDetector(detector, every_k); return 0;
+    MF_CATCH(-1)
+}
+// FrameData::mask / classIDs as segmentation read them on the last frame (replaces the reference's WRITE_MASK_FILES dump)
+extern "C" int mf_download_frame_masks(mf_context* ctx, uint8_t* mask, int32_t* class_ids_256, int* n_masks)
+{
+    MF_TRY MF_NEED(ctx)
+    MaskFusion* o = ctx->mf;
+    if (!o->cfg.enableMultipleModels) { g_err = "not a multi-model context"; return -5; }
+    FrameHdr h;
+    cudaCheck(cudaMemcpyAsync(&h, o->dHdr, sizeof h, cudaMemcpyDeviceToHost, o->stream), "D2H");
+    d2h(o, mask, o->frameMask, o->P);
+    o->sync();
+    if (mask && h.nMasks == 0) memset(mask, 0, o->P);            // a frame without masks: the set's mask bytes are stale
+    if (class_ids_256) memcpy(class_ids_256, h.classIDs, sizeof h.classIDs);
+    if (n_masks) *n_masks = h.nMasks;
+    return 0;
+    MF_CATCH(-1)
+}
+
 // stage clock of the last tracking launch: (tag, SM clock) pairs; 0 unless the library was built with -DMF_TRACK_TIMING (A/B builds)
 extern "C" int mf_debug_track_timing(int64_t* out, int cap) { return debug_track_timing((long long*)out, cap); }
 

@@ -15,6 +15,8 @@
 //   unmold_detections +    k_unmold (one thread) maps the detections to integer boxes of the original image and applies
 //   generate_id_image      generate_id_image's export rule; k_paste (one thread per pixel) walks the exported detections from last to first
 //                          and writes the first whose resized mask is >= 0.5 there -- no H x W x N mask stack
+//   hand-off               k_frame_masks (mf_attach_detector): the id image, [0] + exported class ids and their count into a frame's
+//                          FrameData::mask / classIDs (MaskRCNN.cpp:98-112), read from the device buffers above
 // Every stage is enqueued on the backbone's stream and runs on the fixed upstream shapes (1000 ROIs, 100 detection rows); nothing waits
 // for the host.  Everything after the GEMMs is IEEE fp32 (fp64 where R-UNMOLD / R-RESIZE say so) in a fixed operation order (this file is
 // compiled -fmad=false) and is reproduced bit for bit by the numpy restatement in tests/heads_ref.py.
@@ -202,6 +204,19 @@ __global__ void k_paste(const float* __restrict__ masks, const int* __restrict__
     out[p] = v;
 }
 
+// hand-off to segmentation (FrameData::mask / classIDs, MaskRCNN.cpp:98-112): 16 id-image bytes per thread into the frame's mask, block 0
+// also writes the header.  An export error left einfo = {0, 1} and an all-zero id image: the frame carries no masks.
+__global__ void k_frame_masks(const uint4* __restrict__ idimg, const int* __restrict__ einfo, const int* __restrict__ ecls, int n16,
+                              uint4* __restrict__ mask, FrameHdr* __restrict__ hdr)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n16) mask[t] = idimg[t];
+    if (blockIdx.x != 0) return;
+    const int err = einfo[1], n = err ? 0 : einfo[0] + 1;
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hdr->classIDs[i] = (i > 0 && i < n) ? ecls[i - 1] : 0;
+    if (threadIdx.x == 0) { hdr->nMasks = n; hdr->detectError = err; }
+}
+
 static int det_fail(const std::string& msg) { cnn_set_error(msg.c_str()); return -1; }
 
 static int check_launch(const char* what)
@@ -250,6 +265,22 @@ static int set_image(mf_detector* h, int W, int H)
     h->imgW = W; h->imgH = H;
     return 0;
 }
+
+namespace mfb {
+cudaStream_t detector_stream(mf_detector* h) { return h->s; }
+
+int detector_reserve_image(mf_detector* h, int W, int H) { return set_image(h, W, H); }
+
+int detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr)
+{
+    const size_t P = (size_t)h->imgW * h->imgH;
+    if (P % 16 || ((uintptr_t)mask & 15)) return det_fail("detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer");
+    const int n16 = (int)(P / 16);
+    prof_mark(h->s, "k_frame_masks");
+    k_frame_masks<<<(n16 + 255) / 256, 256, 0, h->s>>>((const uint4*)h->idimg, h->einfo, h->ecls, n16, (uint4*)mask, hdr);
+    return check_launch("k_frame_masks");
+}
+}  // namespace mfb
 
 static int gemm(mf_detector* h, int layer, const void* A, void* out, int M, int relu, bool f32)
 {

@@ -371,6 +371,7 @@ MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), d
 
 MaskFusion::~MaskFusion()
 {
+    if (detector && bbMoldDone) cudaEventSynchronize(bbMoldDone);     // the last hand-off writes into this context's input set
     cudaStreamSynchronize(stream);
     if (g_prof == &prof) g_prof = nullptr;
     for (cudaEvent_t e : prof.events) cudaEventDestroy(e);
@@ -607,6 +608,9 @@ void MaskFusion::performSegmentation(bool allowNew)
     launch_geometric_edges(vmap[0], nmap[0], W, H, cfg.segWeightDistance, cfg.segWeightConvexity, cfg.segThreshold, edgeMap, edgeBinary, stream);
     launch_morph_close_invert(edgeBinary, edgeBuf, W, H, cfg.segMorphEdgeRadius, cfg.segMorphEdgeIterations, edgeInv, stream);
     launches += 2 + 2 * cfg.segMorphEdgeIterations;
+    // the first readers of the frame's mask and of the header's mask fields: a detector's hand-off must have landed (tracking and the ID
+    // projection above ran next to the detector)
+    if (detWaitPending) { cudaCheck(cudaStreamWaitEvent(stream, bbMoldDone, 0), "cudaStreamWaitEvent"); detWaitPending = false; }
     // ignore map (:221-235)
     launch_person_table(dHdr, personClassID, tblIsPerson, stream);
     launch_apply_ignore(frameMask, tblIsPerson, dHdr, P, ignoreMap, edgeInv, stream);
@@ -687,6 +691,7 @@ int MaskFusion::pickOwner(const int64_t* loads, int world)
 void MaskFusion::configureShard(int rank_, int world_)
 {
     if (world_ < 1 || world_ > 64 || rank_ < 0 || rank_ >= world_) throw CudaError{"configureShard: need 0 <= rank < world <= 64"};
+    if (detector) throw CudaError{"configureShard: a detector is attached; the object-sharded mode does not run one"};
     if (tick != 1) throw CudaError{"configureShard: must be called before the first frame"};
     if (world_ > 1 && !cfg.enableMultipleModels) throw CudaError{"configureShard: a -static run has one model and does not shard (run replicas instead)"};
     rank = rank_; world = world_;
@@ -700,6 +705,7 @@ void MaskFusion::configureShard(int rank_, int world_)
 // communicator of the shards (mf_shard_comm_init): from here on the three exchanges of a frame are NCCL calls on the context's stream
 void MaskFusion::initShardComm(const unsigned char* id128, int rank_, int world_)
 {
+    if (detector) throw CudaError{"initShardComm: a detector is attached; the object-sharded mode does not run one"};
     if (world == 1 && world_ > 1) configureShard(rank_, world_);
     if (rank_ != rank || world_ != world) throw CudaError{"initShardComm: rank / world differ from configureShard"};
     cudaCheck(cudaSetDevice(device), "cudaSetDevice");
@@ -714,11 +720,51 @@ extern "C" void* mf_backbone_stream(struct mf_backbone* h);
 
 void MaskFusion::attachBackbone(void* bb, int everyK)
 {
+    if (bb && detector) throw CudaError{"attachBackbone: a detector is attached (it runs its own backbone on the same stream); detach it first"};
     backbone = bb; backboneEvery = bb ? (everyK > 0 ? everyK : 1) : 0;
     if (bb && !bbFrameReady) {
         cudaCheck(cudaEventCreateWithFlags(&bbFrameReady, cudaEventDisableTiming), "cudaEventCreate");
         cudaCheck(cudaEventCreateWithFlags(&bbMoldDone, cudaEventDisableTiming), "cudaEventCreate");
     }
+}
+
+void MaskFusion::attachDetector(mf_detector* det, int everyK)
+{
+    if (det) {
+        if (!cfg.enableMultipleModels) throw CudaError{"attachDetector: a -static context runs no segmentation to feed"};
+        if (world > 1 || shardNccl) throw CudaError{"attachDetector: the object-sharded mode is not supported (rank 0 would have to detect before the packet broadcast)"};
+        if (backbone) throw CudaError{"attachDetector: a backbone is attached (the detector runs its own backbone on the same stream); detach it first"};
+    }
+    waitDetector();
+    if (det && detector_reserve_image(det, W, H) != 0) throw CudaError{std::string("attachDetector: ") + cnn_last_error()};
+    detector = det; detectorEvery = det ? (everyK > 0 ? everyK : 1) : 0;
+    if (det && !bbFrameReady) {
+        cudaCheck(cudaEventCreateWithFlags(&bbFrameReady, cudaEventDisableTiming), "cudaEventCreate");
+        cudaCheck(cudaEventCreateWithFlags(&bbMoldDone, cudaEventDisableTiming), "cudaEventCreate");
+    }
+}
+
+void MaskFusion::waitDetector()
+{
+    if (detector && bbMoldDone) cudaCheck(cudaEventSynchronize(bbMoldDone), "cudaEventSynchronize");
+}
+
+// MfSegmentation.cpp:128-131: `if (frame->mask.total() == 0) maskRCNN->executeSequential(frame)` on the frames that run segmentation
+// (wanted: tracking frame, no caller mask) and tick % k == 0.  Detection of this frame's RGBA copy, then the hand-off into this frame's
+// input set, both on the detector's stream behind `producer` (which ran the upload, the header and preprocess).  The host never waits.
+void MaskFusion::runDetector(cudaStream_t producer, bool wanted)
+{
+    if (!detector || !wanted || (tick % detectorEvery) != 0) return;
+    if (!producer) producer = stream;
+    cudaStream_t ds = detector_stream(detector);
+    cudaCheck(cudaEventRecord(bbFrameReady, producer), "cudaEventRecord");          // the RGBA copy and the header (nMasks = 0) exist
+    cudaCheck(cudaStreamWaitEvent(ds, bbFrameReady, 0), "cudaStreamWaitEvent");
+    if (mf_detector_detect(detector, rgb, W, H) != 0 || detector_frame_masks(detector, frameMask, dHdr) != 0)
+        throw CudaError{std::string("detector: ") + cnn_last_error()};
+    // one event for both guards: the frame's image has been read and its mask / header written (the input set may be reused), and
+    // segmentation may read them
+    cudaCheck(cudaEventRecord(bbMoldDone, ds), "cudaEventRecord");
+    bbMoldPending = true; detWaitPending = true;
 }
 
 // every k-th frame: RGBA image of this frame -> letter-boxed network input -> backbone forward, all on the backbone's stream
@@ -825,6 +871,7 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
             uploadInputs(rgbIn, depthIn, maskIn, timestamp, onDevice, preStream);
         preprocess(preStream);
         runBackbone(preStream);
+        runDetector(preStream, !maskIn);
         generateCUDATextures(preStream);
         if (cfg.rgbOnly || cfg.icpWeight < 100 || cfg.so3) frameIntensity(preStream);
         cudaCheck(cudaEventRecord(preDone, preStream), "cudaEventRecord");
@@ -843,6 +890,7 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
             uploadInputs(rgbIn, depthIn, maskIn, timestamp, onDevice);     // -static: textureMask stays all zero (MaskFusion.cpp:223-230)
         preprocess();
         runBackbone();
+        runDetector(stream, multi && tracking && !maskIn);
     }
     commOnPre = moverlap && shardNccl;
     Model* g = models[0].get();
@@ -1004,6 +1052,10 @@ void MaskFusion::applyFrameResult()
         nm->age = 1;
     }
     logPoses(R.timestamp);
+    // the frame has been processed without masks; the error surfaces here, with everything else the frame decided already applied
+    if (R.detectError)
+        throw CudaError{"detector: generate_id_image: special_assignments[class_id] out of range (IndexError upstream) on the frame of timestamp " +
+                        std::to_string(R.timestamp) + ", which was processed without masks"};
 }
 
 }  // namespace mfb

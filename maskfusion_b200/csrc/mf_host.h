@@ -185,6 +185,13 @@ public:
     void* backbone = nullptr; int backboneEvery = 0; cudaEvent_t bbFrameReady = nullptr, bbMoldDone = nullptr; bool bbMoldPending = false;
     void attachBackbone(void* bb, int everyK);
     void runBackbone(cudaStream_t producer = nullptr);
+    // Mask R-CNN detector on the frame path (MfSegmentation.cpp:128-131): a segmentation frame that the caller gave no mask runs the
+    // detector every k-th tick on the detector's (= its backbone's) stream; k_frame_masks writes the id image and class list into the
+    // frame's mask / header; the main stream waits (bbMoldDone, recorded behind the hand-off) just before segmentation reads them.
+    mf_detector* detector = nullptr; int detectorEvery = 0; bool detWaitPending = false;
+    void attachDetector(mf_detector* det, int everyK);
+    void runDetector(cudaStream_t producer, bool wanted);
+    void waitDetector();                                        // the host waits for the last hand-off (it writes into an input set)
     // multi-model frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
     bool spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
     FrameResult* hRes = nullptr; DevBuf<FrameResult> dRes; cudaEvent_t resEvt = nullptr; bool pendingResult = false;

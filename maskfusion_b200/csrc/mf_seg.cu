@@ -319,6 +319,7 @@ __global__ void k_vote(const FrameHdr* __restrict__ hdr, VoteParams vp, const in
         }
     }
     res->hasNewLabel = hasNew; res->newClassID = newClass; res->nMasks = nMasks; res->nComponents = (int)*ccCounter + 1; res->timestamp = hdr->timestamp;
+    res->detectError = hdr->detectError;
 }
 __global__ void k_seg_tables(SegTables t, uint8_t* __restrict__ idToIndex, uint8_t* __restrict__ indexToId, uint8_t* __restrict__ isModel)
 {
@@ -328,7 +329,7 @@ __global__ void k_seg_tables(SegTables t, uint8_t* __restrict__ idToIndex, uint8
 __global__ void k_frame_header(FrameHdr h, FrameHdr* __restrict__ d)
 {
     const int i = threadIdx.x;
-    if (i == 0) { d->timestamp = h.timestamp; d->nMasks = h.nMasks; d->pad = 0; }
+    if (i == 0) { d->timestamp = h.timestamp; d->nMasks = h.nMasks; d->detectError = 0; }
     d->classIDs[i] = h.classIDs[i];
 }
 __global__ void k_person_table(const FrameHdr* __restrict__ hdr, int personClassID, uint8_t* __restrict__ isPerson)
