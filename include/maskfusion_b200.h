@@ -21,6 +21,7 @@
  */
 #ifndef MASKFUSION_B200_H
 #define MASKFUSION_B200_H
+#include <stddef.h>
 #include <stdint.h>
 #ifdef __cplusplus
 extern "C" {
@@ -131,8 +132,8 @@ int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k);
  *     mf_set_frame_classes; the detector does not run.
  *   - A failing export rule (special_assignments[class_id] out of range, an IndexError upstream) leaves that frame without masks, and the
  *     NEXT call on the context returns non-zero with the message.
- *   - Refused: a -static context, world > 1, a backbone attached (and mf_attach_backbone while a detector is attached); mf_shard_configure
- *     and mf_shard_comm_init refuse a context with a detector attached.
+ *   - Refused: a -static context, world > 1 (sharded runs use mf_shard_attach_detector), a backbone attached (and mf_attach_backbone while
+ *     a detector is attached); mf_shard_configure and mf_shard_comm_init refuse a context with a detector attached here.
  *   - NULL detaches; detaching and mf_destroy first wait for the last hand-off.  The context never destroys the detector: detach (or destroy
  *     the context) before destroying it.  Detector launches are not counted in mf_kernel_launches. */
 struct mf_detector;
@@ -165,8 +166,18 @@ int mf_model_class_id(mf_context* ctx, int i);                                /*
  *              [frame to every rank]  mf_set_frame_classes; mf_shard_frame_begin;
  *              mf_shard_get_poses -> [all-gather of 64 x 32 floats] -> mf_shard_set_poses;
  *              mf_shard_project -> [MIN all-reduce of the uint64 keys at mf_shard_projection_keys];
+ *              mf_shard_frame_masks -> [if it returns 1: broadcast of the returned device range from the detector rank];
  *              mf_shard_frame_end
- *      With world == 1 the three phase calls are exactly mf_process_frame. ---- */
+ *      With world == 1 the three phase calls are exactly mf_process_frame.
+ *
+ *      Detector (mf_shard_attach_detector): the Mask R-CNN runs on one rank, detector_rank.  A frame exchanges masks when the context
+ *      is multi-model, the frame tracks (tick > 1) and mf_tick() % every_k == 0 -- every rank evaluates this on replicated state.  On such
+ *      a frame the detector rank detects and hands off into its copy of the frame (a caller's mask, sent with the packet, takes
+ *      precedence on the device: the network still runs, its output is dropped), and a fourth exchange broadcasts that rank's
+ *      mask | header (width*height + header bytes) to every rank: in (1) an ncclBroadcast on the context's stream after the key
+ *      all-reduce, in (2) the range mf_shard_frame_masks returns.  Every rank then computes what one process with mf_attach_detector
+ *      and the same every_k computes, bit for bit; an export error of the detector surfaces on every rank on the next call.  New object
+ *      models prefer ranks other than the detector rank (it counts one more tracked model in the placement rule). ---- */
 int mf_shard_configure(mf_context* ctx, int rank, int world);                 /* before the first frame; rank 0 owns the background model */
 int mf_shard_unique_id(uint8_t* out128);                                      /* ncclGetUniqueId (rank 0) */
 int mf_shard_comm_init(mf_context* ctx, const uint8_t* id128, int rank, int world);   /* ncclCommInitRank on the context's device (+ mf_shard_configure) */
@@ -180,6 +191,14 @@ int mf_shard_set_poses(mf_context* ctx, const float* gathered_world_x_64_x32);
 int mf_shard_project(mf_context* ctx);                                        /* device-side lifecycle after tracking + local models into the key image */
 void* mf_shard_projection_keys(mf_context* ctx);                              /* device pointer, width*height uint64 (depth bits << 32 | model index << 26 | surfel) */
 int mf_shard_frame_end(mf_context* ctx, float weight_multiplier);
+/* every rank, between the same frames, with the same every_k and detector_rank; detector non-NULL exactly on detector_rank (where
+ * detector_reserve_image sizes its id image now).  Needs a sharded multi-model context (world > 1: mf_shard_configure or
+ * mf_shard_comm_init first) and no backbone.  (NULL, 0, -1) detaches on every rank; the detector rank first waits for the last hand-off. */
+int mf_shard_attach_detector(mf_context* ctx, struct mf_detector* detector, int every_k, int detector_rank);
+/* phase call of (2), between mf_shard_project and mf_shard_frame_end: 1 and the device range (frame mask | header) to broadcast from the
+ * detector rank when this frame exchanges masks (on the detector rank, the context's stream first waits for the hand-off), else 0.
+ * Always 0 with a communicator: the library broadcasts the range itself. */
+int mf_shard_frame_masks(mf_context* ctx, void** d_ptr, size_t* bytes);
 int mf_model_owner(mf_context* ctx, int i);                                   /* rank holding model i's surfels */
 /* CTAs of the persistent tracking launch per tracked model (host only): bit j of light_mask marks an object model (validity bitmask, nearly all
  * pixels culled), the others are full-frame models and get `ratio` times the share.  Model::performTracking of a batch of models (Model.cpp:427-447)

@@ -60,7 +60,7 @@ EXPORTS = [
     "mf_detector_get_head_outputs", "mf_detector_get_mask_layer", "mf_detector_get_detections", "mf_detector_get_masks", "mf_detector_get_id_image",
     "mf_detector_image_size", "mf_attach_detector", "mf_download_frame_masks",
     "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
-    "mf_shard_projection_keys", "mf_shard_frame_end", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
+    "mf_shard_projection_keys", "mf_shard_frame_end", "mf_shard_attach_detector", "mf_shard_frame_masks", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
 ]
 
 
@@ -197,6 +197,8 @@ def load_library():
     L.mf_shard_project.argtypes = [C.c_void_p]
     L.mf_shard_projection_keys.restype = C.c_void_p; L.mf_shard_projection_keys.argtypes = [C.c_void_p]
     L.mf_shard_frame_end.argtypes = [C.c_void_p, C.c_float]
+    L.mf_shard_attach_detector.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    L.mf_shard_frame_masks.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
     L.mf_model_owner.argtypes = [C.c_void_p, C.c_int]
     L.mf_shard_pick_owner.argtypes = [C.c_void_p, C.c_int]
     _LIB = L

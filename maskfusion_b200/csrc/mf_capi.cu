@@ -466,6 +466,23 @@ extern "C" int mf_shard_set_poses(mf_context* ctx, const float* gathered) { MF_T
 extern "C" int mf_shard_project(mf_context* ctx) { MF_TRY MF_NEED(ctx) ctx->mf->frameProject(); return 0; MF_CATCH(-1) }
 extern "C" void* mf_shard_projection_keys(mf_context* ctx) { if (!ctx || !ctx->mf) return nullptr; return ctx->mf->projKeys.p; }
 extern "C" int mf_shard_frame_end(mf_context* ctx, float weight_multiplier) { MF_TRY MF_NEED(ctx) ctx->mf->frameEnd(weight_multiplier); return 0; MF_CATCH(-1) }
+// Mask R-CNN detector in the object-sharded mode: detection on detector_rank, its mask + header broadcast to every rank on detector frames
+extern "C" int mf_shard_attach_detector(mf_context* ctx, mf_detector* detector, int every_k, int detector_rank)
+{
+    MF_TRY MF_NEED(ctx)
+    ctx->mf->attachShardDetector(detector, every_k, detector_rank); return 0;
+    MF_CATCH(-1)
+}
+extern "C" int mf_shard_frame_masks(mf_context* ctx, void** d_ptr, size_t* bytes)
+{
+    MF_TRY MF_NEED(ctx)
+    if (!d_ptr || !bytes) { g_err = "frame_masks: null output"; return -3; }
+    void* p = nullptr; size_t n = 0;
+    if (!ctx->mf->shardFrameMasks(&p, &n)) return 0;
+    *d_ptr = p; *bytes = n;
+    return 1;
+    MF_CATCH(-1)
+}
 extern "C" int mf_model_owner(mf_context* ctx, int i) { MF_NEED(ctx) MF_MODEL(ctx, i) return m->ownerRank; }
 extern "C" int mf_track_shares(int n_jobs, unsigned light_mask, int total_ctas, int ratio, int* shares)
 {

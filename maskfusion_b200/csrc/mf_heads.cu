@@ -205,10 +205,12 @@ __global__ void k_paste(const float* __restrict__ masks, const int* __restrict__
 }
 
 // hand-off to segmentation (FrameData::mask / classIDs, MaskRCNN.cpp:98-112): 16 id-image bytes per thread into the frame's mask, block 0
-// also writes the header.  An export error left einfo = {0, 1} and an all-zero id image: the frame carries no masks.
+// also writes the header.  An export error left einfo = {0, 1} and an all-zero id image: the frame carries no masks.  A frame the caller
+// gave a mask keeps it (the detector rank of a sharded run detects before it can know; one process never detects such a frame).
 __global__ void k_frame_masks(const uint4* __restrict__ idimg, const int* __restrict__ einfo, const int* __restrict__ ecls, int n16,
                               uint4* __restrict__ mask, FrameHdr* __restrict__ hdr)
 {
+    if (hdr->maskGiven) return;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t < n16) mask[t] = idimg[t];
     if (blockIdx.x != 0) return;

@@ -413,6 +413,7 @@ void MaskFusion::uploadInputs(const uint8_t* rgbIn, const float* depthIn, const 
         // instance masks + their class list ride with the images: the header is a kernel argument (no staging buffer to keep alive)
         FrameHdr h; memset(&h, 0, sizeof h);
         h.timestamp = timestamp;
+        h.maskGiven = maskIn != nullptr;
         if (maskIn && !classIDs.empty()) {
             if (classIDs.size() > 256) throw CudaError{"more than 256 mask labels"};
             cudaCheck(cudaMemcpyAsync(frameMask, maskIn, (size_t)P, kind, s), "mask upload");
@@ -611,6 +612,7 @@ void MaskFusion::performSegmentation(bool allowNew)
     // the first readers of the frame's mask and of the header's mask fields: a detector's hand-off must have landed (tracking and the ID
     // projection above ran next to the detector)
     if (detWaitPending) { cudaCheck(cudaStreamWaitEvent(stream, bbMoldDone, 0), "cudaStreamWaitEvent"); detWaitPending = false; }
+    if (maskCommPending) { cudaCheck(cudaStreamWaitEvent(stream, evComm, 0), "cudaStreamWaitEvent"); maskCommPending = false; }   // sharded: the masks' broadcast
     // ignore map (:221-235)
     launch_person_table(dHdr, personClassID, tblIsPerson, stream);
     launch_apply_ignore(frameMask, tblIsPerson, dHdr, P, ignoreMap, edgeInv, stream);
@@ -665,6 +667,7 @@ Model* MaskFusion::spawnObjectModel()
     // load of a rank = (number of models it tracks, their surfel capacity): every tracked model walks the whole image in the tracker, so
     // the model count dominates; the capacity breaks ties (the background's store is the big one)
     for (auto& m : models) loads[m->ownerRank] += ((int64_t)1 << 32) + m->capacity;
+    if (detRank >= 0) loads[detRank] += (int64_t)1 << 32;          // the network weighs like one more tracked model there
     const int ownerRank = world > 1 ? pickOwner(loads, world) : 0;
     models.emplace_back(new Model(this, getNextModelID(true), cfg.confObject, false, cfg.capacityObject, ownerRank, ownerRank != rank));
     Model* nm = models.back().get();
@@ -691,7 +694,8 @@ int MaskFusion::pickOwner(const int64_t* loads, int world)
 void MaskFusion::configureShard(int rank_, int world_)
 {
     if (world_ < 1 || world_ > 64 || rank_ < 0 || rank_ >= world_) throw CudaError{"configureShard: need 0 <= rank < world <= 64"};
-    if (detector) throw CudaError{"configureShard: a detector is attached; the object-sharded mode does not run one"};
+    if (detector || detRank >= 0)
+        throw CudaError{"configureShard: a detector is attached; detach it, configure the shards, then attach it with mf_shard_attach_detector"};
     if (tick != 1) throw CudaError{"configureShard: must be called before the first frame"};
     if (world_ > 1 && !cfg.enableMultipleModels) throw CudaError{"configureShard: a -static run has one model and does not shard (run replicas instead)"};
     rank = rank_; world = world_;
@@ -705,7 +709,8 @@ void MaskFusion::configureShard(int rank_, int world_)
 // communicator of the shards (mf_shard_comm_init): from here on the three exchanges of a frame are NCCL calls on the context's stream
 void MaskFusion::initShardComm(const unsigned char* id128, int rank_, int world_)
 {
-    if (detector) throw CudaError{"initShardComm: a detector is attached; the object-sharded mode does not run one"};
+    if (detector && detRank < 0)
+        throw CudaError{"initShardComm: a detector is attached to this single process; detach it, then attach it to the shards with mf_shard_attach_detector"};
     if (world == 1 && world_ > 1) configureShard(rank_, world_);
     if (rank_ != rank || world_ != world) throw CudaError{"initShardComm: rank / world differ from configureShard"};
     cudaCheck(cudaSetDevice(device), "cudaSetDevice");
@@ -720,7 +725,7 @@ extern "C" void* mf_backbone_stream(struct mf_backbone* h);
 
 void MaskFusion::attachBackbone(void* bb, int everyK)
 {
-    if (bb && detector) throw CudaError{"attachBackbone: a detector is attached (it runs its own backbone on the same stream); detach it first"};
+    if (bb && (detector || detRank >= 0)) throw CudaError{"attachBackbone: a detector is attached (it runs its own backbone on the same stream); detach it first"};
     backbone = bb; backboneEvery = bb ? (everyK > 0 ? everyK : 1) : 0;
     if (bb && !bbFrameReady) {
         cudaCheck(cudaEventCreateWithFlags(&bbFrameReady, cudaEventDisableTiming), "cudaEventCreate");
@@ -732,7 +737,7 @@ void MaskFusion::attachDetector(mf_detector* det, int everyK)
 {
     if (det) {
         if (!cfg.enableMultipleModels) throw CudaError{"attachDetector: a -static context runs no segmentation to feed"};
-        if (world > 1 || shardNccl) throw CudaError{"attachDetector: the object-sharded mode is not supported (rank 0 would have to detect before the packet broadcast)"};
+        if (world > 1 || shardNccl) throw CudaError{"attachDetector: this context is one rank of an object-sharded run; attach the detector on every rank with mf_shard_attach_detector"};
         if (backbone) throw CudaError{"attachDetector: a backbone is attached (the detector runs its own backbone on the same stream); detach it first"};
     }
     waitDetector();
@@ -747,6 +752,44 @@ void MaskFusion::attachDetector(mf_detector* det, int everyK)
 void MaskFusion::waitDetector()
 {
     if (detector && bbMoldDone) cudaCheck(cudaEventSynchronize(bbMoldDone), "cudaEventSynchronize");
+}
+
+// every rank of a sharded run, between the same frames, with the same everyK / detectorRank; det on detectorRank only.
+// (NULL, 0, -1) detaches on every rank.
+void MaskFusion::attachShardDetector(mf_detector* det, int everyK, int detectorRank)
+{
+    if (!det && everyK == 0 && detectorRank == -1) {
+        if (detRank < 0) return;
+        waitDetector();
+        detector = nullptr; detectorEvery = 0; detRank = -1;
+        return;
+    }
+    if (!cfg.enableMultipleModels) throw CudaError{"shard_attach_detector: a -static context runs no segmentation to feed"};
+    if (world == 1) throw CudaError{"shard_attach_detector: not a sharded context (world == 1); call mf_shard_configure or mf_shard_comm_init first, or use mf_attach_detector for one process"};
+    if (detectorRank < 0 || detectorRank >= world)
+        throw CudaError{"shard_attach_detector: detector_rank " + std::to_string(detectorRank) + " outside [0, " + std::to_string(world) + ")"};
+    if (det && rank != detectorRank)
+        throw CudaError{"shard_attach_detector: a detector was given on rank " + std::to_string(rank) + ", which is not the detector rank " + std::to_string(detectorRank)};
+    if (!det && rank == detectorRank) throw CudaError{"shard_attach_detector: no detector given on the detector rank " + std::to_string(detectorRank)};
+    if (backbone) throw CudaError{"shard_attach_detector: a backbone is attached (the detector runs its own backbone on the same stream); detach it first"};
+    waitDetector();
+    if (det && detector_reserve_image(det, W, H) != 0) throw CudaError{std::string("shard_attach_detector: ") + cnn_last_error()};
+    detector = det; detectorEvery = everyK > 0 ? everyK : 1; detRank = detectorRank;
+    if (det && !bbFrameReady) {
+        cudaCheck(cudaEventCreateWithFlags(&bbFrameReady, cudaEventDisableTiming), "cudaEventCreate");
+        cudaCheck(cudaEventCreateWithFlags(&bbMoldDone, cudaEventDisableTiming), "cudaEventCreate");
+    }
+}
+
+// external transport (no communicator), between frameProject and frameEnd: on a mask-exchange frame, the detector rank's stream first
+// waits for the hand-off; the caller then broadcasts [frameMask, +P + sizeof(FrameHdr)) from detRank.  With a communicator the library
+// issues that broadcast itself, and there is nothing for the caller to move.
+bool MaskFusion::shardFrameMasks(void** ptr, size_t* bytes)
+{
+    if (shardNccl || !fExchange) return false;
+    if (detWaitPending) { cudaCheck(cudaStreamWaitEvent(stream, bbMoldDone, 0), "cudaStreamWaitEvent"); detWaitPending = false; }
+    *ptr = frameMask; *bytes = (size_t)P + sizeof(FrameHdr);
+    return true;
 }
 
 // MfSegmentation.cpp:128-131: `if (frame->mask.total() == 0) maskRCNN->executeSequential(frame)` on the frames that run segmentation
@@ -837,6 +880,10 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
     finalisePending();                                  // previous frame: tracked poses, pose log, (multi) inactivations and the deferred spawn
     fTimestamp = timestamp; fHasPose = inPose != nullptr; if (inPose) fInPose = *inPose; fBootstrap = bootstrap;
     const bool tracking = tick > 1 && (bootstrap || !inPose);
+    fExchange = detRank >= 0 && multi && tracking && tick % detectorEvery == 0;
+    // one process: the caller's mask decides on the host; sharded: the detector rank detects on every exchange frame and k_frame_masks
+    // keeps a caller's mask (FrameHdr::maskGiven), which only rank 0 has seen
+    const bool detWanted = detRank >= 0 ? fExchange : multi && tracking && !maskIn;
     // -static tracking frames: upload + bilateral + pyramids + maps + intensity/Sobel of THIS frame go to preStream and into the other
     // input set, so they run next to the surfel passes of the previous frame that are still queued on the main stream (those read the
     // previous frame's images; the copy engine and the issue-bound bilateral overlap well with the HBM-bound clean/scatter).
@@ -871,7 +918,7 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
             uploadInputs(rgbIn, depthIn, maskIn, timestamp, onDevice, preStream);
         preprocess(preStream);
         runBackbone(preStream);
-        runDetector(preStream, !maskIn);
+        runDetector(preStream, detWanted);
         generateCUDATextures(preStream);
         if (cfg.rgbOnly || cfg.icpWeight < 100 || cfg.so3) frameIntensity(preStream);
         cudaCheck(cudaEventRecord(preDone, preStream), "cudaEventRecord");
@@ -890,7 +937,7 @@ void MaskFusion::frameBegin(const uint8_t* rgbIn, const float* depthIn, int64_t 
             uploadInputs(rgbIn, depthIn, maskIn, timestamp, onDevice);     // -static: textureMask stays all zero (MaskFusion.cpp:223-230)
         preprocess();
         runBackbone();
-        runDetector(stream, multi && tracking && !maskIn);
+        runDetector(stream, detWanted);
     }
     commOnPre = moverlap && shardNccl;
     Model* g = models[0].get();
@@ -967,6 +1014,15 @@ void MaskFusion::frameEnd(float weightMultiplier)
                         cudaCheck(cudaEventRecord(evComm, preStream), "cudaEventRecord"); cudaCheck(cudaStreamWaitEvent(stream, evComm, 0), "cudaStreamWaitEvent");
                     } else
                         shard.allReduceMinU64(projKeys, (size_t)P, stream);
+                    if (fExchange) {
+                        // detector frame: the detector rank's mask and header replace every rank's (a caller's mask travels back unchanged).
+                        // The main stream waits for it only where segmentation first reads the mask.
+                        prof_mark(stream, "nccl_broadcast_masks");
+                        cudaStream_t cs = commOnPre ? preStream : stream;
+                        if (detWaitPending) { cudaCheck(cudaStreamWaitEvent(cs, bbMoldDone, 0), "cudaStreamWaitEvent"); detWaitPending = false; }
+                        shard.broadcast(frameMask, (size_t)P + sizeof(FrameHdr), detRank, cs);
+                        if (commOnPre) { cudaCheck(cudaEventRecord(evComm, preStream), "cudaEventRecord"); maskCommPending = true; }
+                    }
                 }
                 segTables();
                 projectResolve();

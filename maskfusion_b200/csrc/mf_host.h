@@ -160,11 +160,12 @@ public:
     Model* spawnObjectModel();                                                                    // MaskFusion::spawnObjectModel + moveNewModelToList
     void setFrameClasses(const int32_t* ids, int n) { classIDs.assign(ids, ids + n); }            // FrameData::classIDs
 
-    // ---- a frame in three phases; between them sit the two exchanges of the object-sharded mode (SURVEY 8e):
+    // ---- a frame in three phases; between them sit the exchanges of the object-sharded mode (SURVEY 8e):
     //   frameBegin  inputs (+ frame-packet broadcast), preprocessing, tracking of the models whose store lives here, pose rows
     //   [pose-row all-gather]
     //   frameProject  device-side lifecycle (inactivation, static poses), local part of the global ID projection
     //   [64-bit MIN all-reduce of the projection keys]
+    //   [detector frames: broadcast of frameMask | FrameHdr from the detector rank]
     //   frameEnd  resolve, segmentation + vote (device driven), FrameResult copy, fusion of the local stores, prediction
     // With an NCCL communicator (initShardComm) the exchanges are issued from here on the context's stream and NOTHING in a frame
     // waits for the host; without one the caller moves the rows / keys itself between the phase calls (any transport: the gloo tests).
@@ -192,6 +193,13 @@ public:
     void attachDetector(mf_detector* det, int everyK);
     void runDetector(cudaStream_t producer, bool wanted);
     void waitDetector();                                        // the host waits for the last hand-off (it writes into an input set)
+    // object-sharded run with a detector (mf_shard_attach_detector): `detector` is set on rank detRank only, detectorEvery on every rank.
+    // A frame exchanges masks (fExchange) when detRank >= 0, the context is multi-model, the frame tracks and tick % detectorEvery == 0:
+    // replicated host state, so every rank issues the same collectives.  The detector rank then runs the detector whatever the caller
+    // passed (the mask exists on rank 0 only; FrameHdr::maskGiven keeps it on the device) and its frameMask | FrameHdr goes to every rank.
+    int detRank = -1; bool fExchange = false, maskCommPending = false;
+    void attachShardDetector(mf_detector* det, int everyK, int detectorRank);
+    bool shardFrameMasks(void** ptr, size_t* bytes);            // external transport: the range to broadcast from detRank on this frame
     // multi-model frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
     bool spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
     FrameResult* hRes = nullptr; DevBuf<FrameResult> dRes; cudaEvent_t resEvt = nullptr; bool pendingResult = false;

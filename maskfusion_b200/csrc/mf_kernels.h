@@ -93,7 +93,9 @@ __device__ inline void derivePose(DevPose* d, const float* m, const float* last)
 // FrameHdr: what the loader knows about the frame besides the images; in the object-sharded mode it is the tail of the broadcast
 // frame packet, so the ranks that never saw the host inputs read it where the kernels read it: on the device.
 // detectError: the attached detector's export rule failed on this frame (special_assignments[class_id] out of range), which then carries no masks
-struct FrameHdr { long long timestamp; int nMasks; int detectError; int classIDs[256]; };   // nMasks == 0: the frame carries no instance masks
+// maskGiven: the caller passed a mask with the frame; the detector's hand-off (k_frame_masks) then leaves mask and header alone.  It travels
+// in the packet because a sharded run's detector rank may not be the rank that received the caller's inputs.
+struct FrameHdr { long long timestamp; int nMasks; int detectError; int classIDs[256]; int maskGiven; };   // nMasks == 0: the frame carries no instance masks
 // FrameResult: everything the host learns from a frame (one asynchronous copy behind the vote kernel; read at the START of the next
 // frame): the spawn decision of MfSegmentation, which tracked models jumped > 0.2 m (MaskFusion.cpp:268-272), every model's pose,
 // the header's detectError.

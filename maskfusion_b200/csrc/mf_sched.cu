@@ -8,7 +8,8 @@
 //                                  wants to know in a FrameResult that is copied back asynchronously and read at the start of the NEXT frame.
 //   NcclApi / ShardComm         <- SURVEY 8(e): the three couplings between object models of a frame as NCCL collectives issued from
 //                                  inside the library on the context's stream (frame packet broadcast, pose-row all-gather, 64-bit MIN
-//                                  all-reduce of the ID-projection keys).  libnccl is opened at run time (dlopen: the same copy torch has
+//                                  all-reduce of the ID-projection keys), plus, on detector frames of a run with a detector rank, the
+//                                  broadcast of that rank's frame mask and header.  libnccl is opened at run time (dlopen: the same copy torch has
 //                                  already mapped, if any); a process that never shards never needs it.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
@@ -135,7 +136,7 @@ void ShardComm::init(const unsigned char* id128, int rank_, int world_)
 }
 void ShardComm::broadcast(void* buf, size_t bytes, int root, cudaStream_t s)
 {
-    ncclCheck(nccl().Broadcast(buf, buf, bytes, ncclUint8, root, (ncclComm_t)comm, s), "ncclBroadcast (frame packet)");
+    ncclCheck(nccl().Broadcast(buf, buf, bytes, ncclUint8, root, (ncclComm_t)comm, s), "ncclBroadcast (frame packet / frame masks)");
     bytesMoved += bytes; ++calls;
 }
 void ShardComm::allGatherFloats(const float* send, float* recv, size_t countPerRank, cudaStream_t s)

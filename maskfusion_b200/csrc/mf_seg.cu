@@ -329,7 +329,7 @@ __global__ void k_seg_tables(SegTables t, uint8_t* __restrict__ idToIndex, uint8
 __global__ void k_frame_header(FrameHdr h, FrameHdr* __restrict__ d)
 {
     const int i = threadIdx.x;
-    if (i == 0) { d->timestamp = h.timestamp; d->nMasks = h.nMasks; d->detectError = 0; }
+    if (i == 0) { d->timestamp = h.timestamp; d->nMasks = h.nMasks; d->detectError = 0; d->maskGiven = h.maskGiven; }
     d->classIDs[i] = h.classIDs[i];
 }
 __global__ void k_person_table(const FrameHdr* __restrict__ hdr, int personClassID, uint8_t* __restrict__ isPerson)

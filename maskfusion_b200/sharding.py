@@ -5,6 +5,7 @@ Per frame the ranks exchange exactly what couples the models in the reference:
   frame in          rgb + depth + instance mask + class ids, broadcast from the loader rank     (MaskFusion.cpp:212-217)
   poses             every tracked model's pose / last transform, all-gather                      (MaskFusion.cpp:257-276)
   ID projection     64-bit (depth bits << 32 | model index << 26 | surfel) keys, all-reduce MIN  (GlobalProjection.cpp:66-95)
+  masks             with a detector rank (attachDetector), on detector frames: that rank's frame mask + header, broadcast
 
 Everything after the merged key image (segmentation, mask<->model voting, spawn decision, inactivation) is a
 deterministic function of replicated inputs and is evaluated on every rank; the surfel passes (index map,
@@ -141,6 +142,7 @@ class ShardedMaskFusion:
         self.W, self.H = cfg.width, cfg.height
         self.P = self.W * self.H
         self.bytes_collective = 0
+        self.det_rank = -1
         if self.on_nccl:
             uid = torch.zeros(128, dtype=torch.uint8)
             if self.rank == 0:
@@ -179,6 +181,18 @@ class ShardedMaskFusion:
         allreduce_min_u64(k, self.group)
         self.keys.copy_(k)
         self.bytes_collective += self.P * 8
+
+    def _exchange_masks(self):
+        """detector frames: the detector rank's frame mask | header to every rank (mf_shard_frame_masks says when and where)"""
+        ptr, n = C.c_void_p(), C.c_size_t()
+        if not self.mf._ck(self.L.mf_shard_frame_masks(self.h, C.byref(ptr), C.byref(n))):
+            return
+        tail = self.torch.as_tensor(_DevPtr(ptr.value, n.value, "|u1"), device=self.dev)
+        host = tail.cpu()
+        src = self.det_rank if self.group is None else self.dist.get_global_rank(self.group, self.det_rank)
+        self.dist.broadcast(host, src=src, group=self.group)
+        tail.copy_(host)
+        self.bytes_collective += n.value
 
     # -- one frame --
     def processFrame(self, rgb=None, depth=None, timestamp: int = 0, mask=None, classIDs=None, weightMultiplier: float = 1.0):
@@ -225,8 +239,28 @@ class ShardedMaskFusion:
         ck(L.mf_shard_project(h))
         if self.mf.cfg.enableMultipleModels and self.mf.getTick() > 1:
             self._merge_keys()
+        self._exchange_masks()
         ck(L.mf_shard_frame_end(h, float(weightMultiplier)))
         return False
+
+    # -- Mask R-CNN on one rank --
+    def attachDetector(self, detector, every_k: int = 1, rank: int | None = None):
+        """every rank, between the same frames: the detector runs on `rank` (default world - 1: rank 0 already carries the loader and the
+        background model) every k-th tracking frame, and its masks reach every rank.  `detector` is ignored, and may be None, on the
+        other ranks.  The shards then compute what one MaskFusion with attachDetector(detector, every_k) computes."""
+        r = self.world - 1 if rank is None else int(rank)
+        d = C.c_void_p(detector.h) if detector is not None and self.rank == r else None
+        self.mf._ck(self.L.mf_shard_attach_detector(self.h, d, int(every_k), r))
+        self.det_rank = r
+
+    def detachDetector(self):
+        """every rank, between the same frames; the detector rank first waits for the last hand-off"""
+        self.mf._ck(self.L.mf_shard_attach_detector(self.h, None, 0, -1))
+        self.det_rank = -1
+
+    def frameMasks(self):
+        """-> (mask, class ids) that segmentation read on the last frame: the same on every rank"""
+        return self.mf.frameMasks()
 
     def stats(self):
         """-> dict(bytes, calls, nranks, nccl_version): collectives issued by the library (NCCL path) or by this class (staged path)"""
