@@ -422,20 +422,28 @@ MF_D double shflXorD(double v, int m)
 {
     return __hiloint2double(__shfl_xor_sync(0xffffffffu, __double2hiint(v), m), __shfl_xor_sync(0xffffffffu, __double2loint(v), m));
 }
+// One halving step: H is a template parameter so that the value loop has a constant trip count when it is unrolled.  (With
+// h = 16 >> s of an enclosing unrolled loop, the inner loop is unrolled first, while its trip count is still unknown: it stayed a runtime
+// loop, v[] was indexed dynamically and lived in local memory -- about 70 local loads and stores per reduction on sm_90a.)
+template <int H>
+MF_D void warpHalvingStep(double* v, int lane)
+{
+    const bool up = (lane & H) != 0;
+#pragma unroll
+    for (int k = 0; k < H; ++k) {
+        double keep = up ? v[k + H] : v[k];
+        double send = up ? v[k] : v[k + H];
+        v[k] = keep + shflXorD(send, H);
+    }
+}
 MF_D void warpReduceHalving32(double* v)
 {
     const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int s = 0; s < 5; ++s) {
-        const int off = 16 >> s, h = 16 >> s;
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-            double keep = up ? v[k + h] : v[k];
-            double send = up ? v[k] : v[k + h];
-            v[k] = keep + shflXorD(send, off);
-        }
-    }
+    warpHalvingStep<16>(v, lane);
+    warpHalvingStep<8>(v, lane);
+    warpHalvingStep<4>(v, lane);
+    warpHalvingStep<2>(v, lane);
+    warpHalvingStep<1>(v, lane);
 }
 
 // ---- flagged exchange of the partial rows (the LL scheme of collective libraries) ----
@@ -796,7 +804,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                 double kr[3];
 #pragma unroll
                 for (int q = 0; q < 3; ++q) kr[q] = so3K[r * 3] * st->resultR[q] + so3K[r * 3 + 1] * st->resultR[3 + q] + so3K[r * 3 + 2] * st->resultR[6 + q];
-                so3Krlr[threadIdx.x] = (float)kr[cc];
+                so3Krlr[threadIdx.x] = (float)(cc == 0 ? kr[0] : cc == 1 ? kr[1] : kr[2]);     // constant indices: kr[] stays in registers
                 so3B[threadIdx.x] = (float)(kr[0] * so3KinvD[cc] + kr[1] * so3KinvD[3 + cc] + kr[2] * so3KinvD[6 + cc]);
             }
             __syncthreads();
