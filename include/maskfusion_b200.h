@@ -213,9 +213,22 @@ int mf_debug_set_poses(mf_context* ctx, int i, const float pose16[16], const flo
 int mf_icp_step(mf_context* ctx, int i, int level, const float Rcurr9[9], const float tcurr3[3], float out29[29]);  /* icpStep, reduce.cu:446-525 */
 
 /* ---- Mask R-CNN backbone: ResNet-101 + FPN as wgmma GEMMs (replaces the dense part of the Keras/TF sidecar,
- *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded: no COCO weights offline) ---- */
+ *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded unless loaded with mf_*_load_weights) ---- */
 typedef struct mf_backbone mf_backbone;
 const char* mf_cnn_last_error(void);
+/* Pretrained weights (the reference's model.load_weights(COCO_MODEL_PATH, by_name=True)): a safetensors file of matterport's Keras
+ * arrays named "<layer>/<param>", F32, Keras layouts (scripts/convert_mrcnn_h5.py writes it from mask_rcnn_coco.h5; DESIGN §3c has the
+ * name table).  BatchNorm is folded on the host (R-FOLD).  Each loader reads its own handle's tensors and ignores the others; all or
+ * nothing: everything is read, checked and folded before the handle changes, and on an error (mf_cnn_last_error() names the file and the
+ * tensor) its weights stay as they were.  The copy is ordered on the handle's stream after the work queued there, and complete on
+ * return: safe between frames with the detector attached; mf_*_get_weights read the new tables afterwards.  mf_rpn_load_weights and
+ * mf_detector_load_weights are declared with their handles below. */
+int mf_backbone_load_weights(mf_backbone* h, const char* path);
+/* one handle layer exactly as the loaders fold it, on the host (no CUDA device needed): w [rows x K] (K order (ky, kx, cin), zero padded),
+ * bias [rows]; dims = {rows, K}.  Layer names: the Keras conv layer ("conv1", "res4b_branch2a", "fpn_c3p3", "fpn_p2", "rpn_conv_shared",
+ * "mrcnn_class_conv1", "mrcnn_mask_conv2", "mrcnn_mask_deconv", "mrcnn_mask", ...) or the stacked pairs "rpn_class_raw+rpn_bbox_pred"
+ * and "mrcnn_class_logits+mrcnn_bbox_fc".  w or bias NULL: only dims, the file is not read. */
+int mf_mrcnn_read_layer(const char* path, const char* layer, float* w_rows_K, float* bias_rows, int* dims);
 /* out[MxN] = relu?(A[MxK] * B[NxK]^T + bias[N] + residual[MxN]); bf16 device pointers, K % 64 == 0, N % 64 == 0 */
 int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, const void* dResidual, void* dOut, int M, int N, int K, int relu, void* stream);
 /* implicit-GEMM 3x3/s1/p1 convolution, NHWC bf16, weights [Cout][3][3][Cin]; the activation is read through a 3-D TMA map (no im2col) */
@@ -235,7 +248,7 @@ double mf_backbone_flops(mf_backbone* h);
 int mf_backbone_num_gemms(mf_backbone* h);
 
 /* ---- Mask R-CNN region proposals on the backbone's P2..P6 (matterport mrcnn rpn_graph + ProposalLayer + PyramidROIAlign, COCO
- *      InferenceConfig; weights synthetic/seeded and owned by the handle, not by the backbone's layer table).  The handle reads the
+ *      InferenceConfig; weights synthetic/seeded unless loaded, owned by the handle, not by the backbone's layer table).  The handle reads the
  *      backbone's outputs and enqueues on the backbone's stream; destroy it before the backbone.  Errors: mf_cnn_last_error().
  *      Anchors: 3 per feature pixel (ratios 0.5, 1, 2), order (level P2..P6, y, x, ratio), normalised y1 x1 y2 x2; A anchors in all.
  *      Boxes are normalised y1 x1 y2 x2 float; pooled features are [n][pool][pool][256] bf16. ---- */
@@ -245,6 +258,7 @@ typedef struct mf_rpn mf_rpn;
 #define MF_RPN_PROPOSALS 4     /* top 6000 by score, decode + clip, NMS 0.7 -> 1000 proposals (zero padded) and the kept count */
 #define MF_RPN_ROI_ALIGN 8     /* 7x7 ROI Align of the 1000 proposals */
 mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed);
+int mf_rpn_load_weights(mf_rpn* h, const char* path);          /* rpn_conv_shared, rpn_class_raw, rpn_bbox_pred (see mf_backbone_load_weights) */
 void mf_rpn_destroy(mf_rpn* h);
 int mf_rpn_forward(mf_rpn* h);                        /* all four stages, after mf_backbone_forward on the same stream */
 int mf_rpn_run(mf_rpn* h, int stages);                /* a subset of the stages (MF_RPN_* bits), in order */
@@ -262,7 +276,7 @@ int mf_rpn_get_proposals(mf_rpn* h, float* rois_1000x4);                        
 int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16_1000x7x7x256);
 
 /* ---- Mask R-CNN detection heads on an mf_rpn's proposals (matterport mrcnn fpn_classifier_graph + DetectionLayer + build_fpn_mask_graph +
- *      unmold_detections + generate_id_image, COCO InferenceConfig: 81 classes; weights synthetic/seeded and owned by the handle).  The handle
+ *      unmold_detections + generate_id_image, COCO InferenceConfig: 81 classes; weights synthetic/seeded unless loaded, owned by the handle).  The handle
  *      reads the RPN's proposals and pooled features and the backbone's P2..P5, and enqueues on the backbone's stream; destroy it before the
  *      RPN.  Errors: mf_cnn_last_error().  Shapes are the upstream ones: 1000 ROIs, 100 detection rows.  Detections are [100][6] float
  *      y1 x1 y2 x2 (normalised to the S x S network input, clipped to the letter-box window of the image) class score, zero rows after the
@@ -274,6 +288,7 @@ typedef struct mf_detector mf_detector;
 #define MF_DET_MASKS 4         /* 14x14 ROI Align of the detections, 4 x 3x3 conv, 2x2/s2 transposed conv, 1x1 logits, own-class sigmoid */
 #define MF_DET_ID_IMAGE 8      /* unmould to image pixels + generate_id_image (export rule of mf_detector_set_export) -> id image, ids, rois */
 mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed);
+int mf_detector_load_weights(mf_detector* h, const char* path);  /* mrcnn_class_*, mrcnn_bbox_fc, mrcnn_mask* (see mf_backbone_load_weights) */
 void mf_detector_destroy(mf_detector* h);
 int mf_detector_run(mf_detector* h, int stages);                  /* a subset of the stages (MF_DET_* bits), in order */
 int mf_detector_forward(mf_detector* h, int image_w, int image_h); /* all stages after mf_rpn_forward, for an image of image_w x image_h */

@@ -59,6 +59,7 @@ EXPORTS = [
     "mf_detector_refine", "mf_detector_paste", "mf_detector_num_layers", "mf_detector_layer", "mf_detector_get_weights", "mf_detector_get_fc",
     "mf_detector_get_head_outputs", "mf_detector_get_mask_layer", "mf_detector_get_detections", "mf_detector_get_masks", "mf_detector_get_id_image",
     "mf_detector_image_size", "mf_attach_detector", "mf_download_frame_masks",
+    "mf_backbone_load_weights", "mf_rpn_load_weights", "mf_detector_load_weights", "mf_mrcnn_read_layer",
     "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
     "mf_shard_projection_keys", "mf_shard_frame_end", "mf_shard_attach_detector", "mf_shard_frame_masks", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
 ]
@@ -185,6 +186,9 @@ def load_library():
     L.mf_detector_get_id_image.argtypes = [C.c_void_p] * 4
     L.mf_detector_image_size.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.mf_attach_detector.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    for name in ("mf_backbone_load_weights", "mf_rpn_load_weights", "mf_detector_load_weights"):
+        getattr(L, name).argtypes = [C.c_void_p, C.c_char_p]
+    L.mf_mrcnn_read_layer.argtypes = [C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.mf_download_frame_masks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
     L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.mf_shard_frame_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
@@ -638,7 +642,8 @@ def write_klg(path: str, timestamps, depth_mm: np.ndarray, rgb: np.ndarray):
 
 
 class Backbone:
-    """Mask R-CNN ResNet-101-FPN backbone on wgmma GEMMs (csrc/mf_cnn.cu).  Weights are synthetic (seeded)."""
+    """Mask R-CNN ResNet-101-FPN backbone on wgmma GEMMs (csrc/mf_cnn.cu).  Weights are synthetic (seeded) unless loaded with
+    loadWeights (matterport's Keras arrays in a safetensors file, BatchNorm folded; see load_mask_rcnn)."""
 
     def __init__(self, input_size=1024, seed=1, stream: int | None = None):
         self.L = load_library()
@@ -664,6 +669,12 @@ class Backbone:
         w = np.zeros((cout, kpad), np.float32); b = np.zeros(cout, np.float32)
         self.L.mf_backbone_get_weights(self.h, i, _p(w), _p(b))
         return w[:, :k * k * cin].reshape(cout, k, k, cin), b
+
+    def loadWeights(self, path: str):
+        """the backbone's tensors of a safetensors weight file (conv1, res*, bn*, fpn_*); all or nothing, complete on return"""
+        if self.L.mf_backbone_load_weights(self.h, os.fsencode(path)) != 0:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+        return self
 
     def forward(self, input_ptr: int):
         if self.L.mf_backbone_forward(self.h, C.c_void_p(input_ptr)) != 0:
@@ -694,8 +705,8 @@ def _bf16_to_f32(raw: np.ndarray) -> np.ndarray:
 
 
 class RegionProposals:
-    """Mask R-CNN RPN head + proposal layer + pyramid ROI Align on a Backbone's P2..P6 (csrc/mf_rpn.cu).  Weights are synthetic (seeded).
-    Runs on the backbone's stream; close it before the backbone."""
+    """Mask R-CNN RPN head + proposal layer + pyramid ROI Align on a Backbone's P2..P6 (csrc/mf_rpn.cu).  Weights are synthetic (seeded)
+    unless loaded with loadWeights.  Runs on the backbone's stream; close it before the backbone."""
 
     POST_NMS, POOL, CHANNELS = 1000, 7, 256
     CONV, HEADS, PROPOSALS, ROI_ALIGN = 1, 2, 4, 8        # stage bits of run()
@@ -763,6 +774,11 @@ class RegionProposals:
         self._ck(self.L.mf_rpn_get_weights(self.h, _p(cw), _p(cb), _p(hw), _p(hb)))
         return cw, cb, hw, hb
 
+    def loadWeights(self, path: str):
+        """rpn_conv_shared, rpn_class_raw and rpn_bbox_pred of a safetensors weight file; all or nothing, complete on return"""
+        self._ck(self.L.mf_rpn_load_weights(self.h, os.fsencode(path)))
+        return self
+
     def propose(self, logits_ptr: int, deltas_ptr: int, anchors_ptr: int, n: int):
         """the proposal stage on caller-supplied device arrays (float32 [n, 2], [n, 4], [n, 4]); results through proposals()"""
         self._ck(self.L.mf_rpn_propose(self.h, C.c_void_p(logits_ptr), C.c_void_p(deltas_ptr), C.c_void_p(anchors_ptr), int(n)))
@@ -778,7 +794,8 @@ def roi_align(backbone: Backbone, boxes_ptr: int, n: int, pool: int, out_ptr: in
 
 class Detector:
     """Mask R-CNN detection heads on a RegionProposals' proposals (csrc/mf_heads.cu): classifier, detection layer, mask head, unmould and
-    generate_id_image.  Weights are synthetic (seeded).  Runs on the backbone's stream; close it before the RegionProposals."""
+    generate_id_image.  Weights are synthetic (seeded) unless loaded with loadWeights.  Runs on the backbone's stream; close it before the
+    RegionProposals."""
 
     ROIS, MAX_DETECTIONS, NUM_CLASSES, MASK = 1000, 100, 81, 28
     CLASSIFIER, DETECTIONS, MASKS, ID_IMAGE = 1, 2, 4, 8        # stage bits of run()
@@ -840,6 +857,12 @@ class Detector:
         self._ck(self.L.mf_detector_get_weights(self.h, int(i), _p(w), _p(b)))
         return w, b
 
+    def loadWeights(self, path: str):
+        """mrcnn_class_*, mrcnn_bbox_fc and mrcnn_mask* of a safetensors weight file; all or nothing, complete on return (also between
+        frames while the detector is attached to a context)"""
+        self._ck(self.L.mf_detector_load_weights(self.h, os.fsencode(path)))
+        return self
+
     def fcOutputs(self):
         """FC1 and FC2 outputs [1000, 1024] as float32 (bf16 values)"""
         a = np.zeros((self.ROIS, 1024), np.uint16); b = np.zeros((self.ROIS, 1024), np.uint16)
@@ -896,3 +919,33 @@ class Detector:
         out = self.idImage()                      # waits for the stream, so the upload outlives its use
         del rgba
         return out
+
+
+def load_mask_rcnn(path: str, input_size: int = 1024, stream: int | None = None):
+    """the reference's model.load_weights(COCO_MODEL_PATH, by_name=True): a Backbone, RegionProposals and Detector on `stream` with the
+    weights of a safetensors file (scripts/convert_mrcnn_h5.py converts matterport's mask_rcnn_coco.h5) -> (backbone, rpn, detector).
+    Close them in the reverse order."""
+    made = []
+    try:
+        made.append(Backbone(input_size, stream=stream).loadWeights(path))
+        made.append(RegionProposals(made[0]).loadWeights(path))
+        made.append(Detector(made[1]).loadWeights(path))
+    except BaseException:
+        for h in reversed(made):
+            h.close()
+        raise
+    return tuple(made)
+
+
+def read_mrcnn_layer(path: str, layer: str):
+    """one handle layer as the loaders fold it, on the host (no CUDA device): -> (weights [rows, K], bias [rows]), float32, zero padded.
+    layer: a Keras conv layer name ("conv1", "res3a_branch2b", "fpn_p2", "mrcnn_mask_deconv", ...) or one of the stacked pairs
+    "rpn_class_raw+rpn_bbox_pred", "mrcnn_class_logits+mrcnn_bbox_fc" (include/maskfusion_b200.h, mf_mrcnn_read_layer)"""
+    L = load_library()
+    dims = np.zeros(2, np.int32)
+    if L.mf_mrcnn_read_layer(os.fsencode(path), layer.encode(), None, None, _p(dims)) != 0:
+        raise MFError(L.mf_cnn_last_error().decode())
+    w = np.zeros((int(dims[0]), int(dims[1])), np.float32); b = np.zeros(int(dims[0]), np.float32)
+    if L.mf_mrcnn_read_layer(os.fsencode(path), layer.encode(), _p(w), _p(b), _p(dims)) != 0:
+        raise MFError(L.mf_cnn_last_error().decode())
+    return w, b

@@ -42,6 +42,7 @@ SOURCES = {
     "mf_cnn.cu": [],                      # tensor-core GEMMs: no bit-exactness contract, FMA contraction on
     "mf_rpn.cu": ["-fmad=false"],         # proposal layer + ROI Align: bit-exact against the numpy restatement (the GEMMs live in mf_cnn.cu)
     "mf_heads.cu": ["-fmad=false"],       # detection layer, mask select, unmould + id image: bit-exact against the numpy restatement
+    "mf_weights.cu": ["-Xcompiler", "-ffp-contract=off"],   # host code only: safetensors weights, R-FOLD bit-exact against numpy
 }
 
 

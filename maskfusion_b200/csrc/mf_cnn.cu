@@ -613,6 +613,34 @@ extern "C" int mf_backbone_get_weights(mf_backbone* h, int i, float* w, float* b
     return 0;
 }
 
+// pretrained weights (mf_weights.cu): every layer is read, checked and folded on the host before the device tables change; the copy is
+// ordered on the handle's stream and complete on return
+extern "C" int mf_backbone_load_weights(mf_backbone* h, const char* path)
+{
+    if (!h) { g_cnn_err = "backbone: null handle"; return -1; }
+    Backbone* b = &h->b;
+    const int n = (int)b->layers.size();
+    if (mrcnn_layer_count(MRCNN_BACKBONE) != n) { g_cnn_err = "backbone: the weight-name table does not match the layer table"; return -1; }
+    std::vector<float> hW(b->hW.size()), hB(b->hB.size());
+    std::vector<float*> wp(n), bp(n);
+    for (int i = 0; i < n; ++i) {
+        const ConvLayer& L = b->layers[i];
+        int rows, K;
+        mrcnn_layer_dims(MRCNN_BACKBONE, i, &rows, &K);
+        if (rows != L.Cout || K != L.Kpad) { g_cnn_err = "backbone: the weight-name table does not match layer " + std::to_string(i); return -1; }
+        wp[i] = hW.data() + L.wOff; bp[i] = hB.data() + L.bOff;
+    }
+    if (mrcnn_fold(path, MRCNN_BACKBONE, wp.data(), bp.data())) return -1;
+    std::vector<__nv_bfloat16> wbf(hW.size());
+    for (size_t i = 0; i < wbf.size(); ++i) wbf[i] = __float2bfloat16(hW[i]);
+    cudaError_t e = cudaMemcpyAsync(b->dW, wbf.data(), wbf.size() * 2, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(b->dB, hB.data(), hB.size() * 4, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) { g_cnn_err = std::string("backbone: weight upload: ") + cudaGetErrorString(e); return -2; }
+    b->hW.swap(hW); b->hB.swap(hB);
+    return 0;
+}
+
 // forward on an already-moulded input (device, NHWC bf16 S x S x 3).  Outputs stay on the device (P2..P6, NHWC bf16).
 extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
 {

@@ -476,6 +476,35 @@ extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* b
     return 0;
 }
 
+// pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
+extern "C" int mf_detector_load_weights(mf_detector* h, const char* path)
+{
+    if (!h) return det_fail("detector: null handle");
+    if (mrcnn_layer_count(MRCNN_DETECTOR) != N_LAYERS) return det_fail("detector: the weight-name table does not match the layer table");
+    std::vector<float> hW[N_LAYERS], hB[N_LAYERS];
+    float *w[N_LAYERS], *b[N_LAYERS];
+    for (int i = 0; i < N_LAYERS; ++i) {
+        int rows, K;
+        mrcnn_layer_dims(MRCNN_DETECTOR, i, &rows, &K);
+        if (rows != LAYERS[i].rows || K != LAYERS[i].K) return det_fail("detector: the weight-name table does not match layer " + std::to_string(i));
+        hW[i].resize((size_t)rows * K); hB[i].resize(rows);
+        w[i] = hW[i].data(); b[i] = hB[i].data();
+    }
+    if (mrcnn_fold(path, MRCNN_DETECTOR, w, b)) return -1;
+    cudaError_t e = cudaSuccess;
+    std::vector<__nv_bfloat16> wbf[N_LAYERS];
+    for (int i = 0; i < N_LAYERS && e == cudaSuccess; ++i) {
+        wbf[i].resize(hW[i].size());
+        for (size_t k = 0; k < hW[i].size(); ++k) wbf[i][k] = __float2bfloat16(hW[i][k]);
+        e = cudaMemcpyAsync(h->dW[i], wbf[i].data(), wbf[i].size() * 2, cudaMemcpyHostToDevice, h->s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(h->dB[i], hB[i].data(), hB[i].size() * 4, cudaMemcpyHostToDevice, h->s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->s);
+    if (e != cudaSuccess) return det_fail(std::string("detector: weight upload: ") + cudaGetErrorString(e));
+    for (int i = 0; i < N_LAYERS; ++i) { h->hW[i].swap(hW[i]); h->hB[i].swap(hB[i]); }
+    return 0;
+}
+
 static int download(mf_detector* h, void* dst, const void* src, size_t bytes)
 {
     if (!dst) return 0;

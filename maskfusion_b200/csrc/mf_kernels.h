@@ -175,6 +175,14 @@ const void* rpn_pooled(mf_rpn* h);                // [1000][7][7][256] bf16
 // seeded He-style weights [rows x K] (bf16-representable) and biases, the backbone's scheme (mf_cnn.cu add_conv)
 void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed);
 
+// ---- mf_weights.cu: pretrained Mask R-CNN weights (safetensors, R-FOLD) for the three handles' layer tables ----
+enum { MRCNN_BACKBONE, MRCNN_RPN, MRCNN_DETECTOR };
+int mrcnn_layer_count(int part);                             // the handle's layers, in its table order
+void mrcnn_layer_dims(int part, int i, int* rows, int* K);   // table of layer i: [rows x K] weights, [rows] bias
+// reads, checks and folds every layer of `part` from the file into w[i] / b[i] (sized by mrcnn_layer_dims); 0, or -1 with the message in
+// cnn_last_error() naming the file and the tensor
+int mrcnn_fold(const char* path, int part, float* const* w, float* const* b);
+
 // ---- mf_heads.cu: the detector on the frame path (mf_attach_detector) ----
 cudaStream_t detector_stream(mf_detector* h);
 int detector_reserve_image(mf_detector* h, int W, int H);      // id image sized for W x H once: mf_detector_detect at W x H then never reallocates

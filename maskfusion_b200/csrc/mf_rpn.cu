@@ -448,6 +448,31 @@ extern "C" int mf_rpn_get_weights(mf_rpn* h, float* conv_w, float* conv_b, float
     return 0;
 }
 
+// pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
+extern "C" int mf_rpn_load_weights(mf_rpn* h, const char* path)
+{
+    if (!h) return rpn_fail("rpn: null handle");
+    std::vector<float> wc(h->hWc.size()), bc(h->hBc.size()), wh(h->hWh.size()), bh(h->hBh.size());
+    float* w[2] = {wc.data(), wh.data()};
+    float* b[2] = {bc.data(), bh.data()};
+    int rows[2], K[2];
+    for (int i = 0; i < 2; ++i) mrcnn_layer_dims(MRCNN_RPN, i, &rows[i], &K[i]);
+    if (mrcnn_layer_count(MRCNN_RPN) != 2 || (size_t)rows[0] * K[0] != wc.size() || (size_t)rows[1] * K[1] != wh.size())
+        return rpn_fail("rpn: the weight-name table does not match the handle's tables");
+    if (mrcnn_fold(path, MRCNN_RPN, w, b)) return -1;
+    std::vector<__nv_bfloat16> wcb(wc.size()), whb(wh.size());
+    for (size_t i = 0; i < wc.size(); ++i) wcb[i] = __float2bfloat16(wc[i]);
+    for (size_t i = 0; i < wh.size(); ++i) whb[i] = __float2bfloat16(wh[i]);
+    cudaError_t e = cudaMemcpyAsync(h->dWc, wcb.data(), wcb.size() * 2, cudaMemcpyHostToDevice, h->s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dWh, whb.data(), whb.size() * 2, cudaMemcpyHostToDevice, h->s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dBc, bc.data(), bc.size() * 4, cudaMemcpyHostToDevice, h->s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dBh, bh.data(), bh.size() * 4, cudaMemcpyHostToDevice, h->s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->s);
+    if (e != cudaSuccess) return rpn_fail(std::string("rpn: weight upload: ") + cudaGetErrorString(e));
+    h->hWc.swap(wc); h->hBc.swap(bc); h->hWh.swap(wh); h->hBh.swap(bh);
+    return 0;
+}
+
 static int download(mf_rpn* h, void* dst, const void* src, size_t bytes)
 {
     if (!h) return rpn_fail("rpn: null handle");
