@@ -17,6 +17,7 @@
 // (the reference clears 3 x texDim^2 x 16 B of update maps on every fuse).
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "mf_host.h"
 
 namespace mfb {
 
@@ -724,39 +725,88 @@ MF_D void splatRange(const SplatVS& v, int W, int H, int& x0, int& x1, int& y0, 
 #define SPLAT_BS 128               // surfels (= threads) per block round: smaller rounds interleave the load phase of one block with the raster phase of another
 #endif
 #ifndef SPLAT_MIN_BLOCKS
-#define SPLAT_MIN_BLOCKS 16            // 32 registers (88 B of spills), 2048 threads per SM.  Measured (k_splat_project, us): 64 registers /
-#endif                                 // 8 blocks 224; 48 / 10: 224; 40 / 12: 205; 32 / 16: 185 -- the rasteriser hides its key / ray loads with warps, not registers
+#define SPLAT_MIN_BLOCKS 8             // 56 registers, no spills; 9 blocks per SM fit.  Measured (k_splat_project, ms; H100 80GB HBM3, 400 W limit): 8 blocks
+#endif                                 // 0.257; 12 (40 registers, 28 B of spills) 0.303; 16 (32 registers, 76 B; shared memory holds 13) 0.364;
+                                       // SPLAT_BS 64 / 16 blocks 0.270; SPLAT_BS 256 / 4 blocks 0.286
+#define SPLAT_Q 64                 // per-warp queue of exact-path fragments: a drain takes 32, so at most 31 + 32 are pending
+
+// one drawable surfel of a round as the raster phase reads it; pn = dot3(pos, n) is the numerator of the ray parameter
+struct __align__(16) SplatEntry { float px, py, pz, pn, nx, ny, nz, rad; int x0, y0, w; uint32_t id; };
+
+// exact path of a fragment that passed the pre-tests (combo_splat.frag): IEEE ray parameter and disc test, depth range, and the
+// (depth, id) key into the key image.  atomicMin does not depend on the order of the fragments.  A stale (larger) key from L1 only
+// lets more fragments reach the atomic.
+MF_D void splatExact(const SplatEntry& e, int pix, const float4* __restrict__ rayTab, unsigned long long* __restrict__ key, float maxDepth)
+{
+    SplatVS sv; sv.pos = make_float3(e.px, e.py, e.pz); sv.n = make_float3(e.nx, e.ny, e.nz); sv.rad = e.rad;
+    const float4 l4 = __ldg(rayTab + pix);
+    float3 cp;
+    if (!splatFragmentRay(sv, make_float3(l4.x, l4.y, l4.z), cp)) return;
+    const float fd = (cp.z / (2 * maxDepth)) + 0.5f;
+    if (!(fd >= 0.0f && fd < 1.0f)) return;
+    const unsigned long long k = ((unsigned long long)__float_as_uint(fd) << 32) | e.id;
+    if (k < key[pix]) atomicMin(key + pix, k);
+}
+
 __global__ void __launch_bounds__(SPLAT_BS, SPLAT_MIN_BLOCKS) k_splat_project(const float4* __restrict__ pos, const float4* __restrict__ col, const float4* __restrict__ nrm,
                                                        const uint32_t* __restrict__ countPtr, const DevPose* __restrict__ dpose, Cam cam, int W, int H,
                                                        float maxDepth, float confThreshold, float ftime, float fmaxTime, float ftimeDelta,
                                                        uint32_t drawBase, const float4* __restrict__ rayTab, unsigned long long* __restrict__ key)
 {
-    const Rt tinv = dpose->tinv;
-    // Row-segment rasterisation.  A block projects 256 surfels and compacts the drawable ones into shared memory.  Their point
-    // sprites (1 .. 2047^2 pixels) are cut into UNITS of up to SPLAT_SEG consecutive pixels of one sprite row; the units are
-    // numbered by an exclusive prefix sum and walked by all threads, unit u belonging to the entry found by binary search.
-    // Balanced whatever the mix of far (1 px) and near (large) surfels, and the per-fragment work is the ray/disc test alone:
-    // the search and the unit -> (row, x range) arithmetic are paid once per SPLAT_SEG fragments, the pixel ray comes from the
-    // table.  (One search + one integer division + one ray normalisation per FRAGMENT made this kernel instruction bound;
-    // a per-thread pixel loop before that ran with ~5 of 32 lanes active.)
-    struct Entry { float px, py, pz, nx, ny, nz, rad; int x0, y0, w; uint32_t id; };
+    // Row-segment rasterisation.  A block projects SPLAT_BS surfels per round and compacts the drawable ones into shared memory.
+    // Their point sprites (1 .. 2047^2 pixels) are cut into UNITS of up to SPLAT_SEG consecutive pixels of one sprite row; the units
+    // are numbered by an exclusive prefix sum and walked by all threads, unit u belonging to the entry found by binary search.
+    // Balanced whatever the mix of far (1 px) and near (large) surfels; the search and the unit -> (row, x range) arithmetic are paid
+    // once per SPLAT_SEG fragments, the pixel ray comes from the table.
+    // With ~100 fragments per pixel almost every fragment loses the depth test or misses its disc.  The fragment loop only runs
+    // conservative pre-tests in fast arithmetic; a fragment that can still win goes to a per-warp queue (pixel << 8 | entry slot),
+    // and the warp drains 32 queued fragments at a time through the IEEE path (splatExact) with all lanes.  The divisions of that
+    // path stay out of the loop, which then needs no local memory.
+    // Rounds alternate between two entry / offset buffers: round r + 2 overwrites round r's buffer only after both barriers of
+    // round r + 1, which every thread reaches after its raster of round r, so a round needs no barrier at its end.  The next
+    // round's positions stream into shared memory (one bulk copy, completion on an mbarrier) behind this round's raster.
     constexpr int NW = SPLAT_BS / 32;
-    __shared__ Entry ent[SPLAT_BS];
-    __shared__ int offs[SPLAT_BS + 1];
+    static_assert(SPLAT_BS % 32 == 0 && SPLAT_BS <= 256, "the queue packs the entry slot into 8 bits");
+    __shared__ SplatEntry ent[2][SPLAT_BS];
+    __shared__ int offs[2][SPLAT_BS];
+    __shared__ __align__(16) float4 spos[SPLAT_BS];
+    __shared__ uint32_t queue[NW][SPLAT_Q];
     __shared__ int wtot[NW], wcnt[NW];
+    __shared__ Rt tinv;
+    __shared__ float inv2md;
+    __shared__ __align__(8) unsigned long long bar;
     const uint32_t count = *countPtr;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t stride = gridDim.x * blockDim.x;
-    const float inv2md = 1.0f / (2 * maxDepth);
-    float4 pNext = make_float4(0, 0, 0, 0);
-    if (blockIdx.x * blockDim.x + threadIdx.x < count) pNext = ldStream(pos + blockIdx.x * blockDim.x + threadIdx.x);
-    for (uint32_t base = blockIdx.x * blockDim.x; base < count; base += stride) {
+    const uint32_t stride = gridDim.x * SPLAT_BS;
+    const unsigned barAddr = (unsigned)__cvta_generic_to_shared(&bar);
+    const unsigned sposAddr = (unsigned)__cvta_generic_to_shared(spos);
+    // one bulk copy of the positions of the round starting at surfel b (16-byte aligned source, destination and size)
+    auto fetch = [&](uint32_t b) {
+        const unsigned bytes = min((uint32_t)SPLAT_BS, count - b) * 16u;
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(barAddr), "r"(bytes) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     ::"r"(sposAddr), "l"(pos + b), "r"(bytes), "r"(barAddr) : "memory");
+    };
+    if (threadIdx.x < 12) tinv.m[threadIdx.x] = dpose->tinv.m[threadIdx.x];
+    if (threadIdx.x == 0) {
+        inv2md = 1.0f / (2 * maxDepth);
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(barAddr));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        if (blockIdx.x * SPLAT_BS < count) fetch(blockIdx.x * SPLAT_BS);
+    }
+    __syncthreads();
+    unsigned parity = 0;
+    for (uint32_t base = blockIdx.x * SPLAT_BS; base < count; base += stride, parity ^= 1u) {
         const uint32_t id = base + threadIdx.x;
         SplatVS v; v.ok = false;
         int x0 = 0, x1 = -1, y0 = 0, y1 = -1;
-        const float4 p = pNext;
-        if (id + stride < count) pNext = ldStream(pos + id + stride);      // next round's position streams in behind this round's raster
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "SPLAT_WAIT:\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+            "@!p bra SPLAT_WAIT;\n\t}" ::"r"(barAddr), "r"(parity) : "memory");
         if (id < count) {
+            const float4 p = spos[threadIdx.x];
             // cheap rejects before touching the other two planes
             float3 ph = xform(tinv, make_float3(p.x, p.y, p.z));
             // ... including the point-clipping test on the projected centre (same arithmetic as splatVertex), which most
@@ -778,60 +828,75 @@ __global__ void __launch_bounds__(SPLAT_BS, SPLAT_MIN_BLOCKS) k_splat_project(co
         if (lane == 31) wtot[warp] = incl;
         if (lane == 0) wcnt[warp] = __popc(db);
         __syncthreads();
+        // every thread has read its position: the next round's positions may overwrite them
+        if (threadIdx.x == 0 && base + stride < count) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fetch(base + stride);
+        }
+        SplatEntry* __restrict__ E = ent[parity];
+        int* __restrict__ O = offs[parity];
         int fbase = 0, sbase = 0, total = 0, nent = 0;
 #pragma unroll
         for (int w = 0; w < NW; ++w) { if (w < warp) { fbase += wtot[w]; sbase += wcnt[w]; } total += wtot[w]; nent += wcnt[w]; }
         if (draw) {
             const int slot = sbase + __popc(db & ((1u << lane) - 1));
-            Entry e; e.px = v.pos.x; e.py = v.pos.y; e.pz = v.pos.z; e.nx = v.n.x; e.ny = v.n.y; e.nz = v.n.z; e.rad = v.rad;
+            SplatEntry e; e.px = v.pos.x; e.py = v.pos.y; e.pz = v.pos.z; e.pn = dot3(v.pos, v.n); e.nx = v.n.x; e.ny = v.n.y; e.nz = v.n.z; e.rad = v.rad;
             e.x0 = x0; e.y0 = y0; e.w = x1 - x0 + 1; e.id = drawBase + id;
-            ent[slot] = e;
-            offs[slot] = fbase + incl - nunit;
+            E[slot] = e;
+            O[slot] = fbase + incl - nunit;
         }
-        if (threadIdx.x == 0) offs[nent] = total;
         __syncthreads();
-        // gridDim.y > 1 (small stores): the blocks of a column redo the (cheap) vertex stage of the same 128 surfels and share their units --
+        // gridDim.y > 1 (small stores): the blocks of a column redo the (cheap) vertex stage of the same surfels and share their units --
         // an object model has ~50 blocks' worth of surfels, and the units of a few large sprites kept one SM busy while the others idled
-        for (int u = threadIdx.x + blockIdx.y * blockDim.x; u < total; u += blockDim.x * gridDim.y) {
-            int lo = 0, hi = nent - 1;                       // last entry with offs[e] <= u
-            while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (offs[mid] <= u) lo = mid; else hi = mid - 1; }
-            const Entry e = ent[lo];
-            const int t = u - offs[lo];
-            const int nseg = (e.w + SPLAT_SEG - 1) / SPLAT_SEG;
-            const int row = t / nseg, seg = t - row * nseg;
-            const int py = e.y0 + row, xs = e.x0 + seg * SPLAT_SEG;
-            const int xe = min(xs + SPLAT_SEG, e.x0 + e.w);
-            SplatVS sv; sv.pos = make_float3(e.px, e.py, e.pz); sv.n = make_float3(e.nx, e.ny, e.nz); sv.rad = e.rad;
-            const float4* __restrict__ ray = rayTab + py * W;
-            unsigned long long* __restrict__ krow = key + py * W;
-            const float pn = dot3(sv.pos, sv.n);
-            for (int px = xs; px < xe; ++px) {
-                const float4 l4 = __ldg(ray + px);
-                const float3 l = make_float3(l4.x, l4.y, l4.z);
-                // Conservative pre-tests in fast arithmetic.  With ~100 fragments per pixel almost every fragment loses the depth
-                // test or misses its disc: those are recognised with an approximate ray parameter (error < 1e-6 relative, margins
-                // 10x larger) and skipped; only a fragment that can still win runs the IEEE path below, so the key image is
-                // bit-identical.  A stale (larger) key from L1 only makes the pre-test pass more often.
-                const unsigned long long cur = krow[px];
-                const float ta = __fdividef(pn, dot3(l, sv.n));
-                if (cur != KEY_EMPTY) {
-                    const float fda = __fmaf_rn(ta * l.z, inv2md, 0.5f);
-                    if (fda > __uint_as_float((unsigned)(cur >> 32)) * 1.00001f) continue;          // clearly behind the current winner
+        uint32_t* __restrict__ q = queue[warp];
+        int qn = 0;
+        for (int ub = threadIdx.x - lane + blockIdx.y * SPLAT_BS; ub < total; ub += SPLAT_BS * gridDim.y) {
+            const int u = ub + lane;
+            int slot = 0, pix = 0, n = 0;
+            if (u < total) {
+                int lo = 0, hi = nent - 1;                       // last entry with offs[e] <= u
+                while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (O[mid] <= u) lo = mid; else hi = mid - 1; }
+                slot = lo;
+                const int t = u - O[slot], w = E[slot].w, x0e = E[slot].x0;
+                const int nseg = (w + SPLAT_SEG - 1) / SPLAT_SEG;
+                const int row = t / nseg, xs = x0e + (t - row * nseg) * SPLAT_SEG;
+                n = min(SPLAT_SEG, x0e + w - xs);
+                pix = (E[slot].y0 + row) * W + xs;
+            }
+            const int nmax = __reduce_max_sync(0xffffffffu, n);
+            for (int i = 0; i < nmax; ++i, ++pix) {
+                bool cand = false;
+                if (i < n) {
+                    // Conservative pre-tests in fast arithmetic: an approximate ray parameter (error < 1e-6 relative, margins 10x larger)
+                    // recognises the fragments that are clearly behind the current winner or clearly outside the disc.
+                    const float4 pp = *reinterpret_cast<const float4*>(&E[slot].px), nr = *reinterpret_cast<const float4*>(&E[slot].nx);
+                    const float4 l4 = __ldg(rayTab + pix);
+                    const unsigned long long cur = key[pix];
+                    const float ta = __fdividef(pp.w, dot3(make_float3(l4.x, l4.y, l4.z), make_float3(nr.x, nr.y, nr.z)));
+                    cand = cur == KEY_EMPTY || !(__fmaf_rn(ta * l4.z, inv2md, 0.5f) > __uint_as_float((unsigned)(cur >> 32)) * 1.00001f);
+                    if (cand) {
+                        const float ax = __fmaf_rn(ta, l4.x, -pp.x), ay = __fmaf_rn(ta, l4.y, -pp.y), az = __fmaf_rn(ta, l4.z, -pp.z);
+                        const float re = nr.w + 8e-6f * fabsf(ta);
+                        cand = !(__fmaf_rn(ax, ax, __fmaf_rn(ay, ay, az * az)) > re * re * 1.0001f);
+                    }
                 }
-                {
-                    const float ax = __fmaf_rn(ta, l.x, -sv.pos.x), ay = __fmaf_rn(ta, l.y, -sv.pos.y), az = __fmaf_rn(ta, l.z, -sv.pos.z);
-                    const float re = sv.rad + 8e-6f * fabsf(ta);
-                    if (__fmaf_rn(ax, ax, __fmaf_rn(ay, ay, az * az)) > re * re * 1.0001f) continue;  // clearly outside the disc
+                const unsigned m = __ballot_sync(0xffffffffu, cand);
+                if (cand) q[qn + __popc(m & ((1u << lane) - 1))] = (uint32_t)pix << 8 | (uint32_t)slot;
+                qn += __popc(m);
+                if (qn >= 32) {
+                    qn -= 32;
+                    __syncwarp();
+                    const uint32_t it = q[qn + lane];
+                    __syncwarp();
+                    splatExact(E[it & 255u], (int)(it >> 8), rayTab, key, maxDepth);
                 }
-                float3 cp;
-                if (!splatFragmentRay(sv, l, cp)) continue;
-                float fd = (cp.z / (2 * maxDepth)) + 0.5f;
-                if (!(fd >= 0.0f && fd < 1.0f)) continue;
-                unsigned long long k = ((unsigned long long)__float_as_uint(fd) << 32) | e.id;
-                if (k < cur) atomicMin(krow + px, k);
             }
         }
-        __syncthreads();
+        __syncwarp();
+        if (lane < qn) {
+            const uint32_t it = q[lane];
+            splatExact(E[it & 255u], (int)(it >> 8), rayTab, key, maxDepth);
+        }
     }
 }
 
@@ -1106,11 +1171,19 @@ void launch_ray_table(Cam cam, int W, int H, float4* tab, cudaStream_t s)
     k_ray_table<<<g, b, 0, s>>>(cam, W, H, tab);
 }
 
-// grid of the splat rasteriser: a persistent grid for large stores; for a small store (an object model: a few thousand surfels) one column
-// of blocks per 128 surfels of CAPACITY is cheap to over-provision, and 8 blocks share the units of each column (gridDim.y)
-static dim3 splatGrid(uint32_t capacity)
+// grid of the splat rasteriser: for large stores a persistent grid of as many blocks as the SMs hold at once; for a small store (an object
+// model: a few thousand surfels) one column of blocks per SPLAT_BS surfels of CAPACITY is cheap to over-provision, and 8 blocks share the
+// units of each column (gridDim.y)
+static dim3 splatGrid(uint32_t capacity, int W, int H)
 {
-    const int persistent = persistentBlocks(8 * 256 / SPLAT_BS);
+    if ((size_t)W * H > (1u << 24)) throw CudaError{"splat rasteriser: more than 2^24 pixels (its exact-path queue keeps 24-bit pixel indices)"};
+    static const int perSM = [] {
+        int n = 0;
+        cudaCheck(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_splat_project, SPLAT_BS, 0), "k_splat_project occupancy");
+        if (n < 1) throw CudaError{"k_splat_project does not fit on an SM"};
+        return n;
+    }();
+    const int persistent = persistentBlocks(perSM);
     if (capacity == 0 || capacity >= (1u << 20)) return dim3(persistent);
     const int cols = (int)std::min<uint32_t>((capacity + SPLAT_BS - 1) / SPLAT_BS, (uint32_t)persistent);
     return dim3(cols, 8);
@@ -1120,7 +1193,7 @@ void launch_combined_predict(const SurfelPlanes& sp, const uint32_t* count, cons
                              float4* normalRad, uint16_t* timeTex, int doFill, const float* depthFilt, const uchar4* rgb, int ptVN, int ptImg,
                              uchar4* fillImage, float4* fillVertex, float4* fillNormal, uint32_t* nonBlackSamples, cudaStream_t s, uint32_t capacity)
 {
-    prof_mark(s, "k_splat_project"); k_splat_project<<<splatGrid(capacity), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
+    prof_mark(s, "k_splat_project"); k_splat_project<<<splatGrid(capacity, W, H), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
                                                         (float)maxTime, (float)timeDelta, 0u, rayTab, (unsigned long long*)key);
     if (nonBlackSamples) cudaMemsetAsync(nonBlackSamples, 0, sizeof(uint32_t), s);
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
@@ -1152,7 +1225,7 @@ void launch_splat_project_only(const SurfelPlanes& sp, const uint32_t* count, co
                                int time, int maxTime, int timeDelta, uint32_t drawBase, const float4* rayTab, uint64_t* key, cudaStream_t s, uint32_t capacity)
 {
     prof_mark(s, "k_splat_project_ids");
-    k_splat_project<<<splatGrid(capacity), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
+    k_splat_project<<<splatGrid(capacity, W, H), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
                                                         (float)maxTime, (float)timeDelta, drawBase, rayTab, (unsigned long long*)key);
 }
 }  // namespace mfb
