@@ -641,20 +641,31 @@ def write_klg(path: str, timestamps, depth_mm: np.ndarray, rgb: np.ndarray):
         raise MFError(L.mf_last_error().decode())
 
 
-class Backbone:
+class _CnnHandle:
+    """what the Mask R-CNN handles share: errors reported through mf_cnn_last_error, close() through their destroy function"""
+
+    _destroy = ""
+
+    def _ck(self, r):
+        if r is None or r < 0:
+            raise MFError(self.L.mf_cnn_last_error().decode())
+        return r
+
+    def close(self):
+        if getattr(self, "h", None):
+            getattr(self.L, self._destroy)(self.h); self.h = None
+
+
+class Backbone(_CnnHandle):
     """Mask R-CNN ResNet-101-FPN backbone on wgmma GEMMs (csrc/mf_cnn.cu).  Weights are synthetic (seeded) unless loaded with
     loadWeights (matterport's Keras arrays in a safetensors file, BatchNorm folded; see load_mask_rcnn)."""
+
+    _destroy = "mf_backbone_destroy"
 
     def __init__(self, input_size=1024, seed=1, stream: int | None = None):
         self.L = load_library()
         self.S = input_size
-        self.h = self.L.mf_backbone_create(input_size, seed, C.c_void_p(stream) if stream else None)
-        if not self.h:
-            raise MFError(self.L.mf_cnn_last_error().decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.mf_backbone_destroy(self.h); self.h = None
+        self.h = self._ck(self.L.mf_backbone_create(input_size, seed, C.c_void_p(stream) if stream else None))
 
     def layers(self):
         out = []
@@ -672,13 +683,11 @@ class Backbone:
 
     def loadWeights(self, path: str):
         """the backbone's tensors of a safetensors weight file (conv1, res*, bn*, fpn_*); all or nothing, complete on return"""
-        if self.L.mf_backbone_load_weights(self.h, os.fsencode(path)) != 0:
-            raise MFError(self.L.mf_cnn_last_error().decode())
+        self._ck(self.L.mf_backbone_load_weights(self.h, os.fsencode(path)))
         return self
 
     def forward(self, input_ptr: int):
-        if self.L.mf_backbone_forward(self.h, C.c_void_p(input_ptr)) != 0:
-            raise MFError(self.L.mf_cnn_last_error().decode())
+        self._ck(self.L.mf_backbone_forward(self.h, C.c_void_p(input_ptr)))
 
     def output(self, level):
         d = np.zeros(3, np.int32)
@@ -689,9 +698,8 @@ class Backbone:
         """bf16 output as float32 numpy (H, W, C)"""
         _, (h, w, c) = self.output(level)
         raw = np.zeros((h, w, c), np.uint16)
-        if self.L.mf_backbone_download(self.h, level, _p(raw)) != 0:
-            raise MFError("backbone download failed")
-        return (raw.astype(np.uint32) << 16).view(np.float32)
+        self._ck(self.L.mf_backbone_download(self.h, level, _p(raw)))
+        return _bf16_to_f32(raw)
 
     def flops(self):
         return float(self.L.mf_backbone_flops(self.h))
@@ -704,30 +712,20 @@ def _bf16_to_f32(raw: np.ndarray) -> np.ndarray:
     return (raw.astype(np.uint32) << 16).view(np.float32)
 
 
-class RegionProposals:
+class RegionProposals(_CnnHandle):
     """Mask R-CNN RPN head + proposal layer + pyramid ROI Align on a Backbone's P2..P6 (csrc/mf_rpn.cu).  Weights are synthetic (seeded)
     unless loaded with loadWeights.  Runs on the backbone's stream; close it before the backbone."""
 
     POST_NMS, POOL, CHANNELS = 1000, 7, 256
     CONV, HEADS, PROPOSALS, ROI_ALIGN = 1, 2, 4, 8        # stage bits of run()
+    _destroy = "mf_rpn_destroy"
 
     def __init__(self, backbone: Backbone, seed=1):
         self.L = load_library()
         self.backbone = backbone
         self.S = backbone.S
-        self.h = self.L.mf_rpn_create(C.c_void_p(backbone.h), seed)
-        if not self.h:
-            raise MFError(self.L.mf_cnn_last_error().decode())
+        self.h = self._ck(self.L.mf_rpn_create(C.c_void_p(backbone.h), seed))
         self.A = int(self.L.mf_rpn_num_anchors(self.h))
-
-    def _ck(self, r):
-        if r < 0:
-            raise MFError(self.L.mf_cnn_last_error().decode())
-        return r
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.mf_rpn_destroy(self.h); self.h = None
 
     def forward(self):
         """conv, heads, proposals and ROI Align of the backbone's last forward"""
@@ -792,29 +790,19 @@ def roi_align(backbone: Backbone, boxes_ptr: int, n: int, pool: int, out_ptr: in
         raise MFError(L.mf_cnn_last_error().decode())
 
 
-class Detector:
+class Detector(_CnnHandle):
     """Mask R-CNN detection heads on a RegionProposals' proposals (csrc/mf_heads.cu): classifier, detection layer, mask head, unmould and
     generate_id_image.  Weights are synthetic (seeded) unless loaded with loadWeights.  Runs on the backbone's stream; close it before the
     RegionProposals."""
 
     ROIS, MAX_DETECTIONS, NUM_CLASSES, MASK = 1000, 100, 81, 28
     CLASSIFIER, DETECTIONS, MASKS, ID_IMAGE = 1, 2, 4, 8        # stage bits of run()
+    _destroy = "mf_detector_destroy"
 
     def __init__(self, rpn: RegionProposals, seed=1):
         self.L = load_library()
         self.rpn = rpn
-        self.h = self.L.mf_detector_create(C.c_void_p(rpn.h), seed)
-        if not self.h:
-            raise MFError(self.L.mf_cnn_last_error().decode())
-
-    def _ck(self, r):
-        if r < 0:
-            raise MFError(self.L.mf_cnn_last_error().decode())
-        return r
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.mf_detector_destroy(self.h); self.h = None
+        self.h = self._ck(self.L.mf_detector_create(C.c_void_p(rpn.h), seed))
 
     def run(self, stages: int):
         self._ck(self.L.mf_detector_run(self.h, int(stages)))

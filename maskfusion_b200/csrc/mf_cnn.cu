@@ -360,7 +360,22 @@ template <int BN>
 static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 2 * GEMM_STAGES * 8 + 1024; }
 
 const char* cnn_last_error() { return g_cnn_err.c_str(); }
-void cnn_set_error(const char* msg) { g_cnn_err = msg; }
+int cnn_fail(const std::string& msg) { g_cnn_err = msg; return -1; }
+
+int cnn_check_launch(const char* what)
+{
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cnn_fail(std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+int cnn_download(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows, size_t pitch)
+{
+    if (!dst) return 0;
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess)
+        e = rows == 1 ? cudaMemcpy(dst, src, width, cudaMemcpyDeviceToHost) : cudaMemcpy2D(dst, width, src, pitch, width, rows, cudaMemcpyDeviceToHost);
+    return e == cudaSuccess ? 0 : cnn_fail(std::string("download: ") + cudaGetErrorString(e));
+}
 
 template <int BN, typename OutT>
 static void launch_wgmma(dim3 grid, cudaStream_t s, const CUtensorMap& mA, const CUtensorMap& mB, const float* bias, const void* residual, void* out,
@@ -408,40 +423,16 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
 }
 
 // ---- backbone ---------------------------------------------------------------------------
-struct ConvLayer {
-    int Cin, Cout, k, stride, pad, Kpad;
-    size_t wOff, bOff;      // offsets into the weight / bias pools (elements)
-};
-
 struct Backbone {
     int S;                                    // square network input (1024)
-    std::vector<ConvLayer> layers;
-    __nv_bfloat16* dW = nullptr; float* dB = nullptr;
-    std::vector<float> hW; std::vector<float> hB;            // fp32 master copy (already bf16-rounded) for the reference check
-    __nv_bfloat16 *input = nullptr, *bufA = nullptr, *bufB = nullptr, *bufC = nullptr, *bufS = nullptr, *col = nullptr;
-    __nv_bfloat16 *C2 = nullptr, *C3 = nullptr, *C4 = nullptr, *C5 = nullptr, *P[5] = {nullptr, nullptr, nullptr, nullptr, nullptr}, *lat = nullptr, *td = nullptr;
+    cudaStream_t stream;
+    std::vector<LayerGeom> layers;            // the table's: conv1, per block branch2a, 2b, 2c (+ branch1 in block a), 4 laterals, 4 outputs
+    WeightStore w;
+    DevBuf<__nv_bfloat16> input, bufA, bufB, bufC, bufS, col, C2, C3, C4, C5, P[5], lat, td;
     double flops = 0;
     int gemms = 0;
+    Backbone(int S, unsigned seed, cudaStream_t s);
 };
-
-static uint32_t lcg(uint32_t& s) { s = s * 1664525u + 1013904223u; return s; }
-static float urand(uint32_t& s) { return (float)(lcg(s) >> 8) * (1.0f / 16777216.0f) * 2.f - 1.f; }
-static float bf16_round(float f) { return __bfloat162float(__float2bfloat16(f)); }
-
-static int add_conv(Backbone* b, int Cin, int Cout, int k, int stride, int pad, uint32_t& seed, float gain)
-{
-    ConvLayer L; L.Cin = Cin; L.Cout = Cout; L.k = k; L.stride = stride; L.pad = pad;
-    int K = k * k * Cin; L.Kpad = (K + 63) / 64 * 64;
-    L.wOff = b->hW.size(); L.bOff = b->hB.size();
-    float sc = gain * sqrtf(2.0f / (float)K);                        // He-style so activations stay O(1) through 101 layers
-    b->hW.resize(L.wOff + (size_t)Cout * L.Kpad, 0.f);
-    for (int o = 0; o < Cout; ++o)
-        for (int kk = 0; kk < K; ++kk) b->hW[L.wOff + (size_t)o * L.Kpad + kk] = bf16_round(urand(seed) * sc * 1.7320508f);
-    b->hB.resize(L.bOff + Cout);
-    for (int o = 0; o < Cout; ++o) b->hB[L.bOff + o] = urand(seed) * 0.05f;
-    b->layers.push_back(L);
-    return (int)b->layers.size() - 1;
-}
 
 // geometry guard of the implicit 3x3 path: the 128-pixel TMA box must tile the image exactly
 bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win)
@@ -451,8 +442,8 @@ bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win)
            (Hin % (128 / wbox)) == 0 && wbox >= 8;
 }
 
-// runs convolution L (weights W [Cout x Kpad], bias B) on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]; col: im2col scratch
-static int conv_layer(const ConvLayer& L, const __nv_bfloat16* W, const float* B, __nv_bfloat16* col, const __nv_bfloat16* in, int Hin, int Win,
+// runs convolution L (weights W [rows x K], bias B) on in[Hin x Win x cin] -> out[Hout x Wout x rows]; col: im2col scratch
+static int conv_layer(const LayerGeom& L, const __nv_bfloat16* W, const float* B, __nv_bfloat16* col, const __nv_bfloat16* in, int Hin, int Win,
                       __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s, int* HoutP, int* WoutP)
 {
     const int Hout = (Hin + 2 * L.pad - L.k) / L.stride + 1, Wout = (Win + 2 * L.pad - L.k) / L.stride + 1;
@@ -460,29 +451,29 @@ static int conv_layer(const ConvLayer& L, const __nv_bfloat16* W, const float* B
     const __nv_bfloat16* A = in;
     if (HoutP) *HoutP = Hout;
     if (WoutP) *WoutP = Wout;
-    if (cnn_conv_implicit(L.k, L.stride, L.pad, L.Cin, Hin, Win)) {
-        int g3[3] = {Win, Hin, L.Cin};
-        return launch_gemm_bf16(in, W, B, residual, out, M, L.Cout, L.Kpad, relu, s, g3);
+    if (cnn_conv_implicit(L.k, L.stride, L.pad, L.cin, Hin, Win)) {
+        int g3[3] = {Win, Hin, L.cin};
+        return launch_gemm_bf16(in, W, B, residual, out, M, L.rows, L.K, relu, s, g3);
     }
     if (!(L.k == 1 && L.stride == 1)) {
-        if (L.k == 1 && L.stride == 2 && (L.Cin % 8) == 0) {
-            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.Cin, col);
+        if (L.k == 1 && L.stride == 2 && (L.cin % 8) == 0) {
+            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.cin, col);
         } else {
-            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.Cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.Kpad, col);
+            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.K, col);
         }
         A = col;
     }
-    return launch_gemm_bf16(A, W, B, residual, out, M, L.Cout, L.Kpad, relu, s);
+    return launch_gemm_bf16(A, W, B, residual, out, M, L.rows, L.K, relu, s);
 }
 
 // runs backbone layer li on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]
 static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int Win, __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s,
                     int* HoutP = nullptr, int* WoutP = nullptr)
 {
-    const ConvLayer& L = b->layers[li];
+    const LayerGeom& L = b->layers[li];
     int Hout, Wout;
-    const int rc = conv_layer(L, b->dW + L.wOff, b->dB + L.bOff, b->col, in, Hin, Win, out, residual, relu, s, &Hout, &Wout);
-    b->flops += 2.0 * Hout * Wout * (double)L.Cout * (double)(L.k * L.k * L.Cin);
+    const int rc = conv_layer(L, b->w.w(li), b->w.b(li), b->col, in, Hin, Win, out, residual, relu, s, &Hout, &Wout);
+    b->flops += 2.0 * Hout * Wout * (double)L.rows * (double)(L.k * L.k * L.cin);
     b->gemms++;
     if (HoutP) *HoutP = Hout;
     if (WoutP) *WoutP = Wout;
@@ -509,7 +500,7 @@ MoldGeom cnn_mold_geometry(int S, int W, int H)
 int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
              cudaStream_t s)
 {
-    ConvLayer L; L.Cin = Cin; L.Cout = Cout; L.k = k; L.stride = stride; L.pad = pad; L.Kpad = (k * k * Cin + 63) / 64 * 64; L.wOff = L.bOff = 0;
+    const LayerGeom L = {Cin, Cout, k, stride, pad, (k * k * Cin + 63) / 64 * 64};
     return conv_layer(L, (const __nv_bfloat16*)W, B, (__nv_bfloat16*)col, (const __nv_bfloat16*)in, Hin, Win, (__nv_bfloat16*)out, nullptr, relu, s,
                       nullptr, nullptr);
 }
@@ -521,7 +512,7 @@ using namespace mfb;
 // ==========================================================================================
 // C ABI (declared in include/maskfusion_b200.h)
 // ==========================================================================================
-struct mf_backbone { Backbone b; cudaStream_t stream; std::vector<int> plan; int stem, fpnLat[4], fpnOut[4]; std::vector<int> blockConv; };
+struct mf_backbone : Backbone { using Backbone::Backbone; };
 
 extern "C" const char* mf_cnn_last_error(void) { return cnn_last_error(); }
 
@@ -539,128 +530,76 @@ extern "C" int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBi
     return launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, H * W, Cout, 9 * Cin, relu, (cudaStream_t)stream, g3);
 }
 
-// ResNet-101 (stages 3,4,23,3; stride in the first 1x1 of each stage as in Keras/matterport) + FPN(256)
+// ResNet-101-FPN (mf_weights.cu has the layer table); throws CudaError
+Backbone::Backbone(int S_, unsigned seed, cudaStream_t s) : S(S_), stream(s), w(MRCNN_BACKBONE, seed, s)
+{
+    for (int i = 0; i < mrcnn_num_layers(MRCNN_BACKBONE); ++i) layers.push_back(mrcnn_layer(MRCNN_BACKBONE, i));
+    const size_t big = (size_t)(S / 2) * (S / 2) * 64;                         // stem output == largest activation (elements): C1 512x512x64 = C2 256x256x256
+    input.alloc((size_t)S * S * 3);
+    bufA.alloc(big); bufB.alloc(big); bufC.alloc(big); bufS.alloc(big);
+    col.alloc((size_t)(S / 4) * (S / 4) * 9 * 256);                            // largest im2col: FPN P2 3x3 on 256x256x256 (and C2 3x3 64ch is smaller); stem: 512*512*192
+    const int fs[4] = {S / 4, S / 8, S / 16, S / 32};
+    C2.alloc((size_t)fs[0] * fs[0] * 256); C3.alloc((size_t)fs[1] * fs[1] * 512); C4.alloc((size_t)fs[2] * fs[2] * 1024); C5.alloc((size_t)fs[3] * fs[3] * 2048);
+    for (int i = 0; i < 4; ++i) P[i].alloc((size_t)fs[i] * fs[i] * 256);
+    P[4].alloc((size_t)(fs[3] / 2) * (fs[3] / 2) * 256);
+    lat.alloc((size_t)fs[0] * fs[0] * 256); td.alloc((size_t)fs[0] * fs[0] * 256);
+}
+
 extern "C" mf_backbone* mf_backbone_create(int input_size, unsigned seed, void* stream)
 {
-    if (input_size % 64) { g_cnn_err = "input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"; return nullptr; }
-    mf_backbone* h = new mf_backbone;
-    Backbone* b = &h->b;
-    b->S = input_size; h->stream = (cudaStream_t)stream;
-    uint32_t sd = seed ? seed : 1u;
-    h->stem = add_conv(b, 3, 64, 7, 2, 3, sd, 1.0f);
-    const int nblocks[4] = {3, 4, 23, 3}, mid[4] = {64, 128, 256, 512};
-    int cin = 64;
-    for (int st = 0; st < 4; ++st)
-        for (int blk = 0; blk < nblocks[st]; ++blk) {
-            const int stride = (blk == 0 && st > 0) ? 2 : 1;
-            const int f = mid[st], cout = f * 4;
-            h->blockConv.push_back(add_conv(b, cin, f, 1, stride, 0, sd, 1.0f));
-            h->blockConv.push_back(add_conv(b, f, f, 3, 1, 1, sd, 1.0f));
-            h->blockConv.push_back(add_conv(b, f, cout, 1, 1, 0, sd, 0.5f));           // damped: residual sums keep O(1) variance
-            h->blockConv.push_back(blk == 0 ? add_conv(b, cin, cout, 1, stride, 0, sd, 0.7f) : -1);
-            cin = cout;
-        }
-    const int cdim[4] = {256, 512, 1024, 2048};
-    for (int i = 0; i < 4; ++i) h->fpnLat[i] = add_conv(b, cdim[i], 256, 1, 1, 0, sd, 0.7f);
-    for (int i = 0; i < 4; ++i) h->fpnOut[i] = add_conv(b, 256, 256, 3, 1, 1, sd, 1.0f);
-    // device pools
-    const int S = b->S;
-    std::vector<__nv_bfloat16> wbf(b->hW.size());
-    for (size_t i = 0; i < wbf.size(); ++i) wbf[i] = __float2bfloat16(b->hW[i]);
-    bool ok = cudaMalloc(&b->dW, wbf.size() * 2) == cudaSuccess && cudaMalloc(&b->dB, b->hB.size() * 4) == cudaSuccess;
-    const size_t big = (size_t)(S / 2) * (S / 2) * 64;                         // stem output == largest activation (elements): C1 512x512x64 = C2 256x256x256
-    ok = ok && cudaMalloc(&b->input, (size_t)S * S * 3 * 2) == cudaSuccess;
-    ok = ok && cudaMalloc(&b->bufA, big * 2) == cudaSuccess && cudaMalloc(&b->bufB, big * 2) == cudaSuccess && cudaMalloc(&b->bufC, big * 2) == cudaSuccess && cudaMalloc(&b->bufS, big * 2) == cudaSuccess;
-    const size_t colElems = (size_t)(S / 4) * (S / 4) * 9 * 256;               // largest im2col: FPN P2 3x3 on 256x256x256 (and C2 3x3 64ch is smaller); stem: 512*512*192
-    ok = ok && cudaMalloc(&b->col, colElems * 2) == cudaSuccess;
-    const int fs[4] = {S / 4, S / 8, S / 16, S / 32};
-    ok = ok && cudaMalloc(&b->C2, (size_t)fs[0] * fs[0] * 256 * 2) == cudaSuccess && cudaMalloc(&b->C3, (size_t)fs[1] * fs[1] * 512 * 2) == cudaSuccess &&
-         cudaMalloc(&b->C4, (size_t)fs[2] * fs[2] * 1024 * 2) == cudaSuccess && cudaMalloc(&b->C5, (size_t)fs[3] * fs[3] * 2048 * 2) == cudaSuccess;
-    for (int i = 0; i < 4; ++i) ok = ok && cudaMalloc(&b->P[i], (size_t)fs[i] * fs[i] * 256 * 2) == cudaSuccess;
-    ok = ok && cudaMalloc(&b->P[4], (size_t)(fs[3] / 2) * (fs[3] / 2) * 256 * 2) == cudaSuccess;
-    ok = ok && cudaMalloc(&b->lat, (size_t)fs[0] * fs[0] * 256 * 2) == cudaSuccess && cudaMalloc(&b->td, (size_t)fs[0] * fs[0] * 256 * 2) == cudaSuccess;
-    if (!ok) { g_cnn_err = "backbone: cudaMalloc failed"; delete h; return nullptr; }
-    cudaMemcpy(b->dW, wbf.data(), wbf.size() * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(b->dB, b->hB.data(), b->hB.size() * 4, cudaMemcpyHostToDevice);
-    return h;
+    if (input_size % 64) { cnn_fail("input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"); return nullptr; }
+    try {
+        return new mf_backbone(input_size, seed, (cudaStream_t)stream);
+    } catch (const CudaError& e) {
+        cnn_fail("backbone: " + e.what);
+        return nullptr;
+    }
 }
 
-extern "C" void mf_backbone_destroy(mf_backbone* h)
-{
-    if (!h) return;
-    Backbone* b = &h->b;
-    void* ptrs[] = {b->dW, b->dB, b->input, b->bufA, b->bufB, b->bufC, b->bufS, b->col, b->C2, b->C3, b->C4, b->C5, b->P[0], b->P[1], b->P[2], b->P[3], b->P[4], b->lat, b->td};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    delete h;
-}
+extern "C" void mf_backbone_destroy(mf_backbone* h) { delete h; }
 
-extern "C" int mf_backbone_num_layers(mf_backbone* h) { return h ? (int)h->b.layers.size() : -1; }
+extern "C" int mf_backbone_num_layers(mf_backbone* h) { return h ? (int)h->layers.size() : cnn_fail("backbone: null handle"); }
 // layer table: Cin Cout k stride pad Kpad
 extern "C" int mf_backbone_layer(mf_backbone* h, int i, int* out6)
 {
-    if (!h || i < 0 || i >= (int)h->b.layers.size()) return -1;
-    const ConvLayer& L = h->b.layers[i];
-    out6[0] = L.Cin; out6[1] = L.Cout; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.Kpad;
+    if (!h || i < 0 || i >= (int)h->layers.size() || !out6) return cnn_fail("backbone: bad layer index");
+    const LayerGeom& L = h->layers[i];
+    out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
     return 0;
 }
 // weights [Cout x Kpad] fp32 (bf16-representable), (ky,kx,cin) order along K; bias [Cout]
 extern "C" int mf_backbone_get_weights(mf_backbone* h, int i, float* w, float* bias)
 {
-    if (!h || i < 0 || i >= (int)h->b.layers.size()) return -1;
-    const ConvLayer& L = h->b.layers[i];
-    memcpy(w, h->b.hW.data() + L.wOff, (size_t)L.Cout * L.Kpad * sizeof(float));
-    memcpy(bias, h->b.hB.data() + L.bOff, (size_t)L.Cout * sizeof(float));
-    return 0;
+    return h ? h->w.get(i, w, bias) : cnn_fail("backbone: null handle");
 }
 
 // pretrained weights (mf_weights.cu): every layer is read, checked and folded on the host before the device tables change; the copy is
 // ordered on the handle's stream and complete on return
 extern "C" int mf_backbone_load_weights(mf_backbone* h, const char* path)
 {
-    if (!h) { g_cnn_err = "backbone: null handle"; return -1; }
-    Backbone* b = &h->b;
-    const int n = (int)b->layers.size();
-    if (mrcnn_layer_count(MRCNN_BACKBONE) != n) { g_cnn_err = "backbone: the weight-name table does not match the layer table"; return -1; }
-    std::vector<float> hW(b->hW.size()), hB(b->hB.size());
-    std::vector<float*> wp(n), bp(n);
-    for (int i = 0; i < n; ++i) {
-        const ConvLayer& L = b->layers[i];
-        int rows, K;
-        mrcnn_layer_dims(MRCNN_BACKBONE, i, &rows, &K);
-        if (rows != L.Cout || K != L.Kpad) { g_cnn_err = "backbone: the weight-name table does not match layer " + std::to_string(i); return -1; }
-        wp[i] = hW.data() + L.wOff; bp[i] = hB.data() + L.bOff;
-    }
-    if (mrcnn_fold(path, MRCNN_BACKBONE, wp.data(), bp.data())) return -1;
-    std::vector<__nv_bfloat16> wbf(hW.size());
-    for (size_t i = 0; i < wbf.size(); ++i) wbf[i] = __float2bfloat16(hW[i]);
-    cudaError_t e = cudaMemcpyAsync(b->dW, wbf.data(), wbf.size() * 2, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(b->dB, hB.data(), hB.size() * 4, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e != cudaSuccess) { g_cnn_err = std::string("backbone: weight upload: ") + cudaGetErrorString(e); return -2; }
-    b->hW.swap(hW); b->hB.swap(hB);
-    return 0;
+    return h ? h->w.load(path, h->stream) : cnn_fail("backbone: null handle");
 }
 
 // forward on an already-moulded input (device, NHWC bf16 S x S x 3).  Outputs stay on the device (P2..P6, NHWC bf16).
 extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
 {
-    if (!h) return -1;
-    Backbone* b = &h->b; cudaStream_t s = h->stream;
+    if (!h) return cnn_fail("backbone: null handle");
+    Backbone* b = h; cudaStream_t s = h->stream;
     b->flops = 0; b->gemms = 0;
     const int S = b->S;
     int H, W;
+    int li = 0;                                      // the next layer of the table
     // C1: 7x7/2 + ReLU, max-pool 3x3/2
-    if (run_conv(b, h->stem, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W)) return -2;
+    if (run_conv(b, li++, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W)) return -2;
     prof_mark(s, "k_maxpool3s2"); k_maxpool3s2<<<8 * num_sms(), 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
     H /= 2; W /= 2;
     __nv_bfloat16* x = b->bufB;                      // current block input
-    __nv_bfloat16* pool[3] = {b->bufA, b->bufC, b->bufS};
     const int nblocks[4] = {3, 4, 23, 3};
     __nv_bfloat16* stageOut[4] = {b->C2, b->C3, b->C4, b->C5};
-    size_t bi = 0;
     for (int st = 0; st < 4; ++st)
-        for (int blk = 0; blk < nblocks[st]; ++blk, bi += 4) {
-            const int c1 = h->blockConv[bi], c2 = h->blockConv[bi + 1], c3 = h->blockConv[bi + 2], sc = h->blockConv[bi + 3];
+        for (int blk = 0; blk < nblocks[st]; ++blk) {
+            const int c1 = li, c2 = li + 1, c3 = li + 2, sc = blk == 0 ? li + 3 : -1;
+            li += blk == 0 ? 4 : 3;
             // pick three scratch buffers different from x
             __nv_bfloat16* t[3]; int n = 0;
             __nv_bfloat16* all[4] = {b->bufA, b->bufB, b->bufC, b->bufS};
@@ -674,37 +613,35 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
             __nv_bfloat16* y = last ? stageOut[st] : t[0];
             if (run_conv(b, c3, t[1], H1, W1, y, shortcut, 1, s)) return -2;
             x = y; H = H1; W = W1;
-            (void)pool;
         }
     // FPN
     const int fs[4] = {S / 4, S / 8, S / 16, S / 32};
     __nv_bfloat16* Cs[4] = {b->C2, b->C3, b->C4, b->C5};
+    const int fpnLat = li, fpnOut = li + 4;
     // P5 lateral
-    if (run_conv(b, h->fpnLat[3], Cs[3], fs[3], fs[3], b->td, nullptr, 0, s)) return -2;
+    if (run_conv(b, fpnLat + 3, Cs[3], fs[3], fs[3], b->td, nullptr, 0, s)) return -2;
     __nv_bfloat16* top = b->td;                       // running top-down map (pre-3x3)
     __nv_bfloat16* tdBuf[2] = {b->bufA, b->bufB};
-    if (run_conv(b, h->fpnOut[3], top, fs[3], fs[3], b->P[3], nullptr, 0, s)) return -2;
+    if (run_conv(b, fpnOut + 3, top, fs[3], fs[3], b->P[3], nullptr, 0, s)) return -2;
     for (int i = 2; i >= 0; --i) {
-        if (run_conv(b, h->fpnLat[i], Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s)) return -2;
+        if (run_conv(b, fpnLat + i, Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s)) return -2;
         __nv_bfloat16* nt = tdBuf[i & 1];
         prof_mark(s, "k_upsample_add"); k_upsample_add<<<8 * num_sms(), 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
         top = nt;
-        if (run_conv(b, h->fpnOut[i], top, fs[i], fs[i], b->P[i], nullptr, 0, s)) return -2;
+        if (run_conv(b, fpnOut + i, top, fs[i], fs[i], b->P[i], nullptr, 0, s)) return -2;
     }
     prof_mark(s, "k_subsample2"); k_subsample2<<<64, 256, 0, s>>>(b->P[3], fs[3], fs[3], 256, b->P[4]);       // P6
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_cnn_err = std::string("backbone forward: ") + cudaGetErrorString(e); return -3; }
-    return 0;
+    return cnn_check_launch("backbone forward") ? -3 : 0;
 }
-extern "C" double mf_backbone_flops(mf_backbone* h) { return h ? h->b.flops : 0; }
-extern "C" int mf_backbone_num_gemms(mf_backbone* h) { return h ? h->b.gemms : 0; }
-extern "C" void* mf_backbone_input_buffer(mf_backbone* h) { return h ? h->b.input : nullptr; }
+extern "C" double mf_backbone_flops(mf_backbone* h) { return h ? h->flops : 0; }
+extern "C" int mf_backbone_num_gemms(mf_backbone* h) { return h ? h->gemms : 0; }
+extern "C" void* mf_backbone_input_buffer(mf_backbone* h) { return h ? h->input.p : nullptr; }
 extern "C" void* mf_backbone_stream(mf_backbone* h) { return h ? (void*)h->stream : nullptr; }
 // level 0..3 = C2..C5, 4..8 = P2..P6; returns device pointer, fills dims (H, W, C)
 extern "C" void* mf_backbone_output(mf_backbone* h, int level, int* dims3)
 {
     if (!h) return nullptr;
-    Backbone* b = &h->b; const int S = b->S;
+    Backbone* b = h; const int S = b->S;
     const int fs[5] = {S / 4, S / 8, S / 16, S / 32, S / 64};
     const int cdim[4] = {256, 512, 1024, 2048};
     if (level >= 0 && level < 4) { dims3[0] = dims3[1] = fs[level]; dims3[2] = cdim[level]; __nv_bfloat16* c[4] = {b->C2, b->C3, b->C4, b->C5}; return c[level]; }
@@ -715,17 +652,16 @@ extern "C" int mf_backbone_download(mf_backbone* h, int level, void* host_bf16)
 {
     int d[3];
     void* p = mf_backbone_output(h, level, d);
-    if (!p) return -1;
-    cudaStreamSynchronize(h->stream);
-    return cudaMemcpy(host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -2;
+    if (!p) return cnn_fail("backbone: no handle or level outside 0..8");
+    return cnn_download(h->stream, host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2) ? -2 : 0;
 }
 // letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs)
 extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H)
 {
-    if (!h) return -1;
-    Backbone* b = &h->b; const int S = b->S;
+    if (!h) return cnn_fail("backbone: null handle");
+    Backbone* b = h; const int S = b->S;
     const MoldGeom g = cnn_mold_geometry(S, W, H);
     prof_mark(h->stream, "k_mold_input");
     k_mold_input<<<8 * num_sms(), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, g.scale, g.offx, g.offy, g.newW, g.newH, b->input);
-    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+    return cnn_check_launch("k_mold_input") ? -2 : 0;
 }

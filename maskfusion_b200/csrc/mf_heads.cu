@@ -26,6 +26,7 @@
 #include "../../include/maskfusion_b200.h"
 #include <cuda_bf16.h>
 #include <algorithm>
+#include <assert.h>
 #include <math.h>
 #include <string.h>
 #include <string>
@@ -36,15 +37,9 @@ namespace mfb {
 constexpr int DET_ROIS = 1000, DET_MAX = 100, NCLS = 81, FC_N = 1024, POOL = 7, CH = 256, HEAD_N = 448;
 constexpr int MPOOL = 14, MPIX = MPOOL * MPOOL, MASK = 28, MLOG_N = 128, MCONV_K = 9 * CH, SEL_N = 1024, EXPORT_CAP = 128;
 constexpr float DET_MIN_CONFIDENCE = 0.7f, DET_NMS_THRESHOLD = 0.3f;
-constexpr float HEAD_LOGIT_GAIN = 1e-3f, HEAD_DELTA_GAIN = 2e-5f, MASK_LOGIT_GAIN = 1e-3f;     // see mf_detector_create
 
-// layer table: FC1, FC2, heads, 4 mask convs, transposed conv, mask logits; rows = GEMM N (zero rows included)
+// the handle's layers in the order of its table (mf_weights.cu)
 enum { L_FC1, L_FC2, L_HEAD, L_M1, L_M2, L_M3, L_M4, L_DECONV, L_MLOG, N_LAYERS };
-struct LayerDef { int cin, cout, k, stride, pad, K, rows; };
-static const LayerDef LAYERS[N_LAYERS] = {
-    {CH, FC_N, POOL, 1, 0, POOL * POOL * CH, FC_N}, {FC_N, FC_N, 1, 1, 0, FC_N, FC_N}, {FC_N, NCLS * 5, 1, 1, 0, FC_N, HEAD_N},
-    {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH}, {CH, CH, 3, 1, 1, MCONV_K, CH},
-    {CH, CH, 2, 2, 0, CH, 4 * CH}, {CH, NCLS, 1, 1, 0, CH, MLOG_N}};
 
 struct ExportParams { double min_score; int n_filter, n_special; int filter[EXPORT_CAP], special[EXPORT_CAP]; };
 
@@ -219,47 +214,38 @@ __global__ void k_frame_masks(const uint4* __restrict__ idimg, const int* __rest
     if (threadIdx.x == 0) { hdr->nMasks = n; hdr->detectError = err; }
 }
 
-static int det_fail(const std::string& msg) { cnn_set_error(msg.c_str()); return -1; }
-
-static int check_launch(const char* what)
-{
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return det_fail(std::string(what) + ": " + cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace mfb
 
 using namespace mfb;
 
 struct mf_detector {
-    mf_rpn* rpn = nullptr;
-    mf_backbone* bb = nullptr;
-    cudaStream_t s = nullptr;
+    mf_rpn* rpn;
+    mf_backbone* bb;
+    cudaStream_t s;
+    WeightStore w;
     int S = 0, imgW = 0, imgH = 0;
     float4 win = make_float4(0.f, 0.f, 1.f, 1.f);             // letter-box window of the current image, normalised (norm_boxes)
     ExportParams ep;
-    std::vector<float> hW[N_LAYERS], hB[N_LAYERS];           // fp32 master copies [rows x K] (bf16-representable), biases [rows]
-    __nv_bfloat16* dW[N_LAYERS] = {};
-    float* dB[N_LAYERS] = {};
-    __nv_bfloat16 *fc1 = nullptr, *fc2 = nullptr, *mpool = nullptr, *col = nullptr, *mconv[4] = {}, *dec = nullptr;
-    float *head = nullptr, *mlog = nullptr, *masks = nullptr, *dets = nullptr, *scores = nullptr;
-    float4 *boxes = nullptr, *dboxes = nullptr;
-    unsigned long long* keys = nullptr;
-    int *count = nullptr, *ebox = nullptr, *ecls = nullptr, *erois = nullptr, *einfo = nullptr;
-    uint8_t *eid = nullptr, *idimg = nullptr;
-    size_t idcap = 0;
+    DevBuf<__nv_bfloat16> fc1, fc2, mpool, col, mconv[4], dec;
+    DevBuf<float> head, mlog, masks, dets, scores;
+    DevBuf<float4> boxes, dboxes;
+    DevBuf<unsigned long long> keys;
+    DevBuf<int> count, ebox, ecls, erois, einfo;
+    DevBuf<uint8_t> eid, idimg;                               // idimg: sized for the largest image so far
+    mf_detector(mf_rpn* rpn, unsigned seed);                  // throws CudaError
 };
 
 // the image geometry: the letter-box window of a W x H image in the S x S input, normalised as norm_boxes does (float64 divide, float32)
 static int set_image(mf_detector* h, int W, int H)
 {
-    if (W < 1 || H < 1 || W > 16384 || H > 16384) return det_fail("detector: image size " + std::to_string(W) + "x" + std::to_string(H) + " outside [1, 16384]");
-    if ((size_t)W * H > h->idcap) {
-        if (h->idimg && (cudaStreamSynchronize(h->s) != cudaSuccess || cudaFree(h->idimg) != cudaSuccess)) return det_fail("detector: id image free failed");
-        h->idimg = nullptr; h->idcap = 0;
-        if (cudaMalloc(&h->idimg, (size_t)W * H) != cudaSuccess) return det_fail("detector: id image cudaMalloc failed");
-        h->idcap = (size_t)W * H;
+    if (W < 1 || H < 1 || W > 16384 || H > 16384) return cnn_fail("detector: image size " + std::to_string(W) + "x" + std::to_string(H) + " outside [1, 16384]");
+    if ((size_t)W * H > h->idimg.n) {
+        if (cudaStreamSynchronize(h->s) != cudaSuccess) return cnn_fail("detector: id image free failed");
+        try {
+            h->idimg.alloc((size_t)W * H);
+        } catch (const CudaError& e) {
+            return cnn_fail("detector: id image " + e.what);
+        }
     }
     const MoldGeom g = cnn_mold_geometry(h->S, W, H);
     const double s1 = (double)(h->S - 1);
@@ -276,18 +262,18 @@ int detector_reserve_image(mf_detector* h, int W, int H) { return set_image(h, W
 int detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr)
 {
     const size_t P = (size_t)h->imgW * h->imgH;
-    if (P % 16 || ((uintptr_t)mask & 15)) return det_fail("detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer");
+    if (P % 16 || ((uintptr_t)mask & 15)) return cnn_fail("detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer");
     const int n16 = (int)(P / 16);
     prof_mark(h->s, "k_frame_masks");
-    k_frame_masks<<<(n16 + 255) / 256, 256, 0, h->s>>>((const uint4*)h->idimg, h->einfo, h->ecls, n16, (uint4*)mask, hdr);
-    return check_launch("k_frame_masks");
+    k_frame_masks<<<(n16 + 255) / 256, 256, 0, h->s>>>((const uint4*)h->idimg.p, h->einfo, h->ecls, n16, (uint4*)mask, hdr);
+    return cnn_check_launch("k_frame_masks");
 }
 }  // namespace mfb
 
 static int gemm(mf_detector* h, int layer, const void* A, void* out, int M, int relu, bool f32)
 {
-    const LayerDef& L = LAYERS[layer];
-    return launch_gemm_bf16(A, h->dW[layer], h->dB[layer], nullptr, out, M, L.rows, L.K, relu, h->s, nullptr, f32) ? -2 : 0;
+    const LayerGeom L = mrcnn_layer(MRCNN_DETECTOR, layer);
+    return launch_gemm_bf16(A, h->w.w(layer), h->w.b(layer), nullptr, out, M, L.rows, L.K, relu, h->s, nullptr, f32) ? -2 : 0;
 }
 
 static int refine(mf_detector* h, const float* rois, const float* logits, int lstride, const float* deltas, int dstride, int n)
@@ -296,7 +282,7 @@ static int refine(mf_detector* h, const float* rois, const float* logits, int ls
     k_det_refine<<<(n + 127) / 128, 128, 0, h->s>>>((const float4*)rois, logits, lstride, deltas, dstride, n, h->win, h->keys, h->boxes, h->scores);
     prof_mark(h->s, "k_det_select");
     k_det_select<<<1, SEL_N, 0, h->s>>>(h->keys, n, h->boxes, h->scores, h->dets, h->dboxes, h->count);
-    return check_launch("detection layer") ? -3 : 0;
+    return cnn_check_launch("detection layer") ? -3 : 0;
 }
 
 static int paste(mf_detector* h, const float* dets, const float* masks)
@@ -305,85 +291,55 @@ static int paste(mf_detector* h, const float* dets, const float* masks)
     k_unmold<<<1, 1, 0, h->s>>>(dets, h->win, h->imgW, h->imgH, h->ep, h->ebox, h->eid, h->ecls, h->erois, h->einfo);
     prof_mark(h->s, "k_paste");
     k_paste<<<(h->imgW * h->imgH + 255) / 256, 256, 0, h->s>>>(masks, h->ebox, h->eid, h->einfo, h->imgW, h->imgH, h->idimg);
-    return check_launch("id image") ? -3 : 0;
+    return cnn_check_launch("id image") ? -3 : 0;
 }
 
 // ==========================================================================================
 // C ABI (declared in include/maskfusion_b200.h)
 // ==========================================================================================
-extern "C" void mf_detector_destroy(mf_detector* h)
+mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed)
+    : rpn(rpn_), bb(rpn_backbone(rpn_)), s((cudaStream_t)mf_backbone_stream(bb)), w(MRCNN_DETECTOR, seed, s)
 {
-    if (!h) return;
-    for (int i = 0; i < N_LAYERS; ++i) { if (h->dW[i]) cudaFree(h->dW[i]); if (h->dB[i]) cudaFree(h->dB[i]); }
-    void* ptrs[] = {h->fc1, h->fc2, h->mpool, h->col, h->mconv[0], h->mconv[1], h->mconv[2], h->mconv[3], h->dec, h->head, h->mlog, h->masks,
-                    h->dets, h->scores, h->boxes, h->dboxes, h->keys, h->count, h->ebox, h->ecls, h->erois, h->einfo, h->eid, h->idimg};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    delete h;
+    const LayerGeom fc1L = mrcnn_layer(MRCNN_DETECTOR, L_FC1), headL = mrcnn_layer(MRCNN_DETECTOR, L_HEAD), m1 = mrcnn_layer(MRCNN_DETECTOR, L_M1),
+                    decL = mrcnn_layer(MRCNN_DETECTOR, L_DECONV), mlogL = mrcnn_layer(MRCNN_DETECTOR, L_MLOG);
+    assert(mrcnn_num_layers(MRCNN_DETECTOR) == N_LAYERS && fc1L.rows == FC_N && fc1L.K == POOL * POOL * CH && headL.rows == HEAD_N &&
+           m1.rows == CH && m1.K == MCONV_K && decL.rows == 4 * CH && mlogL.rows == MLOG_N);     // the shapes the buffers and kernels assume
+    int d[3];
+    mf_backbone_output(bb, 4, d);
+    S = d[0] * 4;
+    memset(&ep, 0, sizeof ep);
+    ep.min_score = 0.55;
+    const size_t mrows = (size_t)DET_MAX * MPIX;
+    fc1.alloc((size_t)DET_ROIS * FC_N); fc2.alloc((size_t)DET_ROIS * FC_N); head.alloc((size_t)DET_ROIS * HEAD_N); keys.alloc(DET_ROIS);
+    boxes.alloc(DET_ROIS); scores.alloc(DET_ROIS); dets.alloc(DET_MAX * 6); dboxes.alloc(DET_MAX); count.alloc(1);
+    mpool.alloc(mrows * CH); col.alloc(mrows * MCONV_K); dec.alloc(mrows * 4 * CH); mlog.alloc(mrows * 4 * MLOG_N);
+    masks.alloc(DET_MAX * MASK * MASK); ebox.alloc(DET_MAX * 5); ecls.alloc(DET_MAX); erois.alloc(DET_MAX * 4); einfo.alloc(2); eid.alloc(DET_MAX);
+    for (int i = 0; i < 4; ++i) mconv[i].alloc(mrows * CH);
+    cudaCheck(cudaMemset(dets, 0, DET_MAX * 6 * 4), "cudaMemset");
+    cudaCheck(cudaMemset(count, 0, 4), "cudaMemset");
+    cudaCheck(cudaMemset(masks, 0, DET_MAX * MASK * MASK * 4), "cudaMemset");
+    cudaCheck(cudaMemset(einfo, 0, 8), "cudaMemset");
 }
 
 extern "C" mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed)
 {
-    if (!rpn) { det_fail("detector: no region-proposal handle"); return nullptr; }
-    mf_detector* h = new mf_detector;
-    h->rpn = rpn;
-    h->bb = rpn_backbone(rpn);
-    h->s = (cudaStream_t)mf_backbone_stream(h->bb);
-    int d[3];
-    mf_backbone_output(h->bb, 4, d);
-    h->S = d[0] * 4;
-    memset(&h->ep, 0, sizeof h->ep);
-    h->ep.min_score = 0.55;
-    // weights: FC1, FC2, the mask convs and the transposed conv at gain 1 (He-style, the backbone's scheme).  Their synthetic outputs are
-    // O(1000) (the pooled features carry the pixel-unit scale of the moulded input), so the output layers are damped: class logits of a
-    // few units (at gain 1 every softmax saturates; far below, the 81-way softmax stays near uniform and no ROI reaches the 0.7
-    // confidence), |delta| ~ 0.15 (refined boxes stay near their proposals), mask logits of a few units (mask pixels on both sides of 0.5).
-    uint32_t sd = seed ? seed : 1u;
-    for (int i = 0; i < N_LAYERS; ++i) {
-        const LayerDef& L = LAYERS[i];
-        h->hW[i].assign((size_t)L.rows * L.K, 0.f);
-        h->hB[i].assign(L.rows, 0.f);
-        if (i == L_HEAD) {
-            synth_weights(h->hW[i].data(), h->hB[i].data(), NCLS, L.K, HEAD_LOGIT_GAIN, sd);
-            synth_weights(h->hW[i].data() + (size_t)NCLS * L.K, h->hB[i].data() + NCLS, 4 * NCLS, L.K, HEAD_DELTA_GAIN, sd);
-        } else if (i == L_MLOG) {
-            synth_weights(h->hW[i].data(), h->hB[i].data(), NCLS, L.K, MASK_LOGIT_GAIN, sd);
-        } else if (i == L_DECONV) {
-            // conv-transpose kernel [dy][dx][cout][cin] as GEMM rows (dy * 2 + dx) * 256 + cout; one bias per output channel
-            synth_weights(h->hW[i].data(), h->hB[i].data(), L.rows, L.K, 1.0f, sd);
-            for (int r = CH; r < L.rows; ++r) h->hB[i][r] = h->hB[i][r % CH];
-        } else
-            synth_weights(h->hW[i].data(), h->hB[i].data(), L.rows, L.K, 1.0f, sd);
+    if (!rpn) { cnn_fail("detector: no region-proposal handle"); return nullptr; }
+    mf_detector* h;
+    try {
+        h = new mf_detector(rpn, seed);
+    } catch (const CudaError& e) {
+        cnn_fail("detector: " + e.what);
+        return nullptr;
     }
-    bool ok = true;
-    for (int i = 0; i < N_LAYERS && ok; ++i)
-        ok = cudaMalloc(&h->dW[i], h->hW[i].size() * 2) == cudaSuccess && cudaMalloc(&h->dB[i], h->hB[i].size() * 4) == cudaSuccess;
-    const size_t mrows = (size_t)DET_MAX * MPIX;
-    ok = ok && cudaMalloc(&h->fc1, (size_t)DET_ROIS * FC_N * 2) == cudaSuccess && cudaMalloc(&h->fc2, (size_t)DET_ROIS * FC_N * 2) == cudaSuccess &&
-         cudaMalloc(&h->head, (size_t)DET_ROIS * HEAD_N * 4) == cudaSuccess && cudaMalloc(&h->keys, DET_ROIS * 8) == cudaSuccess &&
-         cudaMalloc(&h->boxes, DET_ROIS * 16) == cudaSuccess && cudaMalloc(&h->scores, DET_ROIS * 4) == cudaSuccess &&
-         cudaMalloc(&h->dets, DET_MAX * 6 * 4) == cudaSuccess && cudaMalloc(&h->dboxes, DET_MAX * 16) == cudaSuccess &&
-         cudaMalloc(&h->count, 4) == cudaSuccess && cudaMalloc(&h->mpool, mrows * CH * 2) == cudaSuccess &&
-         cudaMalloc(&h->col, mrows * MCONV_K * 2) == cudaSuccess && cudaMalloc(&h->dec, mrows * 4 * CH * 2) == cudaSuccess &&
-         cudaMalloc(&h->mlog, mrows * 4 * MLOG_N * 4) == cudaSuccess && cudaMalloc(&h->masks, DET_MAX * MASK * MASK * 4) == cudaSuccess &&
-         cudaMalloc(&h->ebox, DET_MAX * 5 * 4) == cudaSuccess && cudaMalloc(&h->ecls, DET_MAX * 4) == cudaSuccess &&
-         cudaMalloc(&h->erois, DET_MAX * 16) == cudaSuccess && cudaMalloc(&h->einfo, 8) == cudaSuccess && cudaMalloc(&h->eid, DET_MAX) == cudaSuccess;
-    for (int i = 0; i < 4 && ok; ++i) ok = cudaMalloc(&h->mconv[i], mrows * CH * 2) == cudaSuccess;
-    if (!ok) { det_fail("detector: cudaMalloc failed"); mf_detector_destroy(h); return nullptr; }
-    for (int i = 0; i < N_LAYERS && ok; ++i) {
-        std::vector<__nv_bfloat16> w(h->hW[i].size());
-        for (size_t k = 0; k < w.size(); ++k) w[k] = __float2bfloat16(h->hW[i][k]);
-        ok = cudaMemcpy(h->dW[i], w.data(), w.size() * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
-             cudaMemcpy(h->dB[i], h->hB[i].data(), h->hB[i].size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-    }
-    ok = ok && cudaMemset(h->dets, 0, DET_MAX * 6 * 4) == cudaSuccess && cudaMemset(h->count, 0, 4) == cudaSuccess &&
-         cudaMemset(h->masks, 0, DET_MAX * MASK * MASK * 4) == cudaSuccess && cudaMemset(h->einfo, 0, 8) == cudaSuccess;
-    if (!ok || set_image(h, h->S, h->S)) { det_fail("detector: upload failed"); mf_detector_destroy(h); return nullptr; }
+    if (set_image(h, h->S, h->S)) { delete h; return nullptr; }
     return h;
 }
 
+extern "C" void mf_detector_destroy(mf_detector* h) { delete h; }
+
 extern "C" int mf_detector_run(mf_detector* h, int stages)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     const cudaStream_t s = h->s;
     if (stages & MF_DET_CLASSIFIER) {
         if (gemm(h, L_FC1, rpn_pooled(h->rpn), h->fc1, DET_ROIS, 1, false) || gemm(h, L_FC2, h->fc1, h->fc2, DET_ROIS, 1, false) ||
@@ -391,7 +347,7 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
     }
     if ((stages & MF_DET_DETECTIONS) && refine(h, rpn_rois(h->rpn), h->head, HEAD_N, h->head + NCLS, HEAD_N, DET_ROIS)) return -3;
     if (stages & MF_DET_MASKS) {
-        if (mf_roi_align_bf16(h->bb, (const float*)h->dboxes, DET_MAX, MPOOL, h->mpool)) return -3;
+        if (mf_roi_align_bf16(h->bb, (const float*)h->dboxes.p, DET_MAX, MPOOL, h->mpool)) return -3;
         const __nv_bfloat16* x = h->mpool;
         for (int i = 0; i < 4; ++i) {
             launch_im2col(x, DET_MAX, MPOOL, MPOOL, CH, MPOOL, MPOOL, 3, 1, 1, MCONV_K, h->col, s);
@@ -401,7 +357,7 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
         if (gemm(h, L_DECONV, x, h->dec, DET_MAX * MPIX, 1, false) || gemm(h, L_MLOG, h->dec, h->mlog, DET_MAX * MPIX * 4, 0, true)) return -2;
         prof_mark(s, "k_mask_select");
         k_mask_select<<<(DET_MAX * MASK * MASK + 255) / 256, 256, 0, s>>>(h->mlog, h->dets, h->masks);
-        if (check_launch("k_mask_select")) return -3;
+        if (cnn_check_launch("k_mask_select")) return -3;
     }
     if ((stages & MF_DET_ID_IMAGE) && paste(h, h->dets, h->masks)) return -3;
     return 0;
@@ -409,18 +365,18 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
 
 extern "C" int mf_detector_forward(mf_detector* h, int image_w, int image_h)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     if (set_image(h, image_w, image_h)) return -1;
     return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
 }
 
 extern "C" int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int H)
 {
-    if (!h) return det_fail("detector: null handle");
-    if (!d_rgba || ((uintptr_t)d_rgba & 3)) return det_fail("detector: the image needs a 4-byte aligned device pointer");
+    if (!h) return cnn_fail("detector: null handle");
+    if (!d_rgba || ((uintptr_t)d_rgba & 3)) return cnn_fail("detector: the image needs a 4-byte aligned device pointer");
     if (set_image(h, W, H)) return -1;
     if (mf_backbone_mold(h->bb, d_rgba, W, H) || mf_backbone_forward(h->bb, mf_backbone_input_buffer(h->bb)))
-        return det_fail(std::string("detector: backbone: ") + cnn_last_error());
+        return cnn_fail(std::string("detector: backbone: ") + cnn_last_error());
     if (mf_rpn_forward(h->rpn)) return -3;
     return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
 }
@@ -428,9 +384,9 @@ extern "C" int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int
 extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const int32_t* class_filter, int n_filter, const int32_t* special_assignments,
                                       int n_special)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     if (n_filter < 0 || n_special < 0 || n_filter > EXPORT_CAP || n_special > EXPORT_CAP || (n_filter && !class_filter) || (n_special && !special_assignments))
-        return det_fail("detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries");
+        return cnn_fail("detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries");
     ExportParams ep;
     memset(&ep, 0, sizeof ep);
     ep.min_score = min_score; ep.n_filter = n_filter; ep.n_special = n_special;
@@ -442,18 +398,18 @@ extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const in
 
 extern "C" int mf_detector_refine(mf_detector* h, const float* d_rois, const float* d_logits, const float* d_deltas, int n)
 {
-    if (!h) return det_fail("detector: null handle");
-    if (n < 1 || n > DET_ROIS) return det_fail("detector_refine: n = " + std::to_string(n) + " outside [1, 1000]");
+    if (!h) return cnn_fail("detector: null handle");
+    if (n < 1 || n > DET_ROIS) return cnn_fail("detector_refine: n = " + std::to_string(n) + " outside [1, 1000]");
     if (!d_rois || !d_logits || !d_deltas || ((uintptr_t)d_rois & 15) || ((uintptr_t)d_logits & 3) || ((uintptr_t)d_deltas & 3))
-        return det_fail("detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer");
+        return cnn_fail("detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer");
     return refine(h, d_rois, d_logits, NCLS, d_deltas, 4 * NCLS, n);
 }
 
 extern "C" int mf_detector_paste(mf_detector* h, const float* d_detections, const float* d_masks, int W, int H)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     if (!d_detections || !d_masks || ((uintptr_t)d_detections & 3) || ((uintptr_t)d_masks & 3))
-        return det_fail("detector_paste: detections and masks need 4-byte aligned device pointers");
+        return cnn_fail("detector_paste: detections and masks need 4-byte aligned device pointers");
     if (set_image(h, W, H)) return -1;
     return paste(h, d_detections, d_masks);
 }
@@ -462,120 +418,76 @@ extern "C" int mf_detector_num_layers(mf_detector* h) { return h ? N_LAYERS : -1
 
 extern "C" int mf_detector_layer(mf_detector* h, int i, int* out6)
 {
-    if (!h || i < 0 || i >= N_LAYERS || !out6) return det_fail("detector: bad layer index");
-    const LayerDef& L = LAYERS[i];
+    if (!h || i < 0 || i >= N_LAYERS || !out6) return cnn_fail("detector: bad layer index");
+    const LayerGeom L = mrcnn_layer(MRCNN_DETECTOR, i);
     out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
     return 0;
 }
 
 extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* bias)
 {
-    if (!h || i < 0 || i >= N_LAYERS) return det_fail("detector: bad layer index");
-    if (w) memcpy(w, h->hW[i].data(), h->hW[i].size() * 4);
-    if (bias) memcpy(bias, h->hB[i].data(), h->hB[i].size() * 4);
-    return 0;
+    return h ? h->w.get(i, w, bias) : cnn_fail("detector: bad layer index");
 }
 
 // pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
 extern "C" int mf_detector_load_weights(mf_detector* h, const char* path)
 {
-    if (!h) return det_fail("detector: null handle");
-    if (mrcnn_layer_count(MRCNN_DETECTOR) != N_LAYERS) return det_fail("detector: the weight-name table does not match the layer table");
-    std::vector<float> hW[N_LAYERS], hB[N_LAYERS];
-    float *w[N_LAYERS], *b[N_LAYERS];
-    for (int i = 0; i < N_LAYERS; ++i) {
-        int rows, K;
-        mrcnn_layer_dims(MRCNN_DETECTOR, i, &rows, &K);
-        if (rows != LAYERS[i].rows || K != LAYERS[i].K) return det_fail("detector: the weight-name table does not match layer " + std::to_string(i));
-        hW[i].resize((size_t)rows * K); hB[i].resize(rows);
-        w[i] = hW[i].data(); b[i] = hB[i].data();
-    }
-    if (mrcnn_fold(path, MRCNN_DETECTOR, w, b)) return -1;
-    cudaError_t e = cudaSuccess;
-    std::vector<__nv_bfloat16> wbf[N_LAYERS];
-    for (int i = 0; i < N_LAYERS && e == cudaSuccess; ++i) {
-        wbf[i].resize(hW[i].size());
-        for (size_t k = 0; k < hW[i].size(); ++k) wbf[i][k] = __float2bfloat16(hW[i][k]);
-        e = cudaMemcpyAsync(h->dW[i], wbf[i].data(), wbf[i].size() * 2, cudaMemcpyHostToDevice, h->s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(h->dB[i], hB[i].data(), hB[i].size() * 4, cudaMemcpyHostToDevice, h->s);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->s);
-    if (e != cudaSuccess) return det_fail(std::string("detector: weight upload: ") + cudaGetErrorString(e));
-    for (int i = 0; i < N_LAYERS; ++i) { h->hW[i].swap(hW[i]); h->hB[i].swap(hB[i]); }
-    return 0;
-}
-
-static int download(mf_detector* h, void* dst, const void* src, size_t bytes)
-{
-    if (!dst) return 0;
-    if (cudaStreamSynchronize(h->s) != cudaSuccess || cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return det_fail(std::string("detector download: ") + cudaGetErrorString(cudaGetLastError()));
-    return 0;
+    return h ? h->w.load(path, h->s) : cnn_fail("detector: null handle");
 }
 
 extern "C" int mf_detector_get_fc(mf_detector* h, void* fc1_bf16, void* fc2_bf16)
 {
-    if (!h) return det_fail("detector: null handle");
-    return download(h, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2) || download(h, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2) ? -1 : 0;
+    if (!h) return cnn_fail("detector: null handle");
+    return cnn_download(h->s, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2) || cnn_download(h->s, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2) ? -1 : 0;
 }
 
 extern "C" int mf_detector_get_head_outputs(mf_detector* h, float* logits, float* deltas)
 {
-    if (!h) return det_fail("detector: null handle");
-    std::vector<float> head((size_t)DET_ROIS * HEAD_N);
-    if (download(h, head.data(), h->head, head.size() * 4)) return -1;
-    for (int r = 0; r < DET_ROIS; ++r) {
-        if (logits) memcpy(logits + (size_t)r * NCLS, &head[(size_t)r * HEAD_N], NCLS * 4);
-        if (deltas) memcpy(deltas + (size_t)r * NCLS * 4, &head[(size_t)r * HEAD_N + NCLS], NCLS * 16);
-    }
-    return 0;
+    if (!h) return cnn_fail("detector: null handle");
+    return cnn_download(h->s, logits, h->head, NCLS * 4, DET_ROIS, HEAD_N * 4) ||
+                   cnn_download(h->s, deltas, h->head.p + NCLS, NCLS * 16, DET_ROIS, HEAD_N * 4) ? -1 : 0;
 }
 
 extern "C" int mf_detector_get_mask_layer(mf_detector* h, int i, void* host)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     const size_t px = (size_t)DET_MAX * MPIX;
     switch (i) {
-    case 0: return download(h, host, h->mpool, px * CH * 2);
-    case 1: case 2: case 3: case 4: return download(h, host, h->mconv[i - 1], px * CH * 2);
-    case 5: return download(h, host, h->dec, px * 4 * CH * 2);
-    case 6: {
-        std::vector<float> m(px * 4 * MLOG_N);
-        if (download(h, m.data(), h->mlog, m.size() * 4)) return -1;
-        for (size_t r = 0; r < px * 4; ++r) memcpy((float*)host + r * NCLS, &m[r * MLOG_N], NCLS * 4);
-        return 0;
-    }
-    default: return det_fail("detector: mask layer must be 0..6");
+    case 0: return cnn_download(h->s, host, h->mpool, px * CH * 2);
+    case 1: case 2: case 3: case 4: return cnn_download(h->s, host, h->mconv[i - 1], px * CH * 2);
+    case 5: return cnn_download(h->s, host, h->dec, px * 4 * CH * 2);
+    case 6: return cnn_download(h->s, host, h->mlog, NCLS * 4, px * 4, MLOG_N * 4);
+    default: return cnn_fail("detector: mask layer must be 0..6");
     }
 }
 
 extern "C" int mf_detector_get_detections(mf_detector* h, float* detections)
 {
     int n = 0;
-    if (!h) return det_fail("detector: null handle");
-    if (download(h, detections, h->dets, DET_MAX * 6 * 4) || download(h, &n, h->count, 4)) return -1;
+    if (!h) return cnn_fail("detector: null handle");
+    if (cnn_download(h->s, detections, h->dets, DET_MAX * 6 * 4) || cnn_download(h->s, &n, h->count, 4)) return -1;
     return n;
 }
 
 extern "C" int mf_detector_get_masks(mf_detector* h, float* masks)
 {
-    return h ? download(h, masks, h->masks, DET_MAX * MASK * MASK * 4) : det_fail("detector: null handle");
+    return h ? cnn_download(h->s, masks, h->masks, DET_MAX * MASK * MASK * 4) : cnn_fail("detector: null handle");
 }
 
 extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32_t* class_ids, int32_t* rois)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     int info[2];
-    if (download(h, info, h->einfo, 8)) return -1;
-    if (info[1]) return det_fail("generate_id_image: special_assignments[class_id] out of range");
-    if (download(h, id_image, h->idimg, (size_t)h->imgW * h->imgH) || download(h, class_ids, h->ecls, (size_t)info[0] * 4) ||
-        download(h, rois, h->erois, (size_t)info[0] * 16)) return -1;
+    if (cnn_download(h->s, info, h->einfo, 8)) return -1;
+    if (info[1]) return cnn_fail("generate_id_image: special_assignments[class_id] out of range");
+    if (cnn_download(h->s, id_image, h->idimg, (size_t)h->imgW * h->imgH) || cnn_download(h->s, class_ids, h->ecls, (size_t)info[0] * 4) ||
+        cnn_download(h->s, rois, h->erois, (size_t)info[0] * 16)) return -1;
     return info[0];
 }
 
 extern "C" int mf_detector_image_size(mf_detector* h, int* w, int* hgt)
 {
-    if (!h) return det_fail("detector: null handle");
+    if (!h) return cnn_fail("detector: null handle");
     *w = h->imgW; *hgt = h->imgH;
     return 0;
 }

@@ -24,21 +24,6 @@ Mat4 rigidInverse(const Mat4& T);
 Mat4 mul(const Mat4& A, const Mat4& B);
 Rt toRt(const Mat4& T);
 
-struct CudaError { std::string what; };
-void cudaCheck(cudaError_t e, const char* where);
-
-template <typename T>
-struct DevBuf {
-    T* p = nullptr; size_t n = 0;
-    DevBuf() {}
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() { if (p) cudaFree(p); }
-    void alloc(size_t count) { if (p) cudaFree(p); p = nullptr; n = count; if (count) cudaCheck(cudaMalloc((void**)&p, count * sizeof(T)), "cudaMalloc"); }
-    void zero(cudaStream_t s) { if (n) cudaCheck(cudaMemsetAsync(p, 0, n * sizeof(T), s), "memset"); }
-    operator T*() const { return p; }
-};
-
 struct Profiler {
     bool on = false; int used = 0;
     std::vector<cudaEvent_t> events; std::vector<const char*> names;

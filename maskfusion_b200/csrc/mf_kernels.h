@@ -2,7 +2,10 @@
 // structures they share with the host classes (mf_host.cu).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
+#include <string>
+#include <vector>
 #include "mf_common.cuh"
 
 struct mf_backbone;
@@ -12,6 +15,21 @@ struct mf_detector;
 namespace mfb {
 
 struct SurfelPlanes { float4* pos; float4* col; float4* nrm; };
+
+struct CudaError { std::string what; };
+void cudaCheck(cudaError_t e, const char* where);        // throws CudaError
+
+template <typename T>
+struct DevBuf {
+    T* p = nullptr; size_t n = 0;
+    DevBuf() {}
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+    void alloc(size_t count) { if (p) cudaFree(p); p = nullptr; n = 0; if (count) cudaCheck(cudaMalloc((void**)&p, count * sizeof(T)), "cudaMalloc"); n = count; }
+    void zero(cudaStream_t s) { if (n) cudaCheck(cudaMemsetAsync(p, 0, n * sizeof(T), s), "memset"); }
+    operator T*() const { return p; }
+};
 
 // photometric correspondence record (reference: DataTerm, Core/Cuda/types.cuh:75-81)
 struct DataTerm { short2 zero; short2 one; float diff; int valid; };
@@ -166,22 +184,40 @@ void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout
 struct MoldGeom { float scale; int newW, newH, offx, offy; };
 MoldGeom cnn_mold_geometry(int S, int W, int H);
 const char* cnn_last_error();
-void cnn_set_error(const char* msg);
+// what the backbone, RPN and detector handles share: the message into cnn_last_error() and -1; a failed launch; a read-back of `rows` rows
+// of `width` bytes, `pitch` bytes apart on the device (0: one block), packed into dst after `s` is drained.  dst NULL: nothing is copied
+int cnn_fail(const std::string& msg);
+int cnn_check_launch(const char* what);
+int cnn_download(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows = 1, size_t pitch = 0);
 
 // ---- mf_rpn.cu: what the detection heads read of the RPN handle ----
 mf_backbone* rpn_backbone(mf_rpn* h);
 const float* rpn_rois(mf_rpn* h);                 // [1000][4] proposals, zero padded
 const void* rpn_pooled(mf_rpn* h);                // [1000][7][7][256] bf16
-// seeded He-style weights [rows x K] (bf16-representable) and biases, the backbone's scheme (mf_cnn.cu add_conv)
-void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed);
 
-// ---- mf_weights.cu: pretrained Mask R-CNN weights (safetensors, R-FOLD) for the three handles' layer tables ----
+// ---- mf_weights.cu: the layer table of the three Mask R-CNN handles and their weights (seeded, or pretrained: safetensors, R-FOLD) ----
 enum { MRCNN_BACKBONE, MRCNN_RPN, MRCNN_DETECTOR };
-int mrcnn_layer_count(int part);                             // the handle's layers, in its table order
-void mrcnn_layer_dims(int part, int i, int* rows, int* K);   // table of layer i: [rows x K] weights, [rows] bias
-// reads, checks and folds every layer of `part` from the file into w[i] / b[i] (sized by mrcnn_layer_dims); 0, or -1 with the message in
-// cnn_last_error() naming the file and the tensor
-int mrcnn_fold(const char* path, int part, float* const* w, float* const* b);
+// layer i of a handle, in its table order: input channels, GEMM rows (output channels and zero rows), kernel side, stride, pad, GEMM K
+// (kh * kw * Cin zero padded).  The weights are [rows x K], (ky, kx, cin) along K; the bias [rows]
+struct LayerGeom { int cin, rows, k, stride, pad, K; };
+int mrcnn_num_layers(int part);
+LayerGeom mrcnn_layer(int part, int i);
+// every table of one handle in one pool: fp32 master copies (bf16-representable) on the host, bf16 weights and fp32 biases on the device
+struct WeightStore {
+    int part;
+    std::vector<size_t> wOff, bOff;               // layer i: first element of its table / bias (128-byte aligned in the pools)
+    std::vector<float> hW, hB;
+    DevBuf<__nv_bfloat16> dW;
+    DevBuf<float> dB;
+    // the seeded tables (one LCG stream, seed 0 taken as 1), uploaded on `s`; throws CudaError
+    WeightStore(int part, unsigned seed, cudaStream_t s);
+    // every layer read, checked and folded on the host, uploaded on `s` and complete on return; the tables change only on success.
+    // 0, or -1 with the message in cnn_last_error() naming the file and the tensor (-2: the upload failed)
+    int load(const char* path, cudaStream_t s);
+    int get(int i, float* w, float* b, int rows = -1) const;    // the first `rows` rows (-1: all) of layer i; NULL skips
+    const __nv_bfloat16* w(int i) const { return dW.p + wOff[i]; }
+    const float* b(int i) const { return dB.p + bOff[i]; }
+};
 
 // ---- mf_heads.cu: the detector on the frame path (mf_attach_detector) ----
 cudaStream_t detector_stream(mf_detector* h);

@@ -25,6 +25,7 @@
 #include "../../include/maskfusion_b200.h"
 #include <cuda_bf16.h>
 #include <algorithm>
+#include <assert.h>
 #include <math.h>
 #include <string.h>
 #include <string>
@@ -217,43 +218,23 @@ __global__ void __launch_bounds__(128) k_roi_align(const float4* __restrict__ bo
     }
 }
 
-static uint32_t lcg(uint32_t& s) { s = s * 1664525u + 1013904223u; return s; }
-static float urand(uint32_t& s) { return (float)(lcg(s) >> 8) * (1.0f / 16777216.0f) * 2.f - 1.f; }
-static float bf16_round(float f) { return __bfloat162float(__float2bfloat16(f)); }
-
-void synth_weights(float* w, float* b, int rows, int K, float gain, uint32_t& seed)
-{
-    const float sc = gain * sqrtf(2.0f / (float)K);
-    for (int o = 0; o < rows; ++o)
-        for (int kk = 0; kk < K; ++kk) w[(size_t)o * K + kk] = bf16_round(urand(seed) * sc * 1.7320508f);
-    for (int o = 0; o < rows; ++o) b[o] = urand(seed) * 0.05f;
-}
-
-static int rpn_fail(const std::string& msg) { cnn_set_error(msg.c_str()); return -1; }
-
-static int check_launch(const char* what)
-{
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return rpn_fail(std::string(what) + ": " + cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace mfb
 
 using namespace mfb;
 
 struct mf_rpn {
-    mf_backbone* bb = nullptr;
-    cudaStream_t s = nullptr;
+    mf_backbone* bb;
+    cudaStream_t s;
+    WeightStore w;                                           // conv [512 x 2304], heads [64 x 512] (rows >= 18 zero)
     int S = 0, A = 0, pixels = 0;
     int lh[5] = {}, pixOff[6] = {};                          // P2..P6 side length, first pixel of each level in the concatenation
-    std::vector<float> hWc, hBc, hWh, hBh;                   // conv [512 x 2304], heads [64 x 512] (rows >= 18 zero), fp32 master copies
-    __nv_bfloat16 *dWc = nullptr, *dWh = nullptr, *col = nullptr, *conv = nullptr, *pooled = nullptr;
-    float *dBc = nullptr, *dBh = nullptr, *head = nullptr, *logits = nullptr, *deltas = nullptr, *anchors = nullptr, *rois = nullptr;
-    unsigned long long *keys = nullptr, *sel = nullptr, *mask = nullptr;
-    SelState* st = nullptr;
-    float4* boxes = nullptr;
-    int* count = nullptr;
+    DevBuf<__nv_bfloat16> col, conv, pooled;
+    DevBuf<float> head, logits, deltas, anchors, rois;
+    DevBuf<unsigned long long> keys, sel, mask;
+    DevBuf<SelState> st;
+    DevBuf<float4> boxes;
+    DevBuf<int> count;
+    mf_rpn(mf_backbone* bb, unsigned seed);                  // throws CudaError
 };
 
 static RoiLevels roi_levels(mf_backbone* bb)
@@ -276,7 +257,7 @@ static int roi_align(mf_backbone* bb, const float* boxes, int n, int pool, void*
     const float areaScale = (float)((double)S * (double)S / (224.0 * 224.0));
     prof_mark(s, "k_roi_align");
     k_roi_align<<<dim3(n, pool), RPN_CH / 2, 0, s>>>((const float4*)boxes, pool, roi_levels(bb), areaScale, (__nv_bfloat16*)out);
-    return check_launch("k_roi_align");
+    return cnn_check_launch("k_roi_align");
 }
 
 // the proposal layer on logits [n][2], deltas [n][4], anchors [n][4] (device) -> h->rois [1000][4], h->count
@@ -307,55 +288,34 @@ static int propose(mf_rpn* h, const float* logits, const float* deltas, const fl
     prof_mark(s, "k_nms_mask");
     k_nms_mask<<<dim3(words, words), 64, 0, s>>>(h->boxes, k, words, h->mask);
     prof_mark(s, "k_nms_scan");
-    k_nms_scan<<<1, 32, 0, s>>>(h->boxes, h->mask, k, words, (float4*)h->rois, h->count);
-    return check_launch("proposal layer");
+    k_nms_scan<<<1, 32, 0, s>>>(h->boxes, h->mask, k, words, (float4*)h->rois.p, h->count);
+    return cnn_check_launch("proposal layer");
 }
 
 // ==========================================================================================
 // C ABI (declared in include/maskfusion_b200.h)
 // ==========================================================================================
-extern "C" void mf_rpn_destroy(mf_rpn* h)
+mf_rpn::mf_rpn(mf_backbone* bb_, unsigned seed) : bb(bb_), s((cudaStream_t)mf_backbone_stream(bb_)), w(MRCNN_RPN, seed, s)
 {
-    if (!h) return;
-    void* ptrs[] = {h->dWc, h->dWh, h->col, h->conv, h->pooled, h->dBc, h->dBh, h->head, h->logits, h->deltas, h->anchors, h->rois,
-                    h->keys, h->sel, h->mask, h->st, h->boxes, h->count};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    delete h;
-}
-
-extern "C" mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed)
-{
-    if (!bb) { rpn_fail("rpn: no backbone"); return nullptr; }
-    mf_rpn* h = new mf_rpn;
-    h->bb = bb;
-    h->s = (cudaStream_t)mf_backbone_stream(bb);
+    const LayerGeom c = mrcnn_layer(MRCNN_RPN, 0), hd = mrcnn_layer(MRCNN_RPN, 1);
+    assert(c.cin == RPN_CH && c.rows == RPN_MID && hd.K == RPN_MID && hd.rows == RPN_HEAD_N);     // the shapes the kernels are compiled for
     int d[3];
     mf_backbone_output(bb, 4, d);
-    h->S = d[0] * 4;
+    S = d[0] * 4;
     for (int l = 0; l < 5; ++l) {
-        h->lh[l] = h->S >> (l + 2);
-        h->pixOff[l + 1] = h->pixOff[l] + h->lh[l] * h->lh[l];
+        lh[l] = S >> (l + 2);
+        pixOff[l + 1] = pixOff[l] + lh[l] * lh[l];
     }
-    h->pixels = h->pixOff[5];
-    h->A = 3 * h->pixels;
-    // weights: shared conv (gain 1).  The synthetic P levels are O(100) (the moulded input is in pixel units), and so is the conv output:
-    // the class-logit layer is damped to logits of a few units (scores spread over (0, 1) instead of saturating at 0 / 1) and the delta
-    // layer to |delta| ~ 0.1 (decoded boxes stay near their anchors)
-    uint32_t sd = seed ? seed : 1u;
-    const int Kc = 9 * RPN_CH;
-    h->hWc.assign((size_t)RPN_MID * Kc, 0.f); h->hBc.assign(RPN_MID, 0.f);
-    h->hWh.assign((size_t)RPN_HEAD_N * RPN_MID, 0.f); h->hBh.assign(RPN_HEAD_N, 0.f);
-    synth_weights(h->hWc.data(), h->hBc.data(), RPN_MID, Kc, 1.0f, sd);
-    synth_weights(h->hWh.data(), h->hBh.data(), 6, RPN_MID, 2e-4f, sd);
-    synth_weights(h->hWh.data() + 6 * RPN_MID, h->hBh.data() + 6, 12, RPN_MID, 2e-5f, sd);
+    pixels = pixOff[5];
+    A = 3 * pixels;
     // anchors: generate_pyramid_anchors + norm_boxes in double, rounded once to float; order (level, y, x, ratio)
-    std::vector<float> anc((size_t)h->A * 4);
-    const double ratios[3] = {0.5, 1.0, 2.0}, S1 = (double)(h->S - 1);
+    std::vector<float> anc((size_t)A * 4);
+    const double ratios[3] = {0.5, 1.0, 2.0}, S1 = (double)(S - 1);
     size_t a = 0;
     for (int l = 0; l < 5; ++l) {
         const double scale = 32.0 * (1 << l), stride = 4.0 * (1 << l);
-        for (int y = 0; y < h->lh[l]; ++y)
-            for (int x = 0; x < h->lh[l]; ++x)
+        for (int y = 0; y < lh[l]; ++y)
+            for (int x = 0; x < lh[l]; ++x)
                 for (int r = 0; r < 3; ++r, ++a) {
                     const double bh = scale / sqrt(ratios[r]), bw = scale * sqrt(ratios[r]), cy = y * stride, cx = x * stride;
                     anc[a * 4 + 0] = (float)((cy - 0.5 * bh) / S1);
@@ -367,48 +327,47 @@ extern "C" mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed)
     // im2col scratch only for the levels whose shape the implicit 3x3 path refuses
     size_t colElems = 0;
     for (int l = 0; l < 5; ++l)
-        if (!cnn_conv_implicit(3, 1, 1, RPN_CH, h->lh[l], h->lh[l])) colElems = std::max(colElems, (size_t)h->lh[l] * h->lh[l] * Kc);
-    const size_t A = h->A;
-    bool ok = cudaMalloc(&h->dWc, h->hWc.size() * 2) == cudaSuccess && cudaMalloc(&h->dWh, h->hWh.size() * 2) == cudaSuccess &&
-              cudaMalloc(&h->dBc, RPN_MID * 4) == cudaSuccess && cudaMalloc(&h->dBh, RPN_HEAD_N * 4) == cudaSuccess &&
-              (colElems == 0 || cudaMalloc(&h->col, colElems * 2) == cudaSuccess) &&
-              cudaMalloc(&h->conv, (size_t)h->pixels * RPN_MID * 2) == cudaSuccess && cudaMalloc(&h->head, (size_t)h->pixels * RPN_HEAD_N * 4) == cudaSuccess &&
-              cudaMalloc(&h->logits, A * 2 * 4) == cudaSuccess && cudaMalloc(&h->deltas, A * 4 * 4) == cudaSuccess &&
-              cudaMalloc(&h->anchors, A * 4 * 4) == cudaSuccess && cudaMalloc(&h->keys, A * 8) == cudaSuccess &&
-              cudaMalloc(&h->sel, RPN_PRE_NMS * 8) == cudaSuccess && cudaMalloc(&h->mask, (size_t)RPN_PRE_NMS * NMS_WORDS * 8) == cudaSuccess &&
-              cudaMalloc(&h->st, sizeof(SelState)) == cudaSuccess && cudaMalloc(&h->boxes, RPN_PRE_NMS * 16) == cudaSuccess &&
-              cudaMalloc(&h->rois, RPN_POST_NMS * 16) == cudaSuccess && cudaMalloc(&h->count, 4) == cudaSuccess &&
-              cudaMalloc(&h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) == cudaSuccess;
-    if (!ok) { rpn_fail("rpn: cudaMalloc failed"); mf_rpn_destroy(h); return nullptr; }
-    std::vector<__nv_bfloat16> wc(h->hWc.size()), wh(h->hWh.size());
-    for (size_t i = 0; i < wc.size(); ++i) wc[i] = __float2bfloat16(h->hWc[i]);
-    for (size_t i = 0; i < wh.size(); ++i) wh[i] = __float2bfloat16(h->hWh[i]);
-    ok = cudaMemcpy(h->dWc, wc.data(), wc.size() * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(h->dWh, wh.data(), wh.size() * 2, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(h->dBc, h->hBc.data(), RPN_MID * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(h->dBh, h->hBh.data(), RPN_HEAD_N * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(h->anchors, anc.data(), anc.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemset(h->rois, 0, RPN_POST_NMS * 16) == cudaSuccess && cudaMemset(h->count, 0, 4) == cudaSuccess &&
-         cudaFuncSetAttribute(k_sort_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, SORT_CAP * (int)sizeof(unsigned long long)) == cudaSuccess;
-    if (!ok) { rpn_fail("rpn: upload failed"); mf_rpn_destroy(h); return nullptr; }
-    return h;
+        if (!cnn_conv_implicit(3, 1, 1, RPN_CH, lh[l], lh[l])) colElems = std::max(colElems, (size_t)lh[l] * lh[l] * c.K);
+    col.alloc(colElems);
+    conv.alloc((size_t)pixels * RPN_MID); head.alloc((size_t)pixels * RPN_HEAD_N);
+    logits.alloc((size_t)A * 2); deltas.alloc((size_t)A * 4); anchors.alloc((size_t)A * 4); keys.alloc(A);
+    sel.alloc(RPN_PRE_NMS); mask.alloc((size_t)RPN_PRE_NMS * NMS_WORDS); st.alloc(1); boxes.alloc(RPN_PRE_NMS);
+    rois.alloc(RPN_POST_NMS * 4); count.alloc(1); pooled.alloc((size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH);
+    cudaCheck(cudaMemcpy(anchors, anc.data(), anc.size() * 4, cudaMemcpyHostToDevice), "anchor upload");
+    cudaCheck(cudaMemset(rois, 0, RPN_POST_NMS * 16), "cudaMemset");
+    cudaCheck(cudaMemset(count, 0, 4), "cudaMemset");
+    cudaCheck(cudaFuncSetAttribute(k_sort_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, SORT_CAP * (int)sizeof(unsigned long long)),
+              "cudaFuncSetAttribute");
 }
+
+extern "C" mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed)
+{
+    if (!bb) { cnn_fail("rpn: no backbone"); return nullptr; }
+    try {
+        return new mf_rpn(bb, seed);
+    } catch (const CudaError& e) {
+        cnn_fail("rpn: " + e.what);
+        return nullptr;
+    }
+}
+
+extern "C" void mf_rpn_destroy(mf_rpn* h) { delete h; }
 
 extern "C" int mf_rpn_run(mf_rpn* h, int stages)
 {
-    if (!h) return rpn_fail("rpn: null handle");
+    if (!h) return cnn_fail("rpn: null handle");
     const cudaStream_t s = h->s;
     if (stages & MF_RPN_CONV)
         for (int l = 0; l < 5; ++l) {
             int d[3];
             const void* in = mf_backbone_output(h->bb, 4 + l, d);
-            if (cnn_conv(in, d[0], d[1], RPN_CH, RPN_MID, 3, 1, 1, h->dWc, h->dBc, h->col, h->conv + (size_t)h->pixOff[l] * RPN_MID, 1, s)) return -2;
+            if (cnn_conv(in, d[0], d[1], RPN_CH, RPN_MID, 3, 1, 1, h->w.w(0), h->w.b(0), h->col, h->conv.p + (size_t)h->pixOff[l] * RPN_MID, 1, s)) return -2;
         }
     if (stages & MF_RPN_HEADS) {
-        if (launch_gemm_bf16(h->conv, h->dWh, h->dBh, nullptr, h->head, h->pixels, RPN_HEAD_N, RPN_MID, 0, s, nullptr, true)) return -2;
+        if (launch_gemm_bf16(h->conv, h->w.w(1), h->w.b(1), nullptr, h->head, h->pixels, RPN_HEAD_N, RPN_MID, 0, s, nullptr, true)) return -2;
         prof_mark(s, "k_rpn_split");
         k_rpn_split<<<std::min((h->pixels * 18 + 255) / 256, 8 * num_sms()), 256, 0, s>>>(h->head, h->pixels, h->logits, h->deltas);
-        if (check_launch("k_rpn_split")) return -3;
+        if (cnn_check_launch("k_rpn_split")) return -3;
     }
     if ((stages & MF_RPN_PROPOSALS) && propose(h, h->logits, h->deltas, h->anchors, h->A)) return -3;
     if ((stages & MF_RPN_ROI_ALIGN) && roi_align(h->bb, h->rois, RPN_POST_NMS, RPN_POOL, h->pooled, s)) return -3;
@@ -419,20 +378,20 @@ extern "C" int mf_rpn_forward(mf_rpn* h) { return mf_rpn_run(h, MF_RPN_CONV | MF
 
 extern "C" int mf_rpn_propose(mf_rpn* h, const float* d_logits, const float* d_deltas, const float* d_anchors, int n_anchors)
 {
-    if (!h) return rpn_fail("rpn: null handle");
+    if (!h) return cnn_fail("rpn: null handle");
     if (n_anchors < 1 || n_anchors > h->A)
-        return rpn_fail("rpn_propose: n_anchors = " + std::to_string(n_anchors) + " outside [1, " + std::to_string(h->A) + "]");
+        return cnn_fail("rpn_propose: n_anchors = " + std::to_string(n_anchors) + " outside [1, " + std::to_string(h->A) + "]");
     if (!d_logits || !d_deltas || !d_anchors || ((uintptr_t)d_logits & 7) || ((uintptr_t)d_deltas & 15) || ((uintptr_t)d_anchors & 15))
-        return rpn_fail("rpn_propose: logits need 8-byte, deltas and anchors 16-byte aligned device pointers");
+        return cnn_fail("rpn_propose: logits need 8-byte, deltas and anchors 16-byte aligned device pointers");
     return propose(h, d_logits, d_deltas, d_anchors, n_anchors) ? -3 : 0;
 }
 
 extern "C" int mf_roi_align_bf16(mf_backbone* bb, const float* d_boxes, int n, int pool, void* d_out)
 {
-    if (!bb) return rpn_fail("roi_align: no backbone");
-    if (n < 0 || pool < 2 || pool > 64) return rpn_fail("roi_align: need n >= 0 and 2 <= pool <= 64");
+    if (!bb) return cnn_fail("roi_align: no backbone");
+    if (n < 0 || pool < 2 || pool > 64) return cnn_fail("roi_align: need n >= 0 and 2 <= pool <= 64");
     if (n > 0 && (!d_boxes || !d_out || ((uintptr_t)d_boxes & 15) || ((uintptr_t)d_out & 3)))
-        return rpn_fail("roi_align: boxes need a 16-byte, out a 4-byte aligned device pointer");
+        return cnn_fail("roi_align: boxes need a 16-byte, out a 4-byte aligned device pointer");
     return roi_align(bb, d_boxes, n, pool, d_out, (cudaStream_t)mf_backbone_stream(bb)) ? -3 : 0;
 }
 
@@ -440,76 +399,45 @@ extern "C" int mf_rpn_num_anchors(mf_rpn* h) { return h ? h->A : -1; }
 
 extern "C" int mf_rpn_get_weights(mf_rpn* h, float* conv_w, float* conv_b, float* head_w, float* head_b)
 {
-    if (!h) return rpn_fail("rpn: null handle");
-    if (conv_w) memcpy(conv_w, h->hWc.data(), h->hWc.size() * 4);
-    if (conv_b) memcpy(conv_b, h->hBc.data(), h->hBc.size() * 4);
-    if (head_w) memcpy(head_w, h->hWh.data(), (size_t)18 * RPN_MID * 4);
-    if (head_b) memcpy(head_b, h->hBh.data(), 18 * 4);
-    return 0;
+    if (!h) return cnn_fail("rpn: null handle");
+    return h->w.get(0, conv_w, conv_b) || h->w.get(1, head_w, head_b, 18) ? -1 : 0;     // head rows 0..5 logits, 6..17 deltas
 }
 
 // pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
 extern "C" int mf_rpn_load_weights(mf_rpn* h, const char* path)
 {
-    if (!h) return rpn_fail("rpn: null handle");
-    std::vector<float> wc(h->hWc.size()), bc(h->hBc.size()), wh(h->hWh.size()), bh(h->hBh.size());
-    float* w[2] = {wc.data(), wh.data()};
-    float* b[2] = {bc.data(), bh.data()};
-    int rows[2], K[2];
-    for (int i = 0; i < 2; ++i) mrcnn_layer_dims(MRCNN_RPN, i, &rows[i], &K[i]);
-    if (mrcnn_layer_count(MRCNN_RPN) != 2 || (size_t)rows[0] * K[0] != wc.size() || (size_t)rows[1] * K[1] != wh.size())
-        return rpn_fail("rpn: the weight-name table does not match the handle's tables");
-    if (mrcnn_fold(path, MRCNN_RPN, w, b)) return -1;
-    std::vector<__nv_bfloat16> wcb(wc.size()), whb(wh.size());
-    for (size_t i = 0; i < wc.size(); ++i) wcb[i] = __float2bfloat16(wc[i]);
-    for (size_t i = 0; i < wh.size(); ++i) whb[i] = __float2bfloat16(wh[i]);
-    cudaError_t e = cudaMemcpyAsync(h->dWc, wcb.data(), wcb.size() * 2, cudaMemcpyHostToDevice, h->s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dWh, whb.data(), whb.size() * 2, cudaMemcpyHostToDevice, h->s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dBc, bc.data(), bc.size() * 4, cudaMemcpyHostToDevice, h->s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->dBh, bh.data(), bh.size() * 4, cudaMemcpyHostToDevice, h->s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->s);
-    if (e != cudaSuccess) return rpn_fail(std::string("rpn: weight upload: ") + cudaGetErrorString(e));
-    h->hWc.swap(wc); h->hBc.swap(bc); h->hWh.swap(wh); h->hBh.swap(bh);
-    return 0;
-}
-
-static int download(mf_rpn* h, void* dst, const void* src, size_t bytes)
-{
-    if (!h) return rpn_fail("rpn: null handle");
-    if (cudaStreamSynchronize(h->s) != cudaSuccess || cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return rpn_fail(std::string("rpn download: ") + cudaGetErrorString(cudaGetLastError()));
-    return 0;
+    return h ? h->w.load(path, h->s) : cnn_fail("rpn: null handle");
 }
 
 extern "C" int mf_rpn_get_anchors(mf_rpn* h, float* anchors)
 {
-    return h ? download(h, anchors, h->anchors, (size_t)h->A * 16) : rpn_fail("rpn: null handle");
+    return h ? cnn_download(h->s, anchors, h->anchors, (size_t)h->A * 16) : cnn_fail("rpn: null handle");
 }
 
 extern "C" int mf_rpn_get_head_outputs(mf_rpn* h, float* logits, float* deltas)
 {
-    if (!h) return rpn_fail("rpn: null handle");
-    return download(h, logits, h->logits, (size_t)h->A * 8) || download(h, deltas, h->deltas, (size_t)h->A * 16) ? -1 : 0;
+    if (!h) return cnn_fail("rpn: null handle");
+    return cnn_download(h->s, logits, h->logits, (size_t)h->A * 8) || cnn_download(h->s, deltas, h->deltas, (size_t)h->A * 16) ? -1 : 0;
 }
 
 extern "C" int mf_rpn_download_conv(mf_rpn* h, int level, void* host_bf16)
 {
-    if (!h) return rpn_fail("rpn: null handle");
-    if (level < 0 || level > 4) return rpn_fail("rpn: level must be 0..4 (P2..P6)");
-    return download(h, host_bf16, h->conv + (size_t)h->pixOff[level] * RPN_MID, (size_t)h->lh[level] * h->lh[level] * RPN_MID * 2);
+    if (!h) return cnn_fail("rpn: null handle");
+    if (level < 0 || level > 4) return cnn_fail("rpn: level must be 0..4 (P2..P6)");
+    return cnn_download(h->s, host_bf16, h->conv.p + (size_t)h->pixOff[level] * RPN_MID, (size_t)h->lh[level] * h->lh[level] * RPN_MID * 2);
 }
 
 extern "C" int mf_rpn_get_proposals(mf_rpn* h, float* rois)
 {
     int n = 0;
-    if (!h) return rpn_fail("rpn: null handle");
-    if (download(h, rois, h->rois, RPN_POST_NMS * 16) || download(h, &n, h->count, 4)) return -1;
+    if (!h) return cnn_fail("rpn: null handle");
+    if (cnn_download(h->s, rois, h->rois, RPN_POST_NMS * 16) || cnn_download(h->s, &n, h->count, 4)) return -1;
     return n;
 }
 
 extern "C" int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16)
 {
-    return h ? download(h, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) : rpn_fail("rpn: null handle");
+    return h ? cnn_download(h->s, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) : cnn_fail("rpn: null handle");
 }
 
 // ---- what the detection heads (mf_heads.cu) read of the handle ----

@@ -1,5 +1,5 @@
-// mf_weights.cu -- pretrained Mask R-CNN weights from a safetensors file into the layer tables of the backbone, RPN and detector handles
-// (host code only).  DESIGN §3c has the name table and the folding rule R-FOLD.
+// mf_weights.cu -- the layer table of the Mask R-CNN backbone, RPN and detector handles and their weight store: seeded tables, or
+// pretrained weights from a safetensors file (host code only).  DESIGN §3c has the name table and the folding rule R-FOLD.
 //
 // File: an 8-byte little-endian header length N, N bytes of JSON {name: {"dtype", "shape", "data_offsets"}, "__metadata__": {str: str}},
 // then the data section; data_offsets are [begin, end) byte offsets into that section.  The JSON is parsed by a reader of exactly this
@@ -12,6 +12,7 @@
 // and s = 1, b' = (float)bias for a layer without BatchNorm.  Compiled with -ffp-contract=off: no fused multiply-add changes a rounding.
 #include "mf_kernels.h"
 #include <cuda_bf16.h>
+#include <assert.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -23,75 +24,92 @@ namespace {
 
 struct Tensor { std::string dtype; std::vector<long long> shape; long long begin = 0, end = 0; };
 
-// one source array of a handle layer: its Keras name, its Keras shape, the first GEMM row it fills
-struct Part { std::string layer; std::vector<long long> shape; int row0; };
+// one source array of a handle layer: its Keras name, its Keras shape, the first GEMM row it fills, the gain of its seeded rows
+struct Part { std::string layer; std::vector<long long> shape; int row0; float gain; };
 struct LayerSpec {
     std::string name;                 // the handle layer's name: the Keras layer, or "a+b" for two layers stacked in one GEMM
     std::vector<Part> parts;
     std::string bn;                   // BatchNorm layer folded into it ("" = none)
-    int rows, K;                      // the handle's table: [rows x K], zero padded
+    int stride, pad;
     bool deconv;                      // Conv2DTranspose (kh, kw, out, in): row (dy*kw + dx)*out + o, column c; bias repeated per (dy, dx)
+    int rows, K;                      // the handle's table: [rows x K], zero padded to the GEMM's multiples of 64
 };
 
-LayerSpec conv(const std::string& name, int kh, int kw, int cin, int cout, const std::string& bn, int rows, int K)
+int kpad(long long n) { return (int)((n + 63) / 64 * 64); }
+
+long long part_cout(const LayerSpec& s, const Part& pt) { return s.deconv ? pt.shape[2] : pt.shape.back(); }
+long long part_rows(const LayerSpec& s, const Part& pt) { return s.deconv ? pt.shape[0] * pt.shape[1] * pt.shape[2] : pt.shape.back(); }
+long long part_cols(const LayerSpec& s, const Part& pt)      // K used: kh * kw * cin, the input width of a dense layer, cin of the deconv
 {
-    LayerSpec s;
-    s.name = name; s.parts = {{name, {kh, kw, cin, cout}, 0}}; s.bn = bn; s.rows = rows; s.K = K; s.deconv = false;
+    if (s.deconv) return pt.shape[3];
+    long long cols = 1;
+    for (size_t d = 0; d + 1 < pt.shape.size(); ++d) cols *= pt.shape[d];
+    return cols;
+}
+
+LayerSpec layer(const std::string& name, std::vector<Part> parts, const std::string& bn, int stride, int pad, bool deconv = false)
+{
+    LayerSpec s{name, std::move(parts), bn, stride, pad, deconv, 0, 0};
+    const Part& last = s.parts.back();
+    s.rows = kpad(last.row0 + part_rows(s, last));
+    s.K = kpad(part_cols(s, last));
     return s;
 }
 
-int kpad(int K) { return (K + 63) / 64 * 64; }
+LayerSpec conv(const std::string& name, int k, int cin, int cout, const std::string& bn, int stride, int pad, float gain)
+{
+    return layer(name, {{name, {k, k, cin, cout}, 0, gain}}, bn, stride, pad);
+}
 
-// the backbone's layer table order (mf_backbone_create): conv1, per block branch2a, 2b, 2c (+ branch1 in block a), fpn_c2p2..c5p5, fpn_p2..p5
+// ResNet-101 (stages 3, 4, 23, 3; the stride in the first 1x1 of a stage, as in Keras/matterport) + FPN(256).  Seeded at gain 1 (He-style:
+// activations stay O(1) through 101 layers) except branch2c at 0.5 (the residual sums keep O(1) variance) and the shortcut and lateral 1x1
+// convs at 0.7.  Order: conv1, per block branch2a, 2b, 2c (+ branch1 in block a), fpn_c2p2..c5p5, fpn_p2..p5
 std::vector<LayerSpec> backbone_specs()
 {
     std::vector<LayerSpec> v;
-    v.push_back(conv("conv1", 7, 7, 3, 64, "bn_conv1", 64, kpad(7 * 7 * 3)));
+    v.push_back(conv("conv1", 7, 3, 64, "bn_conv1", 2, 3, 1.0f));
     const int nblocks[4] = {3, 4, 23, 3}, mid[4] = {64, 128, 256, 512};
     int cin = 64;
     for (int st = 0; st < 4; ++st)
         for (int blk = 0; blk < nblocks[st]; ++blk) {
-            const int f = mid[st], cout = 4 * f;
+            const int f = mid[st], cout = 4 * f, stride = (blk == 0 && st > 0) ? 2 : 1;
             const std::string id = std::to_string(st + 2) + (char)('a' + blk) + "_branch";
-            v.push_back(conv("res" + id + "2a", 1, 1, cin, f, "bn" + id + "2a", f, kpad(cin)));
-            v.push_back(conv("res" + id + "2b", 3, 3, f, f, "bn" + id + "2b", f, kpad(9 * f)));
-            v.push_back(conv("res" + id + "2c", 1, 1, f, cout, "bn" + id + "2c", cout, kpad(f)));
-            if (blk == 0) v.push_back(conv("res" + id + "1", 1, 1, cin, cout, "bn" + id + "1", cout, kpad(cin)));
+            v.push_back(conv("res" + id + "2a", 1, cin, f, "bn" + id + "2a", stride, 0, 1.0f));
+            v.push_back(conv("res" + id + "2b", 3, f, f, "bn" + id + "2b", 1, 1, 1.0f));
+            v.push_back(conv("res" + id + "2c", 1, f, cout, "bn" + id + "2c", 1, 0, 0.5f));
+            if (blk == 0) v.push_back(conv("res" + id + "1", 1, cin, cout, "bn" + id + "1", stride, 0, 0.7f));
             cin = cout;
         }
     const int cdim[4] = {256, 512, 1024, 2048};
-    for (int i = 0; i < 4; ++i) v.push_back(conv("fpn_c" + std::to_string(i + 2) + "p" + std::to_string(i + 2), 1, 1, cdim[i], 256, "", 256, cdim[i]));
-    for (int i = 0; i < 4; ++i) v.push_back(conv("fpn_p" + std::to_string(i + 2), 3, 3, 256, 256, "", 256, 9 * 256));
+    for (int i = 0; i < 4; ++i) v.push_back(conv("fpn_c" + std::to_string(i + 2) + "p" + std::to_string(i + 2), 1, cdim[i], 256, "", 1, 0, 0.7f));
+    for (int i = 0; i < 4; ++i) v.push_back(conv("fpn_p" + std::to_string(i + 2), 3, 256, 256, "", 1, 1, 1.0f));
     return v;
 }
 
-// the RPN handle: shared 3x3 conv [512 x 2304]; class logits (6) and box deltas (12) as one GEMM of 64 rows
+// the RPN handle: shared 3x3 conv [512 x 2304]; class logits (6) and box deltas (12) as one GEMM of 64 rows.  The synthetic P levels are
+// O(100) (the moulded input is in pixel units), and so is the conv output: the seeded class-logit rows are damped to logits of a few units
+// (scores spread over (0, 1) instead of saturating at 0 / 1), the delta rows to |delta| ~ 0.1 (decoded boxes stay near their anchors)
 std::vector<LayerSpec> rpn_specs()
 {
-    LayerSpec head;
-    head.name = "rpn_class_raw+rpn_bbox_pred";
-    head.parts = {{"rpn_class_raw", {1, 1, 512, 6}, 0}, {"rpn_bbox_pred", {1, 1, 512, 12}, 6}};
-    head.rows = 64; head.K = 512; head.deconv = false;
-    return {conv("rpn_conv_shared", 3, 3, 256, 512, "", 512, 9 * 256), head};
+    return {conv("rpn_conv_shared", 3, 256, 512, "", 1, 1, 1.0f),
+            layer("rpn_class_raw+rpn_bbox_pred", {{"rpn_class_raw", {1, 1, 512, 6}, 0, 2e-4f}, {"rpn_bbox_pred", {1, 1, 512, 12}, 6, 2e-5f}}, "", 1, 0)};
 }
 
-// the detector handle, mf_heads.cu LAYERS order: FC1, FC2, class logits + box deltas, 4 mask convs, transposed conv, mask logits
+// the detector handle: FC1, FC2, class logits + box deltas, 4 mask convs, transposed conv, mask logits.  Seeded at gain 1 except the output
+// layers: the synthetic FC and mask-conv outputs are O(1000) (the pooled features carry the pixel-unit scale of the moulded input), so the
+// class logits are damped to a few units (at gain 1 every softmax saturates; far below, the 81-way softmax stays near uniform and no ROI
+// reaches the 0.7 confidence), the deltas to |delta| ~ 0.15 (refined boxes stay near their proposals), the mask logits to a few units
+// (mask pixels on both sides of 0.5)
 std::vector<LayerSpec> detector_specs()
 {
     std::vector<LayerSpec> v;
-    v.push_back(conv("mrcnn_class_conv1", 7, 7, 256, 1024, "mrcnn_class_bn1", 1024, 7 * 7 * 256));
-    v.push_back(conv("mrcnn_class_conv2", 1, 1, 1024, 1024, "mrcnn_class_bn2", 1024, 1024));
-    LayerSpec head;
-    head.name = "mrcnn_class_logits+mrcnn_bbox_fc";
-    head.parts = {{"mrcnn_class_logits", {1024, 81}, 0}, {"mrcnn_bbox_fc", {1024, 324}, 81}};
-    head.rows = 448; head.K = 1024; head.deconv = false;
-    v.push_back(head);
+    v.push_back(conv("mrcnn_class_conv1", 7, 256, 1024, "mrcnn_class_bn1", 1, 0, 1.0f));
+    v.push_back(conv("mrcnn_class_conv2", 1, 1024, 1024, "mrcnn_class_bn2", 1, 0, 1.0f));
+    v.push_back(layer("mrcnn_class_logits+mrcnn_bbox_fc", {{"mrcnn_class_logits", {1024, 81}, 0, 1e-3f}, {"mrcnn_bbox_fc", {1024, 324}, 81, 2e-5f}}, "", 1, 0));
     for (int i = 1; i <= 4; ++i)
-        v.push_back(conv("mrcnn_mask_conv" + std::to_string(i), 3, 3, 256, 256, "mrcnn_mask_bn" + std::to_string(i), 256, 9 * 256));
-    LayerSpec dec;
-    dec.name = "mrcnn_mask_deconv"; dec.parts = {{"mrcnn_mask_deconv", {2, 2, 256, 256}, 0}}; dec.rows = 4 * 256; dec.K = 256; dec.deconv = true;
-    v.push_back(dec);
-    v.push_back(conv("mrcnn_mask", 1, 1, 256, 81, "", 128, 256));
+        v.push_back(conv("mrcnn_mask_conv" + std::to_string(i), 3, 256, 256, "mrcnn_mask_bn" + std::to_string(i), 1, 1, 1.0f));
+    v.push_back(layer("mrcnn_mask_deconv", {{"mrcnn_mask_deconv", {2, 2, 256, 256}, 0, 1.0f}}, "", 2, 0, true));
+    v.push_back(conv("mrcnn_mask", 1, 256, 81, "", 1, 0, 1e-3f));
     return v;
 }
 
@@ -99,6 +117,38 @@ const std::vector<LayerSpec>& specs(int part)
 {
     static const std::vector<LayerSpec> t[3] = {backbone_specs(), rpn_specs(), detector_specs()};
     return t[part];
+}
+
+float bf16_rn(float f) { return __bfloat162float(__float2bfloat16(f)); }
+
+// the relayout of one part into its layer's table, shared by the file (fold) and the seeded generator: row r < part_rows of the part is
+// table row row0 + r and takes bf16_rn(wv(r, j)) in its first part_cols columns j, in that order; then its biases bv(r), in row order
+template <typename WV, typename BV>
+void relayout(const LayerSpec& s, const Part& pt, float* w, float* b, WV wv, BV bv)
+{
+    const long long rows = part_rows(s, pt), cols = part_cols(s, pt);
+    for (long long r = 0; r < rows; ++r) {
+        float* row = w + (size_t)(pt.row0 + r) * s.K;
+        for (long long j = 0; j < cols; ++j) row[j] = bf16_rn(wv(r, j));
+    }
+    for (long long r = 0; r < rows; ++r) b[pt.row0 + r] = bv(r);
+}
+
+struct Lcg {
+    uint32_t s;
+    float urand() { s = s * 1664525u + 1013904223u; return (float)(s >> 8) * (1.0f / 16777216.0f) * 2.f - 1.f; }
+};
+
+// the seeded layer (tables zeroed by the caller): per part, He-style uniform weights of gain * sqrt(2 / K used), then biases of +-0.05
+void seed_layer(const LayerSpec& s, Lcg& g, float* w, float* b)
+{
+    for (const Part& pt : s.parts) {
+        const float sc = pt.gain * sqrtf(2.0f / (float)part_cols(s, pt));
+        relayout(s, pt, w, b, [&](long long, long long) { return g.urand() * sc * 1.7320508f; }, [&](long long) { return g.urand() * 0.05f; });
+        const long long cout = part_cout(s, pt);
+        if (s.deconv)                    // all rows' biases are drawn, then every (dy, dx) takes the first one's
+            for (long long r = cout; r < part_rows(s, pt); ++r) b[pt.row0 + r] = b[pt.row0 + r % cout];
+    }
 }
 
 std::string shape_str(const std::vector<long long>& s)
@@ -307,7 +357,7 @@ struct WeightFile {
         memset(w, 0, (size_t)s.rows * s.K * sizeof(float));
         memset(b, 0, (size_t)s.rows * sizeof(float));
         for (const Part& pt : s.parts) {
-            const long long cout = s.deconv ? pt.shape[2] : pt.shape.back();
+            const long long cout = part_cout(s, pt), rows = part_rows(s, pt), cols = part_cols(s, pt);
             if (!read(pt.layer + "/kernel", pt.shape, kern) || !read(pt.layer + "/bias", {cout}, bias)) return false;
             scale.assign((size_t)cout, 1.0); shift.assign((size_t)cout, 0.0);
             if (!s.bn.empty()) {
@@ -320,21 +370,10 @@ struct WeightFile {
                 }
             } else
                 for (long long o = 0; o < cout; ++o) shift[o] = bias[o];
-            if (s.deconv) {                  // (kh, kw, out, in): already [row = (dy*kw + dx)*out + o][c]
-                const long long cin = pt.shape[3], taps = pt.shape[0] * pt.shape[1];
-                for (long long r = 0; r < taps * cout; ++r) {
-                    for (long long c = 0; c < cin; ++c) w[r * s.K + c] = __bfloat162float(__float2bfloat16(kern[r * cin + c]));
-                    b[r] = (float)shift[r % cout];
-                }
-                continue;
-            }
-            long long cols = 1;                  // (kh, kw, cin, cout) or (in, out): column j of output o is kern[j * cout + o]
-            for (size_t d = 0; d + 1 < pt.shape.size(); ++d) cols *= pt.shape[d];
-            for (long long o = 0; o < cout; ++o) {
-                float* row = w + (size_t)(pt.row0 + o) * s.K;
-                for (long long j = 0; j < cols; ++j) row[j] = __bfloat162float(__float2bfloat16((float)((double)kern[j * cout + o] * scale[o])));
-                b[pt.row0 + o] = (float)shift[o];
-            }
+            // (kh, kw, cin, cout) or (in, out): column j of output o is kern[j * cout + o]; the deconv's (kh, kw, out, in) is already
+            // [row = (dy*kw + dx)*out + o][c]
+            relayout(s, pt, w, b, [&](long long r, long long j) { return (float)((double)kern[s.deconv ? r * cols + j : j * rows + r] * scale[r % cout]); },
+                     [&](long long r) { return (float)shift[r % cout]; });
         }
         return true;
     }
@@ -344,20 +383,66 @@ struct WeightFile {
 
 namespace mfb {
 
-int mrcnn_layer_count(int part) { return (int)specs(part).size(); }
+static const char* const HANDLE_NAME[3] = {"backbone", "rpn", "detector"};
 
-void mrcnn_layer_dims(int part, int i, int* rows, int* K)
+int mrcnn_num_layers(int part) { return (int)specs(part).size(); }
+
+LayerGeom mrcnn_layer(int part, int i)
 {
     const LayerSpec& s = specs(part)[i];
-    *rows = s.rows; *K = s.K;
+    const std::vector<long long>& sh = s.parts[0].shape;
+    const int cin = (int)(s.deconv ? sh[3] : sh.size() == 4 ? sh[2] : sh[0]), k = sh.size() == 4 ? (int)sh[0] : 1;
+    return {cin, s.rows, k, s.stride, s.pad, s.K};
 }
 
-int mrcnn_fold(const char* path, int part, float* const* w, float* const* b)
+// bf16 weights and fp32 biases onto the device, complete on return
+static cudaError_t upload(const WeightStore& st, const std::vector<float>& w, const std::vector<float>& b, cudaStream_t s)
 {
+    std::vector<__nv_bfloat16> wbf(w.size());
+    for (size_t i = 0; i < wbf.size(); ++i) wbf[i] = __float2bfloat16(w[i]);
+    cudaError_t e = cudaMemcpyAsync(st.dW.p, wbf.data(), wbf.size() * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.dB.p, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return e;
+}
+
+WeightStore::WeightStore(int part_, unsigned seed, cudaStream_t s) : part(part_)
+{
+    const std::vector<LayerSpec>& t = specs(part);
+    size_t nw = 0, nb = 0;
+    for (const LayerSpec& l : t) {
+        assert(l.rows % 64 == 0 && l.K % 64 == 0);      // every table and bias starts 128-byte aligned (TMA maps of the GEMM's B operand)
+        wOff.push_back(nw); bOff.push_back(nb);
+        nw += (size_t)l.rows * l.K; nb += (size_t)l.rows;
+    }
+    hW.assign(nw, 0.f); hB.assign(nb, 0.f);
+    Lcg g{seed ? seed : 1u};
+    for (size_t i = 0; i < t.size(); ++i) seed_layer(t[i], g, &hW[wOff[i]], &hB[bOff[i]]);
+    dW.alloc(nw); dB.alloc(nb);
+    cudaCheck(upload(*this, hW, hB, s), "weight upload");
+}
+
+int WeightStore::load(const char* path, cudaStream_t s)
+{
+    const std::vector<LayerSpec>& t = specs(part);
+    std::vector<float> w(hW.size()), b(hB.size());
     WeightFile f;
     bool ok = f.open(path);
-    for (size_t i = 0; ok && i < specs(part).size(); ++i) ok = f.fold(specs(part)[i], w[i], b[i]);
-    if (!ok) { cnn_set_error(f.err.c_str()); return -1; }
+    for (size_t i = 0; ok && i < t.size(); ++i) ok = f.fold(t[i], &w[wOff[i]], &b[bOff[i]]);
+    if (!ok) return cnn_fail(f.err);
+    const cudaError_t e = upload(*this, w, b, s);
+    if (e != cudaSuccess) { cnn_fail(std::string(HANDLE_NAME[part]) + ": weight upload: " + cudaGetErrorString(e)); return -2; }
+    hW.swap(w); hB.swap(b);
+    return 0;
+}
+
+int WeightStore::get(int i, float* w, float* b, int rows) const
+{
+    if (i < 0 || i >= (int)wOff.size()) return cnn_fail(std::string(HANDLE_NAME[part]) + ": bad layer index");
+    const LayerSpec& l = specs(part)[i];
+    if (rows < 0) rows = l.rows;
+    if (w) memcpy(w, &hW[wOff[i]], (size_t)rows * l.K * sizeof(float));
+    if (b) memcpy(b, &hB[bOff[i]], (size_t)rows * sizeof(float));
     return 0;
 }
 
@@ -372,9 +457,8 @@ extern "C" int mf_mrcnn_read_layer(const char* path, const char* layer, float* w
             if (dims) { dims[0] = s.rows; dims[1] = s.K; }
             if (!w_rows_K || !bias_rows) return 0;
             WeightFile f;
-            if (!f.open(path) || !f.fold(s, w_rows_K, bias_rows)) { mfb::cnn_set_error(f.err.c_str()); return -1; }
+            if (!f.open(path) || !f.fold(s, w_rows_K, bias_rows)) return mfb::cnn_fail(f.err);
             return 0;
         }
-    mfb::cnn_set_error((std::string("mrcnn_read_layer: no layer named '") + (layer ? layer : "(null)") + "'").c_str());
-    return -1;
+    return mfb::cnn_fail(std::string("mrcnn_read_layer: no layer named '") + (layer ? layer : "(null)") + "'");
 }
