@@ -119,7 +119,8 @@ int mf_download_edge_map(mf_context* ctx, float* edge, uint8_t* binary);        
  * mask-id image (MfSegmentation.cpp:424-426); ellipse == 0: the binary edge-map close (segmentation.cu:217-255,334-354), `inverted` = 255 - result. */
 /* Mask R-CNN backbone on the frame path (MaskRCNN::executeSequential, MaskRCNN.cpp:147-151, called at MfSegmentation.cpp:130): every k-th
  * processFrame letter-boxes the frame's RGB image into `backbone`'s input (mf_backbone_mold) and enqueues its forward on the backbone's
- * own stream, concurrently with the dense pipeline on the same GPU.  backbone = handle of mf_backbone_create; NULL detaches. */
+ * own stream, concurrently with the dense pipeline on the same GPU.  backbone = handle of mf_backbone_create; NULL detaches.
+ * Refused: a -static context (it runs no segmentation to feed), and a context with a detector attached. */
 int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k);
 /* Mask R-CNN detector on the frame path: MfSegmentation::performSegmentation calls MaskRCNN::executeSequential when the frame has no mask
  * (MfSegmentation.cpp:128-131), which fills FrameData::mask with the id image and FrameData::classIDs with [0] followed by the exported class
@@ -180,7 +181,9 @@ int mf_model_class_id(mf_context* ctx, int i);                                /*
  *      models prefer ranks other than the detector rank (it counts one more tracked model in the placement rule). ---- */
 int mf_shard_configure(mf_context* ctx, int rank, int world);                 /* before the first frame; rank 0 owns the background model */
 int mf_shard_unique_id(uint8_t* out128);                                      /* ncclGetUniqueId (rank 0) */
-int mf_shard_comm_init(mf_context* ctx, const uint8_t* id128, int rank, int world);   /* ncclCommInitRank on the context's device (+ mf_shard_configure) */
+/* ncclCommInitRank on the context's device (+ mf_shard_configure).  Refused, whatever the world size: a -static context (one model, nothing
+ * to shard: run replicas), and a context with a detector attached by mf_attach_detector. */
+int mf_shard_comm_init(mf_context* ctx, const uint8_t* id128, int rank, int world);
 int mf_shard_process_frame(mf_context* ctx, const uint8_t* rgb, const float* depth, int64_t timestamp, const uint8_t* mask,
                            const int32_t* class_ids, int n_class_ids, float weight_multiplier,
                            int inputs_on_device);   /* inputs are read on rank 0 only (class_ids always from the host) */

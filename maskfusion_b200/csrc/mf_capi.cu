@@ -325,11 +325,7 @@ extern "C" int mf_download_edge_map(mf_context* ctx, float* edge, uint8_t* binar
 {
     MF_TRY MF_NEED(ctx)
     MaskFusion* o = ctx->mf;
-    if (!o->frameMapsValid) o->generateCUDATextures();
-    launch_geometric_edges(o->vmap[0], o->nmap[0], o->W, o->H, o->cfg.segWeightDistance, o->cfg.segWeightConvexity, o->cfg.segThreshold,
-                           o->edgeMap, o->edgeBinary, o->stream);
-    launch_morph_close_invert(o->edgeBinary, o->edgeBuf, o->W, o->H, o->cfg.segMorphEdgeRadius, o->cfg.segMorphEdgeIterations, o->edgeInv, o->stream);
-    o->launches += 2 + 2 * o->cfg.segMorphEdgeIterations;
+    o->edgeMaps();
     d2h(o, edge, o->edgeMap.p, o->P); d2h(o, binary, o->edgeInv.p, o->P);
     o->sync(); return 0;
     MF_CATCH(-1)

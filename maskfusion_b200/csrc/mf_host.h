@@ -139,9 +139,12 @@ public:
     bool pendingTrack = false, pendingLog = false; int64_t pendingTimestamp = 0; std::vector<Model*> pendingModels; cudaEvent_t trackDone = nullptr;
     // ---- multi-model path (MaskFusion.cpp:287-375) ----
     void globalProjection();                                                                      // GlobalProjection::project + downloadDirect (stays on the device)
+    void checkModelCount() const;                                                                 // the ID projection and segmentation hold up to 63 models
     void segTables();
+    void edgeMaps();                                                                              // MfSegmentation floatEdgeMap -> binary -> close -> invert
     void performSegmentation(bool allowNew);                                                      // MfSegmentation::performSegmentation (result -> FrameResult)
     unsigned char getNextModelID(bool assign);                                                    // MaskFusion::getNextModelID
+    void initFirstRGB(Model* m);                                                                  // RGBDOdometry::initFirstRGB of the current frame
     Model* spawnObjectModel();                                                                    // MaskFusion::spawnObjectModel + moveNewModelToList
     void setFrameClasses(const int32_t* ids, int n) { classIDs.assign(ids, ids + n); }            // FrameData::classIDs
 
@@ -170,13 +173,15 @@ public:
     // backbone's own stream, next to the dense pipeline of the same GPU (the reference runs its network as a ~5 Hz sidecar)
     void* backbone = nullptr; int backboneEvery = 0; cudaEvent_t bbFrameReady = nullptr, bbMoldDone = nullptr; bool bbMoldPending = false;
     void attachBackbone(void* bb, int everyK);
-    void runBackbone(cudaStream_t producer = nullptr);
     // Mask R-CNN detector on the frame path (MfSegmentation.cpp:128-131): a segmentation frame that the caller gave no mask runs the
     // detector every k-th tick on the detector's (= its backbone's) stream; k_frame_masks writes the id image and class list into the
     // frame's mask / header; the main stream waits (bbMoldDone, recorded behind the hand-off) just before segmentation reads them.
     mf_detector* detector = nullptr; int detectorEvery = 0; bool detWaitPending = false;
     void attachDetector(mf_detector* det, int everyK);
-    void runDetector(cudaStream_t producer, bool wanted);
+    // the backbone and the detector share one slot: one network stream, one event pair, the frame's image as input
+    void attachNetwork(const char* who, bool asDetector, mf_detector* det);
+    void runNetwork(cudaStream_t producer, bool detWanted);     // the attached network on this frame, behind `producer`
+    void waitHandoff(cudaStream_t s);                           // `s` waits for a pending detector hand-off (mask + header written)
     void waitDetector();                                        // the host waits for the last hand-off (it writes into an input set)
     // object-sharded run with a detector (mf_shard_attach_detector): `detector` is set on rank detRank only, detectorEvery on every rank.
     // A frame exchanges masks (fExchange) when detRank >= 0, the context is multi-model, the frame tracks and tick % detectorEvery == 0:
@@ -185,8 +190,11 @@ public:
     int detRank = -1; bool fExchange = false, maskCommPending = false;
     void attachShardDetector(mf_detector* det, int everyK, int detectorRank);
     bool shardFrameMasks(void** ptr, size_t* bytes);            // external transport: the range to broadcast from detRank on this frame
-    // multi-model frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
+    // overlapped frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
     bool spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
+    void waitMain(cudaStream_t s);                              // `s` waits for the work queued on the main stream so far
+    cudaStream_t commStream();                                  // the stream of the next collective, ordered behind the main stream
+    void joinComm(bool now);                                    // the main stream waits for it: now, or where segmentation reads the mask
     FrameResult* hRes = nullptr; DevBuf<FrameResult> dRes; cudaEvent_t resEvt = nullptr; bool pendingResult = false;
     DevBuf<float> poseTable, gathered;
     float fWeight = 1.f; int fTick = 0; bool fTracked = false;

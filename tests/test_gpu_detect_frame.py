@@ -243,21 +243,28 @@ def test_caller_mask_takes_precedence(nets, frames):
 
 def test_refusals(nets):
     import maskfusion_b200 as mfb
+    import torch
     det = nets(256)
+    bst = torch.cuda.Stream()
+    bb = mfb.Backbone(256, seed=3, stream=bst.cuda_stream)
     st = _ctx(enableMultipleModels=0)
+    L = st.L
     with pytest.raises(mfb.MFError, match="static"):
         st.attachDetector(det)
+    with pytest.raises(mfb.MFError, match="static"):
+        st.attachBackbone(bb, 5)
+    st.attachBackbone(None)
+    # a -static context never shards, not even as a one-rank communicator
+    uid = (C.c_uint8 * 128)()
+    assert L.mf_shard_unique_id(uid) == 0
+    assert L.mf_shard_comm_init(st.h, uid, 0, 1) != 0 and "static" in L.mf_last_error().decode()
     st.close()
     mf = _ctx()
-    L = mf.L
     L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
     assert L.mf_shard_configure(mf.h, 0, 2) == 0
     with pytest.raises(mfb.MFError, match="sharded"):
         mf.attachDetector(det)
     mf.close()
-    import torch
-    bst = torch.cuda.Stream()
-    bb = mfb.Backbone(256, seed=3, stream=bst.cuda_stream)
     mf = _ctx()
     mf.attachBackbone(bb, 5)
     with pytest.raises(mfb.MFError, match="backbone is attached"):
@@ -267,7 +274,6 @@ def test_refusals(nets):
     with pytest.raises(mfb.MFError, match="detector is attached"):
         mf.attachBackbone(bb, 5)
     assert L.mf_shard_configure(mf.h, 0, 2) != 0 and "detector" in L.mf_last_error().decode()
-    uid = (C.c_uint8 * 128)()
     assert L.mf_shard_comm_init(mf.h, uid, 0, 2) != 0 and "detector" in L.mf_last_error().decode()
     mf.attachDetector(None)
     mf.close()
