@@ -82,6 +82,23 @@ int mf_process_frame_device(mf_context* ctx, const void* d_rgb, const void* d_de
 int mf_set_input_event(mf_context* ctx, void* cuda_event);
 int mf_sync(mf_context* ctx);                       /* wait for everything enqueued so far */
 int mf_tick(mf_context* ctx);                       /* MaskFusion::getTick */
+/* Frame queue, the reference's queueLength (-frameQ, default 30 there; MaskFusion.cpp:37,200-209, MainController.cpp:223,242).  Every
+ * mf_process_frame[_device] call pushes its frame; while fewer than `length` frames are queued the call returns without processing
+ * anything (mf_tick, poses and the pose log do not change); otherwise it processes the oldest queued frame.  The frame processed by the
+ * n-th call of a run is the frame of call n - length + 1, at tick n - length + 1.  length 0 or 1: no queue (the default).
+ *   - With the frame travel rgb, depth, the caller's mask, the class list set by mf_set_frame_classes before the call, and the
+ *     timestamp.  Host inputs are free when the call returns; device inputs are copied at push time (mf_set_input_event applies).
+ *   - in_pose, weight_multiplier and bootstrap belong to the CALL and apply to the frame it processes, not to the frame it pushes (as
+ *     in the reference, whose processFrame takes them next to the FrameData it queues).
+ *   - An attached detector or backbone runs when the frame is pushed, on the tick the frame will be processed at, and writes its masks
+ *     into the queued frame: with a queue its work overlaps the processing of the frames ahead of it.
+ *   - Frames still queued at mf_destroy are dropped (the reference never processes the last length - 1 frames of a run).
+ *   - Allowed before the first processed frame, with nothing queued; the memory is (max(length, 1) + 1) * (8 * width * height + 1048)
+ *     bytes and is allocated here.  Refused: a negative length, and a sharded context (mf_shard_configure with world > 1 or
+ *     mf_shard_comm_init), which in turn refuse a context with a queue.  While frames are queued, mf_set_frame and the stage-wise
+ *     mf_model_* calls are refused. */
+int mf_set_frame_queue(mf_context* ctx, int length);
+int mf_frame_queue_size(mf_context* ctx);           /* frames queued and not yet processed: whether a call processed a frame */
 int64_t mf_kernel_launches(mf_context* ctx);        /* kernels launched since creation */
 
 /* ---- model list (MaskFusion::getModels) ---- */
@@ -125,9 +142,10 @@ int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k);
 /* Mask R-CNN detector on the frame path: MfSegmentation::performSegmentation calls MaskRCNN::executeSequential when the frame has no mask
  * (MfSegmentation.cpp:128-131), which fills FrameData::mask with the id image and FrameData::classIDs with [0] followed by the exported class
  * ids (MaskRCNN.cpp:98-151).  With a detector attached (handle of mf_detector_create), a frame runs it when the context is multi-model,
- * the caller passed NO mask, the frame runs segmentation (tick > 1 and not an in_pose frame) and mf_tick() % every_k == 0 before the call.
- * Detection (mould, backbone, RPN, heads at the context's W x H) and the hand-off into the frame's mask and class list are enqueued on the
- * detector's stream behind the frame's preprocessing; the context's stream waits for them only where segmentation first reads the mask,
+ * the caller passed NO mask, the frame runs segmentation (tick > 1 and not an in_pose frame) and mf_tick() % every_k == 0 before the call
+ * (with a frame queue: the tick the frame is processed at; whether the processing call passes an in_pose is not known yet, and such a
+ * frame's detection goes unused).  Detection (mould, backbone, RPN, heads at the context's W x H) and the hand-off into the frame's mask and
+ * class list are enqueued on the detector's stream behind the frame's upload; the context's stream waits for them only where segmentation first reads the mask,
  * so tracking and the ID projection overlap the detector.  Nothing in the frame waits for the host.
  *   - A frame skipped by every_k carries no masks (as with mask = NULL and no detector).  A frame given a mask uses it and the classes of
  *     mf_set_frame_classes; the detector does not run.
@@ -136,7 +154,7 @@ int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k);
  *   - Refused: a -static context, world > 1 (sharded runs use mf_shard_attach_detector), a backbone attached (and mf_attach_backbone while
  *     a detector is attached); mf_shard_configure and mf_shard_comm_init refuse a context with a detector attached here.
  *   - NULL detaches; detaching and mf_destroy first wait for the last hand-off.  The context never destroys the detector: detach (or destroy
- *     the context) before destroying it.  Detector launches are not counted in mf_kernel_launches. */
+ *     the context) before destroying it.  Detector launches (the frame's RGBA copy it reads included) are not counted in mf_kernel_launches. */
 struct mf_detector;
 int mf_attach_detector(mf_context* ctx, struct mf_detector* detector, int every_k);
 /* FrameData::mask (W x H) and classIDs (n_masks entries of class_ids_256) that segmentation read on the last frame; mask is all zero when

@@ -42,7 +42,7 @@ class Config(C.Structure):
 
 EXPORTS = [
     "mf_last_error", "mf_abi_version", "mf_config_defaults", "mf_create", "mf_destroy", "mf_process_frame",
-    "mf_process_frame_device", "mf_set_input_event", "mf_sync", "mf_tick", "mf_kernel_launches", "mf_model_count", "mf_model_id", "mf_get_pose",
+    "mf_process_frame_device", "mf_set_input_event", "mf_sync", "mf_tick", "mf_set_frame_queue", "mf_frame_queue_size", "mf_kernel_launches", "mf_model_count", "mf_model_id", "mf_get_pose",
     "mf_set_pose", "mf_model_surfel_count", "mf_model_set_conf_threshold", "mf_download_surfels", "mf_upload_surfels",
     "mf_pose_log_size", "mf_get_pose_log", "mf_set_frame", "mf_model_perform_tracking", "mf_model_predict_indices",
     "mf_model_fuse", "mf_model_clean", "mf_model_combined_predict", "mf_model_init_from_frame",
@@ -86,8 +86,9 @@ def load_library():
     L.mf_process_frame_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int]
     L.mf_set_input_event.argtypes = [C.c_void_p, C.c_void_p]
     L.mf_kernel_launches.restype = C.c_int64
-    for name in ("mf_sync", "mf_tick", "mf_kernel_launches", "mf_model_count"):
+    for name in ("mf_sync", "mf_tick", "mf_kernel_launches", "mf_model_count", "mf_frame_queue_size"):
         getattr(L, name).argtypes = [C.c_void_p]
+    L.mf_set_frame_queue.argtypes = [C.c_void_p, C.c_int]
     for name in ("mf_model_id", "mf_model_surfel_count", "mf_pose_log_size"):
         getattr(L, name).argtypes = [C.c_void_p, C.c_int]
     L.mf_get_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -447,6 +448,15 @@ class MaskFusion:
 
     def getTick(self) -> int:
         return self.L.mf_tick(self.h)
+
+    def setFrameQueue(self, n: int):
+        """the reference's queueLength (-frameQ, mf_set_frame_queue): each processFrame pushes its frame and processes the oldest one
+        once n frames are queued; 0 or 1 = no queue.  Before the first frame."""
+        self._ck(self.L.mf_set_frame_queue(self.h, int(n)))
+
+    def frameQueueSize(self) -> int:
+        """frames queued and not yet processed"""
+        return self._ck(self.L.mf_frame_queue_size(self.h))
 
     def kernelLaunches(self) -> int:
         return int(self.L.mf_kernel_launches(self.h))

@@ -39,6 +39,13 @@ static int mf_finalise(mf_context* ctx)
 #define MF_MODEL(ctx, i) if ((i) < 0 || (i) >= (int)(ctx)->mf->models.size()) { g_err = "model index out of range"; return -2; } Model* m = (ctx)->mf->models[i].get();
 
 #define MF_OWNED(m) if (!(m)->owned) { g_err = "model is owned by another rank (sharded mode): no device buffers here"; return -4; }
+// the stage-wise calls work on the frame processed last, which frames still in the queue would no longer follow
+#define MF_UNQUEUED(ctx, who)                                                                                                                  \
+    if ((ctx)->mf->queued) {                                                                                                                   \
+        g_err = std::string(who) + ": " + std::to_string((ctx)->mf->queued) + " frame(s) are queued (mf_set_frame_queue); the stage-wise calls " \
+                "run on a context with no frames queued";                                                                                      \
+        return -6;                                                                                                                             \
+    }
 
 static Mat4 fromColMajor(const float* p) { Mat4 r; for (int rr = 0; rr < 4; ++rr) for (int c = 0; c < 4; ++c) r.m[rr * 4 + c] = p[c * 4 + rr]; return r; }
 static void toColMajor(const Mat4& T, float* p) { for (int rr = 0; rr < 4; ++rr) for (int c = 0; c < 4; ++c) p[c * 4 + rr] = T.m[rr * 4 + c]; }
@@ -99,6 +106,8 @@ extern "C" int mf_process_frame_device(mf_context* ctx, const void* d_rgb, const
 extern "C" int mf_set_input_event(mf_context* ctx, void* ev) { if (!ctx || !ctx->mf) { g_err = "null context"; return -1; } ctx->mf->inputReady = (cudaEvent_t)ev; return 0; }
 extern "C" int mf_sync(mf_context* ctx) { MF_TRY MF_NEED(ctx) ctx->mf->sync(); return 0; MF_CATCH(-1) }
 extern "C" int mf_tick(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return ctx->mf->tick; }
+extern "C" int mf_set_frame_queue(mf_context* ctx, int length) { MF_TRY MF_NEED(ctx) ctx->mf->setFrameQueue(length); return 0; MF_CATCH(-1) }
+extern "C" int mf_frame_queue_size(mf_context* ctx) { if (!ctx || !ctx->mf) { g_err = "null context"; return -1; } return ctx->mf->queued; }
 extern "C" int64_t mf_kernel_launches(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return ctx->mf->launches; }
 
 extern "C" int mf_model_count(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return (int)ctx->mf->models.size(); }
@@ -178,7 +187,7 @@ extern "C" int mf_export_poses(mf_context* ctx, const char* export_dir)
 // ---- per-stage entry points ----
 extern "C" int mf_set_frame(mf_context* ctx, const uint8_t* rgb, const float* depth, const uint8_t* mask)
 {
-    MF_TRY MF_NEED(ctx)
+    MF_TRY MF_NEED(ctx) MF_UNQUEUED(ctx, "set_frame")
     MaskFusion* o = ctx->mf;
     if (!mask) o->mask.zero(o->stream);
     o->setFrame(rgb, depth, mask, false);
@@ -188,7 +197,7 @@ extern "C" int mf_set_frame(mf_context* ctx, const uint8_t* rgb, const float* de
 }
 extern "C" int mf_model_perform_tracking(mf_context* ctx, int i, float* transform16)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "perform_tracking")
     std::vector<Model*> ms{m};
     ctx->mf->trackModels(ms);
     ctx->mf->finalisePending();
@@ -198,31 +207,31 @@ extern "C" int mf_model_perform_tracking(mf_context* ctx, int i, float* transfor
 }
 extern "C" int mf_model_predict_indices(mf_context* ctx, int i, int time)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "predict_indices")
     m->predictIndices(time, ctx->mf->cfg.maxDepthProcessed, ctx->mf->cfg.timeDelta); return 0;
     MF_CATCH(-1)
 }
 extern "C" int mf_model_fuse(mf_context* ctx, int i, int time, float depth_cutoff, float weight_multiplier)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "fuse")
     m->fuse(time, depth_cutoff, weight_multiplier); return 0;
     MF_CATCH(-1)
 }
 extern "C" int mf_model_clean(mf_context* ctx, int i, int time)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "clean")
     m->clean(time, ctx->mf->cfg.timeDelta, ctx->mf->cfg.maxDepthProcessed); return 0;
     MF_CATCH(-1)
 }
 extern "C" int mf_model_combined_predict(mf_context* ctx, int i, int time, int max_time)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "combined_predict")
     m->combinedPredict(ctx->mf->cfg.maxDepthProcessed, time, max_time, ctx->mf->cfg.timeDelta); return 0;
     MF_CATCH(-1)
 }
 extern "C" int mf_model_init_from_frame(mf_context* ctx, int i, int time)
 {
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
+    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m) MF_UNQUEUED(ctx, "init_from_frame")
     m->initialise(time); return 0;
     MF_CATCH(-1)
 }
@@ -373,6 +382,8 @@ extern "C" int mf_download_frame_masks(mf_context* ctx, uint8_t* mask, int32_t* 
     MF_TRY MF_NEED(ctx)
     MaskFusion* o = ctx->mf;
     if (!o->cfg.enableMultipleModels) { g_err = "not a multi-model context"; return -5; }
+    // a queued frame popped by an in_pose call was detected at push time but does not segment, so nothing has waited for its hand-off yet
+    o->waitHandoff(o->stream);
     FrameHdr h;
     cudaCheck(cudaMemcpyAsync(&h, o->dHdr, sizeof h, cudaMemcpyDeviceToHost, o->stream), "D2H");
     d2h(o, mask, o->frameMask, o->P);
