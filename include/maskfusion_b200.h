@@ -252,7 +252,10 @@ int mf_backbone_load_weights(mf_backbone* h, const char* path);
 int mf_mrcnn_read_layer(const char* path, const char* layer, float* w_rows_K, float* bias_rows, int* dims);
 /* out[MxN] = relu?(A[MxK] * B[NxK]^T + bias[N] + residual[MxN]); bf16 device pointers, K % 64 == 0, N % 64 == 0 */
 int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, const void* dResidual, void* dOut, int M, int N, int K, int relu, void* stream);
-/* implicit-GEMM 3x3/s1/p1 convolution, NHWC bf16, weights [Cout][3][3][Cin]; the activation is read through a 3-D TMA map (no im2col) */
+/* implicit-GEMM 3x3/s1/p1 convolution, NHWC bf16, weights [Cout][3][3][Cin]; the activation is read through a 3-D TMA map (no im2col) in
+ * boxes of Wbox x Hbox = 128 pixels, Wbox = min(W, 128).  Admitted: Cin a positive multiple of 64, Cout a positive multiple of 64, H > 0, and
+ * either W in {8, 16, 32, 64} with H % (128 / W) == 0 or W a multiple of 128 (at most 131072); H * W and 9 * Cin within int.  Any other
+ * shape returns -2 without touching the device; the message of an H, W or Cin outside this is "conv3x3: unsupported geometry". */
 int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBias, const void* dResidual, void* dOut, int H, int W, int Cin, int Cout, int relu, void* stream);
 mf_backbone* mf_backbone_create(int input_size, unsigned seed, void* stream);
 void mf_backbone_destroy(mf_backbone* h);

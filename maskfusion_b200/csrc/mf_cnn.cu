@@ -24,6 +24,7 @@
 #include <vector>
 #include <string>
 #include <math.h>
+#include <limits.h>
 #include <stdlib.h>
 #include <string.h>
 #include <map>
@@ -269,26 +270,53 @@ __global__ void k_subsample2(const __nv_bfloat16* __restrict__ in, int Hin, int 
         *reinterpret_cast<uint4*>(out + p * C + c8 * 8) = *reinterpret_cast<const uint4*>(in + ((size_t)(2 * oy) * Win + 2 * ox) * C + c8 * 8);
     }
 }
-// letter-boxed network input: uint8 RGB HxW -> bf16 NHWC SxS (bilinear resize to fit, zero padding, mean pixel subtracted)
-__global__ void k_mold_input(const uchar4* __restrict__ rgb, int W, int H, int S, float scale, int offx, int offy, int newW, int newH,
-                             __nv_bfloat16* __restrict__ out)
+// R-MOLD (DESIGN §4) one axis: output sample o of the resized image reads input coordinate c = (o + 0.5) * zoom - 0.5, zoom = in / out,
+// between taps i0 = floor(c) and i0 + 1 with weights w0 = 1 - (c - i0) and w1 = 1 - w0 (scipy.ndimage.zoom's arithmetic).  The file is
+// built with FMA contraction on: the _rn intrinsics keep every step a separately rounded double operation.
+MF_D void mold_axis(int o, double zoom, int& i0, double& w0, double& w1)
 {
-    const size_t total = (size_t)S * S;
-    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const int x = (int)(t % S), y = (int)(t / S);
-        float r = 0, g = 0, b = 0;
-        const int lx = x - offx, ly = y - offy;
-        if (lx >= 0 && lx < newW && ly >= 0 && ly < newH) {
-            float sx = fminf(fmaxf((lx + 0.5f) / scale - 0.5f, 0.f), (float)(W - 1)), sy = fminf(fmaxf((ly + 0.5f) / scale - 0.5f, 0.f), (float)(H - 1));
-            int x0 = (int)sx, y0 = (int)sy, x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-            float fx = sx - x0, fy = sy - y0;
-            uchar4 a = rgb[y0 * W + x0], bb = rgb[y0 * W + x1], c = rgb[y1 * W + x0], d = rgb[y1 * W + x1];
-            r = (a.x * (1 - fx) + bb.x * fx) * (1 - fy) + (c.x * (1 - fx) + d.x * fx) * fy - 123.7f;      // MEAN_PIXEL (mrcnn config)
-            g = (a.y * (1 - fx) + bb.y * fx) * (1 - fy) + (c.y * (1 - fx) + d.y * fx) * fy - 116.8f;
-            b = (a.z * (1 - fx) + bb.z * fx) * (1 - fy) + (c.z * (1 - fx) + d.z * fx) * fy - 103.9f;
-        }
-        out[t * 3] = __float2bfloat16(r); out[t * 3 + 1] = __float2bfloat16(g); out[t * 3 + 2] = __float2bfloat16(b);
+    const double c = __dsub_rn(__dmul_rn(__dadd_rn((double)o, 0.5), zoom), 0.5);
+    const double f = floor(c);
+    i0 = (int)f;
+    w0 = __dsub_rn(1.0, __dsub_rn(c, f));
+    w1 = __dsub_rn(1.0, w0);
+}
+// one channel of one resized sample: sum over the taps (y0,x0) (y0,x1) (y1,x0) (y1,x1) of (value * wy) * wx in that order, then truncated
+// to uint8 (the resize's astype), then minus the mean pixel in float, rounded once to bf16
+MF_D __nv_bfloat16 mold_value(int a, int b, int c, int d, double wy0, double wy1, double wx0, double wx1, float mean)
+{
+    double v = __dmul_rn(__dmul_rn((double)a, wy0), wx0);
+    v = __dadd_rn(v, __dmul_rn(__dmul_rn((double)b, wy0), wx1));
+    v = __dadd_rn(v, __dmul_rn(__dmul_rn((double)c, wy1), wx0));
+    v = __dadd_rn(v, __dmul_rn(__dmul_rn((double)d, wy1), wx1));
+    return __float2bfloat16((float)(int)v - mean);
+}
+// letter-boxed network input (R-MOLD): uint8 RGBA W x H -> bf16 NHWC S x S.  The image is resampled to newW x newH at (offx, offy) with
+// taps outside the image reading 0; the padding is the uint8 value 0, so it becomes -MEAN_PIXEL.  One thread per output pixel, one grid row
+// (blockIdx.y) per output row: no 64-bit index division
+__global__ void k_mold_input(const uchar4* __restrict__ rgb, int W, int H, int S, double zoomx, double zoomy, int offx, int offy, int newW,
+                             int newH, __nv_bfloat16* __restrict__ out)
+{
+    const float mr = 123.7f, mg = 116.8f, mb = 103.9f;      // MEAN_PIXEL (mrcnn config)
+    const int y = blockIdx.y, x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= S) return;
+    const int lx = x - offx, ly = y - offy;
+    __nv_bfloat16* o = out + ((size_t)y * S + x) * 3;
+    if (lx < 0 || lx >= newW || ly < 0 || ly >= newH) {
+        o[0] = __float2bfloat16(-mr); o[1] = __float2bfloat16(-mg); o[2] = __float2bfloat16(-mb);
+        return;
     }
+    int x0, y0;
+    double wx0, wx1, wy0, wy1;
+    mold_axis(lx, zoomx, x0, wx0, wx1);
+    mold_axis(ly, zoomy, y0, wy0, wy1);
+    const uchar4 zero = make_uchar4(0, 0, 0, 0);
+    const bool inx0 = x0 >= 0 && x0 < W, inx1 = x0 + 1 >= 0 && x0 + 1 < W, iny0 = y0 >= 0 && y0 < H, iny1 = y0 + 1 >= 0 && y0 + 1 < H;
+    const uchar4 a = iny0 && inx0 ? rgb[(size_t)y0 * W + x0] : zero, b = iny0 && inx1 ? rgb[(size_t)y0 * W + x0 + 1] : zero;
+    const uchar4 c = iny1 && inx0 ? rgb[(size_t)(y0 + 1) * W + x0] : zero, d = iny1 && inx1 ? rgb[(size_t)(y0 + 1) * W + x0 + 1] : zero;
+    o[0] = mold_value(a.x, b.x, c.x, d.x, wy0, wy1, wx0, wx1, mr);
+    o[1] = mold_value(a.y, b.y, c.y, d.y, wy0, wy1, wx0, wx1, mg);
+    o[2] = mold_value(a.z, b.z, c.z, d.z, wy0, wy1, wx0, wx1, mb);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -392,19 +420,22 @@ static void launch_wgmma(dim3 grid, cudaStream_t s, const CUtensorMap& mA, const
 int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
                      const int* conv3x3 /* Wimg, Himg, Cin */, bool outF32)
 {
+    // every refusal comes before the first driver call
     if (outF32 && residual) { g_cnn_err = "gemm: the fp32 output takes no residual"; return -2; }
+    ConvGeom geo; memset(&geo, 0, sizeof geo);
+    if (conv3x3) {
+        const int Wimg = conv3x3[0], Himg = conv3x3[1], Cin = conv3x3[2];
+        if (!cnn_conv_implicit(3, 1, 1, Cin, Himg, Wimg) || K != 9 * Cin || M != Wimg * Himg) { g_cnn_err = "conv3x3: unsupported geometry"; return -2; }
+        geo.mode = 1; geo.Wimg = Wimg; geo.Himg = Himg; geo.Wbox = Wimg >= 128 ? 128 : Wimg; geo.Hbox = 128 / geo.Wbox; geo.cblocks = Cin / 64;
+    }
+    if (K <= 0 || N <= 0 || M <= 0 || K % 64 || N % 64) { g_cnn_err = "gemm: need M > 0, and K > 0 and N > 0 multiples of 64"; return -2; }
     if (!ensure_encode()) return -1;
-    if (K % 64 || N % 64 || M <= 0) { g_cnn_err = "gemm: need K % 64 == 0 and N % 64 == 0"; return -2; }
     const int mtiles = (M + GEMM_BM - 1) / GEMM_BM;
     // fill the machine: with few M tiles prefer the narrow N tile (twice the CTAs)
     const int BN = (N % 128 == 0 && mtiles * (N / 128) >= num_sms()) ? 128 : 64;
     CUtensorMap mA, mB;
-    ConvGeom geo; memset(&geo, 0, sizeof geo);
     if (conv3x3) {
-        const int Wimg = conv3x3[0], Himg = conv3x3[1], Cin = conv3x3[2];
-        geo.mode = 1; geo.Wimg = Wimg; geo.Himg = Himg; geo.Wbox = Wimg >= 128 ? 128 : Wimg; geo.Hbox = 128 / geo.Wbox; geo.cblocks = Cin / 64;
-        if (Wimg % geo.Wbox || Himg % geo.Hbox || Cin % 64 || K != 9 * Cin) { g_cnn_err = "conv3x3: unsupported geometry"; return -2; }
-        if (!cached_map_nhwc(&mA, A, Cin, Wimg, Himg, geo.Wbox, geo.Hbox)) return -3;
+        if (!cached_map_nhwc(&mA, A, conv3x3[2], geo.Wimg, geo.Himg, geo.Wbox, geo.Hbox)) return -3;
     } else if (!cached_map(&mA, A, (uint64_t)M, (uint64_t)K, GEMM_BM)) return -3;
     if (!cached_map(&mB, B, (uint64_t)N, (uint64_t)K, (uint32_t)BN)) return -3;
     dim3 grid(mtiles, N / BN);
@@ -434,12 +465,17 @@ struct Backbone {
     Backbone(int S, unsigned seed, cudaStream_t s);
 };
 
-// geometry guard of the implicit 3x3 path: the 128-pixel TMA box must tile the image exactly
+// geometry rule of the implicit 3x3 path, the only one (launch_gemm_bf16 refuses exactly what it refuses): the Wbox x Hbox TMA box of
+// 128 pixels (Wbox = min(W, 128), Hbox = 128 / Wbox) must tile the image exactly, since the producer expects a full 16 KiB A tile per
+// k-block and a smaller box would never complete the barrier.  Admitted: W a divisor of 128 of at least 8 with H % (128 / W) == 0, or
+// W a multiple of 128 (up to 128 Ki); Cin a positive multiple of 64; M = H * W within int
 bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win)
 {
+    if (k != 3 || stride != 1 || pad != 1 || Cin <= 0 || Cin % 64 || Cin > INT_MAX / 9 || Hin <= 0 || Win <= 0 || Win > 128 * 1024 ||
+        Hin > INT_MAX / Win)
+        return false;
     const int wbox = Win >= 128 ? 128 : Win;
-    return k == 3 && stride == 1 && pad == 1 && (Cin % 64) == 0 && Win <= 128 * 1024 && (128 % wbox) == 0 && (Win % wbox) == 0 &&
-           (Hin % (128 / wbox)) == 0 && wbox >= 8;
+    return wbox >= 8 && 128 % wbox == 0 && Win % wbox == 0 && Hin % (128 / wbox) == 0;
 }
 
 // runs convolution L (weights W [rows x K], bias B) on in[Hin x Win x cin] -> out[Hout x Wout x rows]; col: im2col scratch
@@ -522,12 +558,15 @@ extern "C" int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, 
     return rc;
 }
 
-// implicit-GEMM 3x3 / stride 1 / pad 1 convolution on an NHWC bf16 activation (weights [Cout][3][3][Cin] bf16)
+// implicit-GEMM 3x3 / stride 1 / pad 1 convolution on an NHWC bf16 activation (weights [Cout][3][3][Cin] bf16); the geometry is
+// cnn_conv_implicit's, anything else returns -2 before a driver call
 extern "C" int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBias, const void* dResidual, void* dOut, int H, int W, int Cin, int Cout,
                                int relu, void* stream)
 {
     int g3[3] = {W, H, Cin};
-    return launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, H * W, Cout, 9 * Cin, relu, (cudaStream_t)stream, g3);
+    // products in unsigned arithmetic: a refused geometry may overflow them, and the refusal does not read them
+    return launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, (int)((unsigned)H * (unsigned)W), Cout, (int)(9u * (unsigned)Cin), relu, (cudaStream_t)stream,
+                            g3);
 }
 
 // ResNet-101-FPN (mf_weights.cu has the layer table); throws CudaError
@@ -655,13 +694,17 @@ extern "C" int mf_backbone_download(mf_backbone* h, int level, void* host_bf16)
     if (!p) return cnn_fail("backbone: no handle or level outside 0..8");
     return cnn_download(h->stream, host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2) ? -2 : 0;
 }
-// letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs)
+// letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs; rule R-MOLD)
 extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H)
 {
     if (!h) return cnn_fail("backbone: null handle");
+    if (W <= 0 || H <= 0) return cnn_fail("mold: the image needs W > 0 and H > 0");
     Backbone* b = h; const int S = b->S;
     const MoldGeom g = cnn_mold_geometry(S, W, H);
+    const double zoomx = (double)W / (double)g.newW, zoomy = (double)H / (double)g.newH;     // in / out per axis (R-MOLD)
+    if (S > 65535) return cnn_fail("mold: the input size exceeds the grid's 65535 rows");
     prof_mark(h->stream, "k_mold_input");
-    k_mold_input<<<8 * num_sms(), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, g.scale, g.offx, g.offy, g.newW, g.newH, b->input);
+    k_mold_input<<<dim3((S + 255) / 256, S), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, zoomx, zoomy, g.offx, g.offy, g.newW, g.newH,
+                                                                   b->input);
     return cnn_check_launch("k_mold_input") ? -2 : 0;
 }

@@ -1,6 +1,6 @@
 """numpy restatement of the Mask R-CNN detection heads after their GEMMs (csrc/mf_heads.cu): the detection layer, the mask select, unmould
 and generate_id_image of matterport mrcnn (COCO InferenceConfig), with the written rules R-SOFTMAX, R-DETNMS, R-UNMOLD, R-RESIZE and R-SIGMOID
-of DESIGN.md section 4.
+of DESIGN.md section 4; and the network's input mould (csrc/mf_cnn.cu k_mold_input), rule R-MOLD.
 
 Float operations are float32 in the kernels' order (the CUDA file is compiled -fmad=false), float64 where R-UNMOLD and R-RESIZE say so, so the
 GPU results are compared bit for bit."""
@@ -175,6 +175,71 @@ def resize_mask(m: np.ndarray, h: int, w: int) -> np.ndarray:
     top = (1.0 - fxb) * at(iy, ix) + fxb * at(iy, ix + 1)
     bot = (1.0 - fxb) * at(iy + 1, ix) + fxb * at(iy + 1, ix + 1)
     return ((1.0 - fyb) * top + fyb * bot).astype(np.float32)
+
+
+MEAN_PIXEL = (123.7, 116.8, 103.9)
+
+
+def resize_channel(img: np.ndarray, h: int, w: int) -> np.ndarray:
+    """R-MOLD step 1: one channel resized to h x w as scipy.ndimage.zoom(order=1, mode='grid-constant', grid_mode=True) computes it, in its
+    own float64 arithmetic: per axis zoom = in / out, c = (o + 0.5) * zoom - 0.5, taps i0 = floor(c) and i0 + 1 (0 outside the image),
+    w0 = 1 - (c - i0), w1 = 1 - w0; the value is the sum of (tap * wy) * wx over (y0, x0), (y0, x1), (y1, x0), (y1, x1), left to right"""
+    H, W = img.shape
+
+    def axis(n, m):
+        c = (np.arange(n, dtype=np.float64) + 0.5) * (np.float64(m) / np.float64(n)) - 0.5
+        i0 = np.floor(c)
+        w0 = 1.0 - (c - i0)
+        return i0.astype(np.int64), w0, 1.0 - w0
+    iy, wy0, wy1 = axis(h, H)
+    ix, wx0, wx1 = axis(w, W)
+    mp = np.zeros((H + 2, W + 2), np.float64)
+    mp[1:-1, 1:-1] = img
+
+    def at(yy, xx):
+        return mp[np.clip(yy + 1, 0, H + 1)[:, None], np.clip(xx + 1, 0, W + 1)[None, :]]
+    Y0, Y1, X0, X1 = wy0[:, None], wy1[:, None], wx0[None, :], wx1[None, :]
+    v = at(iy, ix) * Y0 * X0
+    v = v + at(iy, ix + 1) * Y0 * X1
+    v = v + at(iy + 1, ix) * Y1 * X0
+    return v + at(iy + 1, ix + 1) * Y1 * X1
+
+
+def bf16_bits(x: np.ndarray) -> np.ndarray:
+    """float32 -> bfloat16 bit patterns, round to nearest even (finite values)"""
+    u = np.ascontiguousarray(x, np.float32).view(np.uint32).astype(np.uint64)
+    return ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+
+
+def mold_input(rgb: np.ndarray, S: int):
+    """R-MOLD: resize_image(mode='square') + mold_image on an H x W x >= 3 uint8 image -> (S x S x 3 bf16 bit patterns, the resized uint8
+    letter box).  Resized per channel (resize_channel), truncated to uint8, placed at (offx, offy) of an S x S x 3 zero image,
+    float32(u8) - MEAN_PIXEL in float64 rounded to float32, rounded once to bf16"""
+    H, W = rgb.shape[:2]
+    _, nw, nh, ox, oy = mold_geometry(S, W, H)
+    box = np.stack([resize_channel(rgb[..., c].astype(np.float64), nh, nw) for c in range(3)], -1).astype(np.uint8)
+    img = np.zeros((S, S, 3), np.uint8)
+    img[oy:oy + nh, ox:ox + nw] = box
+    return bf16_bits((img.astype(np.float32) - np.array(MEAN_PIXEL)).astype(np.float32)), box
+
+
+MOLD_KINDS = ("random", "flat", "smooth")
+
+
+def mold_test_image(kind: str, W: int, H: int, seed: int = 0) -> np.ndarray:
+    """H x W x 4 uint8 test images for the mould: random (0 and 255 in every channel, alpha random too), flat, or smooth with ramps"""
+    rng = np.random.default_rng(seed)
+    if kind == "random":
+        img = rng.integers(0, 256, (H, W, 4)).astype(np.uint8)
+        img[0, 0], img[-1, -1], img[H // 2, 0], img[0, W // 2] = 0, 255, 255, 0
+        return img
+    if kind == "flat":
+        img = np.empty((H, W, 4), np.uint8)
+        img[...] = (200, 1, 255, 7)
+        return img
+    yy, xx = np.mgrid[0:H, 0:W].astype(np.float64)
+    rgb = [127.5 + 127.5 * np.sin(xx / 37.0) * np.cos(yy / 23.0), 255.0 * xx / max(W - 1, 1), 255.0 * (1.0 - yy / max(H - 1, 1))]
+    return np.stack([np.floor(np.clip(c, 0, 255)) for c in rgb] + [np.full((H, W), 255.0)], -1).astype(np.uint8)
 
 
 def unmold_mask(m: np.ndarray, box, H: int, W: int) -> np.ndarray:

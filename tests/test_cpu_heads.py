@@ -1,6 +1,7 @@
 """The numpy restatement of the detection heads (tests/heads_ref.py) on its own: per-class NMS against torchvision, the mask resize against
-scipy.ndimage.zoom (the pin of R-RESIZE), unmould on boxes worked out by hand, and the restated export path against api.generate_id_image.
-The GPU kernels are compared with this restatement in tests/test_gpu_heads.py."""
+scipy.ndimage.zoom (the pin of R-RESIZE), unmould on boxes worked out by hand, the restated export path against api.generate_id_image, and
+the input mould's resample against scipy.ndimage.zoom (the pin of R-MOLD).  The GPU kernels are compared with this restatement in
+tests/test_gpu_heads.py and tests/test_gpu_cnn.py."""
 from __future__ import annotations
 
 import numpy as np
@@ -59,6 +60,43 @@ def test_resize_matches_scipy_zoom():
                 differ += int((ulps > 0).sum()); total += ulps.size
     print(f"R-RESIZE: {differ} of {total} float32 values differ from scipy.ndimage.zoom by 1 ulp, none by more; threshold decisions identical")
     assert (ref.resize_mask(masks[2], 28, 28) == masks[2]).all()      # the identity resize reproduces the grid, 0.5 included
+
+
+@pytest.mark.parametrize("W,H,S", [(640, 480, 256), (640, 480, 1024), (1280, 720, 1024), (320, 240, 1024), (480, 640, 1024), (641, 479, 1024),
+                                   (7, 5, 64), (100, 37, 64)])
+def test_mold_resize_matches_scipy_zoom(W, H, S):
+    """R-MOLD's resample, truncated to uint8, against scipy.ndimage.zoom (skimage >= 0.19's resize(order=1, mode='constant',
+    preserve_range=True)) of the same float64 image: zero differing bytes, at sizes whose scale is not an integer ratio too"""
+    import scipy.ndimage as ndi
+    _, nw, nh, ox, oy = ref.mold_geometry(S, W, H)
+    for kind in ref.MOLD_KINDS:
+        rgba = ref.mold_test_image(kind, W, H, seed=W + H)
+        bits, box = ref.mold_input(rgba, S)
+        want = ndi.zoom(rgba[..., :3].astype(np.float64), (nh / H, nw / W, 1), order=1, mode="grid-constant", cval=0.0, grid_mode=True)
+        assert want.shape == box.shape == (nh, nw, 3)
+        assert int((want.astype(np.uint8) != box).sum()) == 0, (kind, W, H, S)
+        # the letter box and only it holds the resized image; the padding is the uint8 value 0 minus the mean pixel
+        pad = ref.bf16_bits(-np.array(ref.MEAN_PIXEL, np.float32))
+        inside = np.zeros((S, S), bool)
+        inside[oy:oy + nh, ox:ox + nw] = True
+        assert (bits[~inside] == pad).all()
+        assert np.array_equal(bits[inside].reshape(nh, nw, 3), ref.bf16_bits((box.astype(np.float32) - np.array(ref.MEAN_PIXEL)).astype(np.float32)))
+
+
+def test_mold_rule_worked_by_hand():
+    """a flat 200 image at 640 x 480 -> S = 1024: letter box 1024 x 768 at y = 128, zoom 640 / 1024 = 0.625.  Resized sample 0 reads
+    c = 0.5 * 0.625 - 0.5 = -0.1875: taps -1 (outside, 0) and 0 with weights 0.1875 and 0.8125, so the first and last row and column
+    blend with 0 (200 * 0.8125 = 162.5 -> 162, a corner 200 * 0.8125^2 = 132.03 -> 132) and the rest is 200.  In bf16: 76.3 -> 76.5,
+    38.3 -> 38.25, 8.3 -> 8.3125, the padding -123.7 -> -123.5"""
+    rgba = np.full((480, 640, 4), 200, np.uint8)
+    bits, box = ref.mold_input(rgba, 1024)
+    r = box[..., 0]
+    assert r[0, 0] == r[0, -1] == r[-1, 0] == r[-1, -1] == 132
+    assert (r[0, 1:-1] == 162).all() and (r[-1, 1:-1] == 162).all() and (r[1:-1, 0] == 162).all() and (r[1:-1, -1] == 162).all()
+    assert (box[1:-1, 1:-1] == 200).all()
+    f = (bits[..., 0].astype(np.uint32) << 16).view(np.float32)
+    assert f[128 + 5, 5] == 76.5 and f[128, 5] == 38.25 and f[128, 0] == 8.3125
+    assert (f[:128] == -123.5).all() and (f[128 + 768:] == -123.5).all()
 
 
 def test_unmold_boxes_worked_by_hand():

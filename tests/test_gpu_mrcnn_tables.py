@@ -1,8 +1,9 @@
 """Pinned values of the seeded Mask R-CNN handles (mf_backbone, mf_rpn, mf_detector) and the NULL-skip read-backs the header promises.
 
 The digests were recorded on an H100 before the three handles' layer tables, seeded generators and weight stores were merged into one
-(mf_weights.cu): every seeded table and bias that *_get_weights returns, the backbone's and the detector's layer tables, and what
-Detector.execute returns on one synthetic frame.  The seeded tables do not depend on the input size, so S = 256 keeps the test small."""
+(mf_weights.cu): every seeded table and bias that *_get_weights returns and the backbone's and the detector's layer tables.  What
+Detector.execute returns on one synthetic frame was recorded on an H100 once the input mould followed R-MOLD (DESIGN section 4).  The seeded
+tables do not depend on the input size, so S = 256 keeps the test small."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,10 +28,11 @@ LAYERS = {
     "backbone": "7cd5f774dcceb542ec92ce0ae0fb8fa3ff6fca1a2ba28c400ce84a48eded8030",
     "detector": "7406a699e68f54219911d9d3b8c069e2cfaec52ab6e279382fe973c0caf23998",
 }
+# re-recorded on an H100 when the mould took rule R-MOLD (DESIGN section 4): the network input changed, the tables above did not
 EXECUTE = {
-    "detections": "300bc790cc118cefda99ce68ef6fbfe2985f97af66c3f190f200e863ac88e621",
-    "masks": "b3c06bd1d389a242f61599413c9c3ea71db37db83c64da76eb6bac8bbc301da2",
-    "id_image": "ee597c39a062b22ffd767d0ba532f2ed406361a78084f49887da33be9dff9d52",
+    "detections": "484b193209b48f7285aa028b98a25f931e8f955530f5d7d4b0743be53940a99f",
+    "masks": "b6b51d73fcd9636a25c3b89f8b493d7f02dfebc6433cb9ebee8aa170eb9ccf89",
+    "id_image": "cae983444315591034b79ab214e1f2d464bf62c9aeff3d033eae2917f0d7de2e",
 }
 
 
@@ -118,7 +120,7 @@ def test_layer_tables_are_pinned():
     assert layer_digests() == LAYERS
 
 
-def test_execute_is_pinned():
+def test_execute_on_the_r_mold_input_is_pinned():
     assert execute_digests() == EXECUTE
 
 
