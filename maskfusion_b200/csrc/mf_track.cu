@@ -416,34 +416,51 @@ struct TrackParams {
     int nJobs; unsigned short jobStart[TRACK_MAX_JOBS + 1];
 };
 
-// sum of 32 per-lane values over the warp with 31 (64-bit) shuffles instead of 5*32: each step exchanges HALF of the remaining
-// values with the xor partner.  Lane l ends with the total of value l.
-MF_D double shflXorD(double v, int m)
+// ---- per-warp normal equations on the fp64 tensor core ----
+// A pixel contributes the outer product of its row (the Jacobian entries, the residual, and for ICP / SO(3) a 1 that counts it: 8 floats,
+// zeros where unused) to an 8x8 sum.  One mma.m8n8k4.f64 (DMMA) adds 4 pixels: A = J^T (8 x 4), B = J (4 x 8), and lane l supplies the SAME
+// value to both, component l >> 2 of pixel l & 3.  The accumulator fragment -- entries (l >> 2, 2 (l & 3)) and (l >> 2, 2 (l & 3) + 1) in
+// lane l -- is the warp's sum over all its lanes: no per-thread accumulators across the pixel loop and no shuffle tree after it.  Every
+// product of two floats is exact in fp64, so the sums are fp64 sums of exact products as before, in another order (R-SUM, DESIGN.md 4).
+// A pixel's row goes straight to its lane's slot of a tile, so no row stays in registers while the other pixel in flight is worked on.
+// A warp's two tiles share their shared memory with the fragment that the CTA reduction reads (the two are never live together).
+union WarpScratch {
+    float rows[2][32][8];              // rows of the two pixels in flight (lane l's in [.][l], read transposed by the MMAs)
+    double frag[66];                   // the warp's 8x8 sum (row major) and its two integer counters
+};
+
+MF_D void putRow(float* slot, float4 lo, float4 hi)
 {
-    return __hiloint2double(__shfl_xor_sync(0xffffffffu, __double2hiint(v), m), __shfl_xor_sync(0xffffffffu, __double2loint(v), m));
+    reinterpret_cast<float4*>(slot)[0] = lo;
+    reinterpret_cast<float4*>(slot)[1] = hi;
 }
-// One halving step: H is a template parameter so that the value loop has a constant trip count when it is unrolled.  (With
-// h = 16 >> s of an enclosing unrolled loop, the inner loop is unrolled first, while its trip count is still unknown: it stayed a runtime
-// loop, v[] was indexed dynamically and lived in local memory -- about 70 local loads and stores per reduction on sm_90a.)
-template <int H>
-MF_D void warpHalvingStep(double* v, int lane)
+
+// Adds the tile's rows to the warp's fragment f.  A lane whose row was not written (has = false) adds a zero row.  All 32 lanes must call.
+MF_D void warpAccumulate(float (*tile)[8], bool has, double (&f)[2])
 {
-    const bool up = (lane & H) != 0;
-#pragma unroll
-    for (int k = 0; k < H; ++k) {
-        double keep = up ? v[k + H] : v[k];
-        double send = up ? v[k] : v[k + H];
-        v[k] = keep + shflXorD(send, H);
-    }
-}
-MF_D void warpReduceHalving32(double* v)
-{
+    if (!__any_sync(0xffffffffu, has)) return;             // 32 zero rows add +0.0 to sums that start at +0.0: skipping them is exact
     const int lane = threadIdx.x & 31;
-    warpHalvingStep<16>(v, lane);
-    warpHalvingStep<8>(v, lane);
-    warpHalvingStep<4>(v, lane);
-    warpHalvingStep<2>(v, lane);
-    warpHalvingStep<1>(v, lane);
+    if (!has) putRow(tile[lane], make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f));
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const double v = (double)tile[4 * i + (lane & 3)][lane >> 2];   // lanes read 32 different banks
+        asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(f[0]), "+d"(f[1]) : "d"(v), "d"(v));
+    }
+    __syncwarp();                                          // the tile is rewritten by the next call
+}
+
+// Position in the 8x8 sum of accumulator q for rows of R entries (R - 1 Jacobian entries and the residual): q walks the upper triangle
+// row by row without the residual's square (the layout solveAndUpdate and the SO(3) step read), then the residual's square, then the count.
+template <int R>
+MF_D int fragIndex(int q)
+{
+    constexpr int nJ = R * (R + 1) / 2 - 1;
+    if (q == nJ) return (R - 1) * 9;
+    if (q == nJ + 1) return R * 9;
+    int a = 0;
+    while (q >= R - a) { q -= R - a; ++a; }
+    return a * 9 + q;
 }
 
 // ---- flagged exchange of the partial rows (the LL scheme of collective libraries) ----
@@ -464,26 +481,28 @@ MF_D uint4 llLoad(const uint4* p)
     return r;
 }
 
-// CTA-wide fp64 sum of N (<= 29) accumulators -> one row of 32 flagged doubles in global memory (row = this CTA's partial); two integer
-// counters ride in columns 29 and 30 (exact in fp64).  Accumulating the exact products of floats in fp64 makes the totals agree with
-// a sequential fp64 sum to ~1e-15 relative whatever the order: rounded to float (the reference's result record) they are the
-// oracle's values bit for bit, which is what keeps tracked trajectories identical instead of merely close (DESIGN.md section 4).
-template <int N>
-MF_D void ctaReduceStore(const double* acc, double (*red)[ROWF], uint4* __restrict__ rowOut, unsigned flag, int extra0, int extra1)
+// CTA-wide fp64 sum of the warps' fragments -> one row of 32 flagged doubles in global memory (row = this CTA's partial): N (<= 29)
+// accumulators, and two integer counters in columns 29 and 30 (exact in fp64).  Accumulating the exact products of floats in fp64 makes
+// the totals agree with a sequential fp64 sum to ~1e-15 relative whatever the order: rounded to float (the reference's result record)
+// they are the oracle's values bit for bit, which is what keeps tracked trajectories identical instead of merely close (DESIGN.md section 4).
+// The warps' scratch is free again once every thread has passed the next barrier of sumRows.
+template <int R, int N>
+MF_D void ctaReduceStore(const double (&f)[2], WarpScratch* wsc, uint4* __restrict__ rowOut, unsigned flag, int extra0, int extra1)
 {
-    double v[32];
-#pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = k < N ? acc[k] : 0.0;
-    v[29] = (double)extra0; v[30] = (double)extra1;
-    warpReduceHalving32(v);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    red[warp][lane] = v[0];
+    const int c0 = __reduce_add_sync(0xffffffffu, extra0), c1 = __reduce_add_sync(0xffffffffu, extra1);
+    reinterpret_cast<double2*>(wsc[warp].frag)[lane] = make_double2(f[0], f[1]);
+    if (lane == 0) { wsc[warp].frag[64] = (double)c0; wsc[warp].frag[65] = (double)c1; }
     __syncthreads();
     if (threadIdx.x < ROWF) {
+        const int q = threadIdx.x;
+        const int e = q < N ? fragIndex<R>(q) : (q == 29 || q == 30) ? 64 + (q - 29) : -1;
         double s = 0;
+        if (e >= 0) {
 #pragma unroll
-        for (int w = 0; w < PT_WARPS; ++w) s += red[w][threadIdx.x];
-        llStore(rowOut + threadIdx.x, s, flag);
+            for (int w = 0; w < PT_WARPS; ++w) s += wsc[w].frag[e];
+        }
+        llStore(rowOut + q, s, flag);
     }
 }
 // every CTA: sum the R partial rows (fixed order, fp64) -> tot[0..32); columns 29/30 carry the integer counters.  Summation order:
@@ -524,16 +543,14 @@ MF_D void sumRows(const uint4* __restrict__ rows, unsigned R, unsigned flag, dou
 // One reduction of the schedule: CTA partial -> flagged exchange -> every CTA holds the same totals (replicated solver state, no
 // broadcast).  G CTAs of the model, the first Gact of them active.
 struct RedCtx { uint4* rows; unsigned G, Gact, gen, llBase, bx; };
-template <int N>
-MF_D void reduceStep(const double* acc, int e0, int e1, bool active, RedCtx& rc, double (*red)[ROWF], double (*ws)[ROWF], double* tot)
+template <int R, int N>
+MF_D void reduceStep(const double (&f)[2], int e0, int e1, bool active, RedCtx& rc, WarpScratch* wsc, double (*ws)[ROWF], double* tot)
 {
     // 16 bytes per value: the two ping-pong buffers are G * ROWF values each
     uint4* rows = rc.rows + (size_t)(rc.gen & 1) * rc.G * ROWF;
     ++rc.gen;
     const unsigned flag = rc.llBase + rc.gen;
-    // (an out-of-line routine shared by the three reductions shrank the loop but cost more than it saved: the 32 values travel
-    // through local memory)
-    if (active) ctaReduceStore<N>(acc, red, rows + (size_t)rc.bx * ROWF, flag, e0, e1);
+    if (active) ctaReduceStore<R, N>(f, wsc, rows + (size_t)rc.bx * ROWF, flag, e0, e1);
     sumRows(rows, rc.Gact, flag, ws, tot);
 }
 
@@ -722,7 +739,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
     __shared__ TrackJob J;
     __shared__ TrackState S;
     __shared__ SolveScratch sc;
-    __shared__ double red[PT_WARPS][ROWF];
+    __shared__ __align__(16) WarpScratch wsc[PT_WARPS];
     __shared__ double ws[PT_WARPS][ROWF];
     __shared__ double tot[64];
     __shared__ double totR[ROWF];
@@ -809,16 +826,16 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
             }
             __syncthreads();
             TT(11);
-            double acc[11];
-#pragma unroll
-            for (int k = 0; k < 11; ++k) acc[k] = 0;
+            double f[2] = {0.0, 0.0};
             if (active) {
-                for (int k = tid; k < N; k += nthr) {
+                // warp-uniform trip count (the MMAs need all 32 lanes): a lane past the last pixel adds a zero row
+                for (int k0 = tid - (threadIdx.x & 31); k0 < N; k0 += nthr) {
+                    const int k = k0 + (threadIdx.x & 31);
                     int y = k / W, x = k - y * W;
                     float3 ur = make_float3((float)x, (float)y, 1.0f);
                     float3 wr = m3v(so3B, ur);
                     int wx = __float2int_rn(wr.x / wr.z), wy = __float2int_rn(wr.y / wr.z);
-                    bool found = (wx >= 1 && wx < W - 1 && wy >= 1 && wy < H - 1 && x >= 1 && x < W - 1 && y >= 1 && y < H - 1);
+                    bool found = (k < N && wx >= 1 && wx < W - 1 && wy >= 1 && wy < H - 1 && x >= 1 && x < W - 1 && y >= 1 && y < H - 1);
                     if (found) {
                         float gnx, gny, glx, gly;
                         gradU8(nextImage, W, wx, wy, gnx, gny);
@@ -831,24 +848,17 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                         float3 l = make_float3(((p.z * (d * gy + a * gx)) - (gy * g * fy) - (gx * g * fxx)) / z2,
                                                ((p.z * (e * gy + b * gx)) - (gy * h * fy) - (gx * h * fxx)) / z2,
                                                ((p.z * (f * gy + cc * gx)) - (gy * i * fy) - (gx * i * fxx)) / z2);
-                        float row[4];
-                        row[0] = l.y * p.z - l.z * p.y;
-                        row[1] = l.z * p.x - l.x * p.z;
-                        row[2] = l.x * p.y - l.y * p.x;
-                        row[3] = -((float)nextImage[wy * W + wx] - (float)lastImage[k]);
-                        int q = 0;
-#pragma unroll
-                        for (int ii = 0; ii < 3; ++ii)
-#pragma unroll
-                            for (int jj = ii; jj < 4; ++jj) { acc[q] = fma((double)row[ii], (double)row[jj], acc[q]); ++q; }
-                        acc[9] = fma((double)row[3], (double)row[3], acc[9]);
-                        acc[10] += 1.0;
+                        // column 4 counts the pixel
+                        putRow(wsc[threadIdx.x >> 5].rows[0][threadIdx.x & 31],
+                               make_float4(l.y * p.z - l.z * p.y, l.z * p.x - l.x * p.z, l.x * p.y - l.y * p.x, -((float)nextImage[wy * W + wx] - (float)lastImage[k])),
+                               make_float4(1.f, 0.f, 0.f, 0.f));
                     }
+                    warpAccumulate(wsc[threadIdx.x >> 5].rows[0], found, f);
                 }
             }
             TT(12);
             rc.Gact = Gact;
-            reduceStep<11>(acc, 0, 0, active, rc, red, ws, tot);
+            reduceStep<4, 11>(f, 0, 0, active, rc, wsc, ws, tot);
             TT(15);
             if (threadIdx.x < 32) {
                 // host logic of RGBDOdometry.cpp:301-324 on warp 0: lane 0 takes the decisions, the 3x3 solve is warp-cooperative
@@ -917,7 +927,11 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
             if (kt < N) kTail = kt;
         }
         const int rounds = active ? fullRounds + (kTail >= 0 ? 1 : 0) : 0;
+        // rounds of the warp (the MMAs need all 32 lanes): a lane without a pixel in the last one adds zero rows
+        const bool tailW = __any_sync(0xffffffffu, kTail >= 0);
+        const int roundsW = active ? fullRounds + (tailW ? 1 : 0) : 0;
         auto kOf = [&](int r) { return r < fullRounds ? tid + r * nthr : kTail; };
+        float (*const tiles)[32][8] = wsc[threadIdx.x >> 5].rows;
         const Cam cam = camLevel(tp.cam, level);
         const float4* __restrict__ vmapC = J.vmapC[level];
         const float4* __restrict__ nmapC = J.nmapC[level];
@@ -975,6 +989,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
             if (tp.rgb) { p.valid = rgbValid[k]; p.d1 = nextDepth[k]; p.ni = nextImage[k]; }
             if (tp.icp) { p.vc = vmapC[k]; p.nc = nmapC[k]; }
         };
+        auto noPixel0 = [&](PixA& p) { p.valid = 0; p.d1 = 0.f; p.ni = 0; p.x = 0; p.y = 0; p.vc = make_float4(0, 0, 0, 0); p.nc = p.vc; };
         // (Tried: source pixels whose model-side depth is exactly 0 -- 95 % of an object model's image -- all warp to ONE target pixel, so
         // whether they can correspond is decidable once per iteration and they could skip the photometric projection.  Exact, but the two
         // dependent loads of that decision sat on the critical path of every iteration and made the
@@ -1008,6 +1023,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                 p.vg = vg; p.vcp = vcp;
             }
         };
+        auto noPixel1 = [&](PixA& p) { p.rOK = false; p.iOK = false; p.jr = 0; p.ji = 0; p.u0 = 0; p.v0 = 0; p.td1 = 0.f; p.vg = make_float3(0, 0, 0); p.vcp = p.vg; };
         auto stage2 = [&](PixA& p) {
             p.d0 = 0.f; p.li = 0; p.vp4 = make_float4(0, 0, 0, 0); p.np4 = p.vp4;
             if (p.rOK) { p.d0 = lastDepth[p.jr]; p.li = lastImage[p.jr]; }
@@ -1017,14 +1033,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
         for (int it = 0; it < tp.iterations[level]; ++it) {
             // ---- phase A: photometric correspondences + statistics, ICP normal equations ----
             TT(100 + level);
-            double acc[NACC_ICP];
-#pragma unroll
-            for (int k = 0; k < NACC_ICP; ++k) acc[k] = 0.0;
+            double f[2] = {0.0, 0.0};
             int cnt = 0, sig = 0;
             if (active) {
                 const float3 tprev = make_float3(st->tprev[0], st->tprev[1], st->tprev[2]);
-                // arithmetic of one pixel (same order of accumulation as a one-pixel-at-a-time loop: a before b, rounds ascending)
-                auto stage3 = [&](const PixA& p, int k, int slot) {
+                // arithmetic of one pixel: photometric correspondence and statistics; returns whether it is an ICP correspondence, whose
+                // row (and a 1 that counts it) goes to `row`
+                auto stage3 = [&](const PixA& p, int slot, float* row) -> bool {
                     if (tp.rgb) {
                         int2 c = make_int2(-1, 0);                     // .x = u0 | v0 << 16 (or -1: no correspondence), .y = bits of diff
                         if (p.rOK && p.d0 > 0 && fabsf(p.td1 - p.d0) <= tp.maxDepthDelta && p.li != 0) {
@@ -1048,25 +1063,17 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                             float3 s_cp = p.vcp;
                             float3 d_cp = m3v(st->RprevInv, sub3(vp, tprev));
                             float3 n_cp = m3v(st->RprevInv, np_);
-                            float row[7];
-                            row[0] = n_cp.x; row[1] = n_cp.y; row[2] = n_cp.z;
-                            row[3] = s_cp.y * n_cp.z - s_cp.z * n_cp.y;
-                            row[4] = s_cp.z * n_cp.x - s_cp.x * n_cp.z;
-                            row[5] = s_cp.x * n_cp.y - s_cp.y * n_cp.x;
-                            row[6] = (n_cp.x * (s_cp.x - d_cp.x) + n_cp.y * (s_cp.y - d_cp.y)) + n_cp.z * (s_cp.z - d_cp.z);
-                            int q = 0;
-#pragma unroll
-                            for (int a = 0; a < 6; ++a)
-#pragma unroll
-                                for (int b = a; b < 7; ++b) { acc[q] = fma((double)row[a], (double)row[b], acc[q]); ++q; }
-                            acc[27] = fma((double)row[6], (double)row[6], acc[27]);
-                            acc[28] += 1.0;
+                            putRow(row, make_float4(n_cp.x, n_cp.y, n_cp.z, s_cp.y * n_cp.z - s_cp.z * n_cp.y),
+                                   make_float4(s_cp.z * n_cp.x - s_cp.x * n_cp.z, s_cp.x * n_cp.y - s_cp.y * n_cp.x,
+                                               (n_cp.x * (s_cp.x - d_cp.x) + n_cp.y * (s_cp.y - d_cp.y)) + n_cp.z * (s_cp.z - d_cp.z), 1.f));
+                            return true;
                         }
                     }
+                    return false;
                 };
-                for (int r = 0; r < rounds; r += 2) {
-                    const bool two = r + 1 < rounds;
-                    const int k0 = kOf(r), k1 = two ? kOf(r + 1) : k0;
+                for (int r = 0; r < roundsW; r += 2) {
+                    const bool hasA = r < rounds, hasB = r + 1 < rounds;
+                    const int k0 = hasA ? kOf(r) : 0, k1 = hasB ? kOf(r + 1) : k0;
                     // next pair's streaming inputs -> L1 while this pair's dependent gathers are in flight (rounds not held in shared memory)
                     for (int q = 2; q < 4; ++q)
                         if (r + q < rounds && r + q >= cRounds) {
@@ -1075,20 +1082,22 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                             if (tp.rgb) { prefetchL1(nextDepth + kn); }
                         }
                     PixA a, b;
-                    stage0(a, k0, r);
-                    if (two) stage0(b, k1, r + 1); else { b.valid = 0; b.d1 = 0.f; b.ni = 0; b.x = 0; b.y = 0; b.vc = make_float4(0, 0, 0, 0); b.nc = b.vc; }
-                    stage1(a, k0, tprev);
-                    if (two) stage1(b, k1, tprev); else { b.rOK = false; b.iOK = false; b.jr = 0; b.ji = 0; b.u0 = 0; b.v0 = 0; b.td1 = 0.f; b.vg = make_float3(0, 0, 0); b.vcp = b.vg; }
+                    if (hasA) stage0(a, k0, r); else noPixel0(a);
+                    if (hasB) stage0(b, k1, r + 1); else noPixel0(b);
+                    if (hasA) stage1(a, k0, tprev); else noPixel1(a);
+                    if (hasB) stage1(b, k1, tprev); else noPixel1(b);
                     stage2(a); stage2(b);
-                    stage3(a, k0, r * PT_THREADS + threadIdx.x);
-                    if (two) stage3(b, k1, (r + 1) * PT_THREADS + threadIdx.x);
+                    const bool fA = hasA && stage3(a, r * PT_THREADS + threadIdx.x, tiles[0][threadIdx.x & 31]);
+                    const bool fB = hasB && stage3(b, (r + 1) * PT_THREADS + threadIdx.x, tiles[1][threadIdx.x & 31]);
+                    warpAccumulate(tiles[0], fA, f);
+                    warpAccumulate(tiles[1], fB, f);
                 }
             }
             TT(2);
             rc.Gact = Gact;
             // phase B's first streaming inputs (pose independent) -> L1 while this CTA waits at the reduction
             if (tp.rgb && rounds > cRounds) { prefetchL1(grad + kOf(cRounds)); }
-            reduceStep<NACC_ICP>(acc, cnt, sig, active, rc, red, ws, tot);
+            reduceStep<7, NACC_ICP>(f, cnt, sig, active, rc, wsc, ws, tot);
             TT(5);
             if (tp.rgb) {
                 if (threadIdx.x == 0) {
@@ -1108,39 +1117,27 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                 __syncthreads();
                 if (flag) break;                                        // uniform over the whole grid: every CTA holds the same state
                 // ---- phase B: photometric normal equations with the weights of this iteration ----
-                double accR[NACC_RGB];
-#pragma unroll
-                for (int k = 0; k < NACC_RGB; ++k) accR[k] = 0.0;
+                double fR[2] = {0.0, 0.0};
                 if (active) {
                     const float sigmaSh = st->sigmaVal;
-                    auto rgbRow = [&](int2 c, short2 g, float4 cp) {
+                    auto rgbRow = [&](int2 c, short2 g, float4 cp, float* row) {
                         const float diff = __int_as_float(c.y);
                         float w = sigmaSh + fabsf(diff);
                         w = w > 1.19209290E-07F ? 1.0f / w : 1.0f;
                         if (sigmaSh == -1) w = 1;
-                        float row[7];
-                        row[6] = -w * diff;
                         const float invz = cp.w;                           // (float)(1.0 / (double)cp.z), precomputed by k_project_points3
                         float dIdx_v = w * tp.sobelScale * (float)g.x;      // grad[one]: `one` is this pixel (reduce.cu:934)
                         float dIdy_v = w * tp.sobelScale * (float)g.y;
                         float v0 = dIdx_v * cam.fx * invz;
                         float v1 = dIdy_v * cam.fy * invz;
                         float v2 = -(v0 * cp.x + v1 * cp.y) * invz;
-                        row[0] = v0; row[1] = v1; row[2] = v2;
-                        row[3] = -cp.z * v1 + cp.y * v2;
-                        row[4] = cp.z * v0 - cp.x * v2;
-                        row[5] = -cp.y * v0 + cp.x * v1;
-                        int q = 0;
-#pragma unroll
-                        for (int a = 0; a < 6; ++a)
-#pragma unroll
-                            for (int b = a; b < 7; ++b) { accR[q] = fma((double)row[a], (double)row[b], accR[q]); ++q; }
+                        putRow(row, make_float4(v0, v1, v2, -cp.z * v1 + cp.y * v2), make_float4(cp.z * v0 - cp.x * v2, -cp.y * v0 + cp.x * v1, -w * diff, 0.f));
                     };
-                    for (int r = 0; r < rounds; r += 2) {
-                        const bool two = r + 1 < rounds;
-                        const int k0 = kOf(r), k1 = two ? kOf(r + 1) : k0;
-                        const int2 c0 = corr[r * PT_THREADS + threadIdx.x];
-                        const int2 c1 = two ? corr[(r + 1) * PT_THREADS + threadIdx.x] : make_int2(-1, 0);
+                    for (int r = 0; r < roundsW; r += 2) {
+                        const bool hasA = r < rounds, hasB = r + 1 < rounds;
+                        const int k0 = hasA ? kOf(r) : 0, k1 = hasB ? kOf(r + 1) : k0;
+                        const int2 c0 = hasA ? corr[r * PT_THREADS + threadIdx.x] : make_int2(-1, 0);
+                        const int2 c1 = hasB ? corr[(r + 1) * PT_THREADS + threadIdx.x] : make_int2(-1, 0);
                         short2 g0 = make_short2(0, 0), g1 = g0;
                         float4 p0 = make_float4(0, 0, 1, 0), p1 = p0;
                         auto gradOf = [&](int k, int rr) -> short2 {
@@ -1149,8 +1146,10 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                         };
                         if (c0.x != -1) { g0 = gradOf(k0, r); p0 = cloud[(c0.x >> 16) * W + (c0.x & 0xffff)]; }
                         if (c1.x != -1) { g1 = gradOf(k1, r + 1); p1 = cloud[(c1.x >> 16) * W + (c1.x & 0xffff)]; }
-                        if (c0.x != -1) rgbRow(c0, g0, p0);
-                        if (c1.x != -1) rgbRow(c1, g1, p1);
+                        if (c0.x != -1) rgbRow(c0, g0, p0, tiles[0][threadIdx.x & 31]);
+                        if (c1.x != -1) rgbRow(c1, g1, p1, tiles[1][threadIdx.x & 31]);
+                        warpAccumulate(tiles[0], c0.x != -1, fR);
+                        warpAccumulate(tiles[1], c1.x != -1, fR);
                     }
                 }
                 TT(6);
@@ -1162,7 +1161,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) k_track_persistent(const TrackJ
                         prefetchL1(nextDepth + kn);
                     }
                 // ICP totals stay in tot[0..28]; the photometric ones go behind them
-                reduceStep<NACC_RGB>(accR, 0, 0, active, rc, red, ws, totR);
+                reduceStep<7, NACC_RGB>(fR, 0, 0, active, rc, wsc, ws, totR);
                 TT(9);
                 if (threadIdx.x < NACC_RGB) tot[NACC_ICP + threadIdx.x] = totR[threadIdx.x];
                 __syncthreads();
