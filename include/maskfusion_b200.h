@@ -6,7 +6,8 @@
  * the flat, toolchain-neutral boundary a maintainer binds instead; each entry point
  * names the reference method it replaces.  Plain pointers and sizes only: no torch,
  * Eigen, OpenCV or GL types.  All functions return 0 on success, non-zero on error
- * (text via mf_last_error()); nothing calls exit() (the reference does on CUDA
+ * (text via mf_last_error(), which keeps one message per calling thread); no C++
+ * exception leaves a function, and nothing calls exit() (the reference does on CUDA
  * errors, Core/Cuda/convenience.cuh:76-83).
  *
  * Conventions
@@ -236,11 +237,11 @@ int mf_icp_step(mf_context* ctx, int i, int level, const float Rcurr9[9], const 
 /* ---- Mask R-CNN backbone: ResNet-101 + FPN as wgmma GEMMs (replaces the dense part of the Keras/TF sidecar,
  *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded unless loaded with mf_*_load_weights) ---- */
 typedef struct mf_backbone mf_backbone;
-const char* mf_cnn_last_error(void);
+const char* mf_cnn_last_error(void);      /* the same text as mf_last_error(), under the name kept for existing bindings */
 /* Pretrained weights (the reference's model.load_weights(COCO_MODEL_PATH, by_name=True)): a safetensors file of matterport's Keras
  * arrays named "<layer>/<param>", F32, Keras layouts (scripts/convert_mrcnn_h5.py writes it from mask_rcnn_coco.h5; DESIGN §3c has the
  * name table).  BatchNorm is folded on the host (R-FOLD).  Each loader reads its own handle's tensors and ignores the others; all or
- * nothing: everything is read, checked and folded before the handle changes, and on an error (mf_cnn_last_error() names the file and the
+ * nothing: everything is read, checked and folded before the handle changes, and on an error (mf_last_error() names the file and the
  * tensor) its weights stay as they were.  The copy is ordered on the handle's stream after the work queued there, and complete on
  * return: safe between frames with the detector attached; mf_*_get_weights read the new tables afterwards.  mf_rpn_load_weights and
  * mf_detector_load_weights are declared with their handles below. */
@@ -273,7 +274,7 @@ int mf_backbone_num_gemms(mf_backbone* h);
 
 /* ---- Mask R-CNN region proposals on the backbone's P2..P6 (matterport mrcnn rpn_graph + ProposalLayer + PyramidROIAlign, COCO
  *      InferenceConfig; weights synthetic/seeded unless loaded, owned by the handle, not by the backbone's layer table).  The handle reads the
- *      backbone's outputs and enqueues on the backbone's stream; destroy it before the backbone.  Errors: mf_cnn_last_error().
+ *      backbone's outputs and enqueues on the backbone's stream; destroy it before the backbone.  Errors: mf_last_error().
  *      Anchors: 3 per feature pixel (ratios 0.5, 1, 2), order (level P2..P6, y, x, ratio), normalised y1 x1 y2 x2; A anchors in all.
  *      Boxes are normalised y1 x1 y2 x2 float; pooled features are [n][pool][pool][256] bf16. ---- */
 typedef struct mf_rpn mf_rpn;
@@ -302,7 +303,7 @@ int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16_1000x7x7x256);
 /* ---- Mask R-CNN detection heads on an mf_rpn's proposals (matterport mrcnn fpn_classifier_graph + DetectionLayer + build_fpn_mask_graph +
  *      unmold_detections + generate_id_image, COCO InferenceConfig: 81 classes; weights synthetic/seeded unless loaded, owned by the handle).  The handle
  *      reads the RPN's proposals and pooled features and the backbone's P2..P5, and enqueues on the backbone's stream; destroy it before the
- *      RPN.  Errors: mf_cnn_last_error().  Shapes are the upstream ones: 1000 ROIs, 100 detection rows.  Detections are [100][6] float
+ *      RPN.  Errors: mf_last_error().  Shapes are the upstream ones: 1000 ROIs, 100 detection rows.  Detections are [100][6] float
  *      y1 x1 y2 x2 (normalised to the S x S network input, clipped to the letter-box window of the image) class score, zero rows after the
  *      count; masks are [100][28][28] float (sigmoid of the detection's own class).  The image size (W x H, the letter-box window) is the one
  *      given to the last mf_detector_forward / detect / paste; S x S after create. ---- */

@@ -10,6 +10,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
+
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -40,33 +42,49 @@ class Config(C.Structure):
     ]
 
 
-EXPORTS = [
-    "mf_last_error", "mf_abi_version", "mf_config_defaults", "mf_create", "mf_destroy", "mf_process_frame",
-    "mf_process_frame_device", "mf_set_input_event", "mf_sync", "mf_tick", "mf_set_frame_queue", "mf_frame_queue_size", "mf_kernel_launches", "mf_model_count", "mf_model_id", "mf_get_pose",
-    "mf_set_pose", "mf_model_surfel_count", "mf_model_set_conf_threshold", "mf_download_surfels", "mf_upload_surfels",
-    "mf_pose_log_size", "mf_get_pose_log", "mf_set_frame", "mf_model_perform_tracking", "mf_model_predict_indices",
-    "mf_model_fuse", "mf_model_clean", "mf_model_combined_predict", "mf_model_init_from_frame",
-    "mf_download_filtered_depth", "mf_download_frame_maps", "mf_download_model_maps", "mf_download_index_map",
-    "mf_download_prediction", "mf_download_fill_in", "mf_download_association", "mf_download_track_stats",
-    "mf_download_edge_map", "mf_morph_close", "mf_debug_track_timing", "mf_attach_backbone", "mf_backbone_stream", "mf_icp_step", "mf_debug_set_poses", "mf_set_profiling", "mf_get_stage_times", "mf_set_frame_classes", "mf_download_segmentation", "mf_model_class_id", "mf_klg_open", "mf_klg_num_frames", "mf_klg_has_more", "mf_klg_get_next",
-    "mf_klg_close", "mf_klg_write", "mf_dir_open", "mf_dir_num_frames", "mf_dir_has_more", "mf_dir_has_masks", "mf_dir_set_max_masks", "mf_dir_size",
-    "mf_dir_get_next", "mf_dir_close", "mf_decode_jpeg", "mf_decode_exr_depth", "mf_export_poses", "mf_generate_id_image", "mf_pre_segmentation", "mf_write_ply", "mf_cnn_last_error", "mf_gemm_bf16", "mf_conv3x3_bf16", "mf_backbone_create", "mf_backbone_destroy", "mf_backbone_num_layers",
-    "mf_backbone_layer", "mf_backbone_get_weights", "mf_backbone_mold", "mf_backbone_input_buffer", "mf_backbone_forward", "mf_backbone_output",
-    "mf_backbone_flops", "mf_backbone_num_gemms", "mf_backbone_download",
-    "mf_rpn_create", "mf_rpn_destroy", "mf_rpn_forward", "mf_rpn_run", "mf_rpn_num_anchors", "mf_rpn_propose", "mf_roi_align_bf16",
-    "mf_rpn_get_weights", "mf_rpn_get_anchors", "mf_rpn_get_head_outputs", "mf_rpn_download_conv", "mf_rpn_get_proposals", "mf_rpn_get_pooled",
-    "mf_detector_create", "mf_detector_destroy", "mf_detector_run", "mf_detector_forward", "mf_detector_detect", "mf_detector_set_export",
-    "mf_detector_refine", "mf_detector_paste", "mf_detector_num_layers", "mf_detector_layer", "mf_detector_get_weights", "mf_detector_get_fc",
-    "mf_detector_get_head_outputs", "mf_detector_get_mask_layer", "mf_detector_get_detections", "mf_detector_get_masks", "mf_detector_get_id_image",
-    "mf_detector_image_size", "mf_attach_detector", "mf_download_frame_masks",
-    "mf_backbone_load_weights", "mf_rpn_load_weights", "mf_detector_load_weights", "mf_mrcnn_read_layer",
-    "mf_shard_configure", "mf_shard_unique_id", "mf_shard_comm_init", "mf_shard_process_frame", "mf_shard_stats", "mf_shard_frame_begin", "mf_shard_get_poses", "mf_shard_set_poses", "mf_shard_project",
-    "mf_shard_projection_keys", "mf_shard_frame_end", "mf_shard_attach_detector", "mf_shard_frame_masks", "mf_model_owner", "mf_shard_pick_owner", "mf_track_shares",
-]
+HEADER = os.path.join(HERE, "..", "include", "maskfusion_b200.h")
+# ctypes type of each scalar the header uses; every pointer is c_void_p (c_char_p for strings), so no handle is truncated to int
+_SCALARS = {"int": C.c_int, "unsigned": C.c_uint, "int64_t": C.c_int64, "float": C.c_float, "double": C.c_double}
+
+
+def _spaced(t: str) -> str:
+    return " ".join(t.replace("*", " * ").split()).replace(" *", "*")          # "const char *" -> "const char*"
+
+
+def _prototypes():
+    """[(name, return type, [parameter types])] of every mf_* function the header declares, types as written there ("const char*")"""
+    src = open(HEADER).read()
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", src, flags=re.S)         # comments
+    src = re.sub(r"^\s*#[^\n]*", " ", src, flags=re.M)                 # preprocessor lines
+    out = []
+    for ret, name, params in re.findall(r"([^;{}()]*?)\b(mf_\w+)\s*\(([^()]*)\)\s*;", src):
+        types = []
+        for p in params.split(","):
+            p, array = re.subn(r"\[[^\]]*\]\s*$", "", p.strip())         # float pose16[16] is a float*
+            p = re.sub(r"(?<=[\s*])\w+$", "", p.strip())                 # the parameter's name
+            types.append(_spaced(p) + "*" * array)
+        out.append((name, _spaced(ret), [] if types == ["void"] else types))
+    return out
+
+
+def _ctype(decl: str, where: str):
+    t = _spaced(re.sub(r"\b(const|struct)\b", "", decl))
+    if t == "void":
+        return None
+    if t == "char*":
+        return C.c_char_p
+    if t.endswith("*"):
+        return C.c_void_p
+    if t in _SCALARS:
+        return _SCALARS[t]
+    raise MFError(f"{where}: no ctypes binding for the type '{decl.strip()}' ({HEADER})")
+
+
+EXPORTS = tuple(name for name, _, _ in _prototypes())
 
 
 def load_library():
-    """dlopen the in-tree CUDA library; loud failure if it has not been built."""
+    """dlopen the in-tree CUDA library and bind every function of include/maskfusion_b200.h; loud failure if it has not been built"""
     global _LIB
     if _LIB is not None:
         return _LIB
@@ -77,137 +95,19 @@ def load_library():
     if not os.path.exists(path):
         raise MFError(f"{path} not found: run `python -m maskfusion_b200.build` (there is no CPU fallback)")
     L = C.CDLL(path)
-    L.mf_last_error.restype = C.c_char_p
-    L.mf_create.restype = C.c_void_p
-    L.mf_create.argtypes = [C.POINTER(Config), C.c_int, C.c_void_p]
-    L.mf_destroy.argtypes = [C.c_void_p]
-    L.mf_config_defaults.argtypes = [C.POINTER(Config), C.c_int, C.c_int]
-    L.mf_process_frame.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int]
-    L.mf_process_frame_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int]
-    L.mf_set_input_event.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_kernel_launches.restype = C.c_int64
-    for name in ("mf_sync", "mf_tick", "mf_kernel_launches", "mf_model_count", "mf_frame_queue_size"):
-        getattr(L, name).argtypes = [C.c_void_p]
-    L.mf_set_frame_queue.argtypes = [C.c_void_p, C.c_int]
-    for name in ("mf_model_id", "mf_model_surfel_count", "mf_pose_log_size"):
-        getattr(L, name).argtypes = [C.c_void_p, C.c_int]
-    L.mf_get_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_set_pose.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_model_set_conf_threshold.argtypes = [C.c_void_p, C.c_int, C.c_float]
-    L.mf_download_surfels.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.mf_upload_surfels.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.mf_get_pose_log.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.mf_set_frame.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_model_perform_tracking.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_model_predict_indices.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.mf_model_fuse.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float]
-    L.mf_model_clean.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.mf_model_combined_predict.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
-    L.mf_model_init_from_frame.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.mf_download_filtered_depth.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_download_frame_maps.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_download_model_maps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    L.mf_download_index_map.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4
-    L.mf_download_prediction.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4
-    L.mf_download_fill_in.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 3
-    L.mf_download_association.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 3
-    L.mf_download_track_stats.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 3
-    L.mf_download_edge_map.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_debug_track_timing.argtypes = [C.c_void_p, C.c_int]
-    L.mf_attach_backbone.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.mf_backbone_stream.restype = C.c_void_p; L.mf_backbone_stream.argtypes = [C.c_void_p]
-    L.mf_morph_close.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    L.mf_set_frame_classes.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.mf_download_segmentation.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_model_class_id.argtypes = [C.c_void_p, C.c_int]
-    L.mf_set_profiling.argtypes = [C.c_void_p, C.c_int]
-    L.mf_get_stage_times.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
-    L.mf_debug_set_poses.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    L.mf_icp_step.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_klg_open.restype = C.c_void_p
-    L.mf_klg_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int]
-    for name in ("mf_klg_num_frames", "mf_klg_has_more", "mf_klg_close"):
-        getattr(L, name).argtypes = [C.c_void_p]
-    L.mf_klg_close.restype = None
-    L.mf_klg_get_next.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_klg_write.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_dir_open.restype = C.c_void_p
-    L.mf_dir_open.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p]
-    for name in ("mf_dir_num_frames", "mf_dir_has_more", "mf_dir_has_masks"):
-        getattr(L, name).argtypes = [C.c_void_p]
-    L.mf_dir_set_max_masks.argtypes = [C.c_void_p, C.c_int]
-    L.mf_dir_size.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.mf_dir_get_next.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int64)]
-    L.mf_dir_close.argtypes = [C.c_void_p]
-    L.mf_cnn_last_error.restype = C.c_char_p
-    L.mf_gemm_bf16.argtypes = [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_void_p]
-    L.mf_conv3x3_bf16.argtypes = [C.c_void_p] * 5 + [C.c_int] * 5 + [C.c_void_p]
-    L.mf_backbone_create.restype = C.c_void_p
-    L.mf_backbone_create.argtypes = [C.c_int, C.c_uint, C.c_void_p]
-    L.mf_backbone_destroy.argtypes = [C.c_void_p]; L.mf_backbone_destroy.restype = None
-    L.mf_backbone_num_layers.argtypes = [C.c_void_p]
-    L.mf_backbone_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_backbone_get_weights.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    L.mf_backbone_mold.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.mf_backbone_input_buffer.restype = C.c_void_p; L.mf_backbone_input_buffer.argtypes = [C.c_void_p]
-    L.mf_backbone_forward.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_backbone_output.restype = C.c_void_p; L.mf_backbone_output.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_backbone_flops.restype = C.c_double; L.mf_backbone_flops.argtypes = [C.c_void_p]
-    L.mf_backbone_num_gemms.argtypes = [C.c_void_p]
-    L.mf_backbone_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_rpn_create.restype = C.c_void_p; L.mf_rpn_create.argtypes = [C.c_void_p, C.c_uint]
-    L.mf_rpn_destroy.restype = None; L.mf_rpn_destroy.argtypes = [C.c_void_p]
-    L.mf_rpn_forward.argtypes = [C.c_void_p]
-    L.mf_rpn_run.argtypes = [C.c_void_p, C.c_int]
-    L.mf_rpn_num_anchors.argtypes = [C.c_void_p]
-    L.mf_rpn_propose.argtypes = [C.c_void_p] * 4 + [C.c_int]
-    L.mf_roi_align_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-    L.mf_rpn_get_weights.argtypes = [C.c_void_p] * 5
-    L.mf_rpn_get_anchors.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_rpn_get_head_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_rpn_download_conv.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_rpn_get_proposals.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_rpn_get_pooled.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_detector_create.restype = C.c_void_p; L.mf_detector_create.argtypes = [C.c_void_p, C.c_uint]
-    L.mf_detector_destroy.restype = None; L.mf_detector_destroy.argtypes = [C.c_void_p]
-    L.mf_detector_run.argtypes = [C.c_void_p, C.c_int]
-    L.mf_detector_forward.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.mf_detector_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.mf_detector_set_export.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    L.mf_detector_refine.argtypes = [C.c_void_p] * 4 + [C.c_int]
-    L.mf_detector_paste.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_int]
-    L.mf_detector_num_layers.argtypes = [C.c_void_p]
-    L.mf_detector_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_detector_get_weights.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    L.mf_detector_get_fc.argtypes = [C.c_void_p] * 3
-    L.mf_detector_get_head_outputs.argtypes = [C.c_void_p] * 3
-    L.mf_detector_get_mask_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.mf_detector_get_detections.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_detector_get_masks.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_detector_get_id_image.argtypes = [C.c_void_p] * 4
-    L.mf_detector_image_size.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.mf_attach_detector.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    for name in ("mf_backbone_load_weights", "mf_rpn_load_weights", "mf_detector_load_weights"):
-        getattr(L, name).argtypes = [C.c_void_p, C.c_char_p]
-    L.mf_mrcnn_read_layer.argtypes = [C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.mf_download_frame_masks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    L.mf_shard_configure.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.mf_shard_frame_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
-    L.mf_shard_unique_id.argtypes = [C.c_void_p]
-    L.mf_shard_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.mf_shard_process_frame.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int]
-    L.mf_shard_stats.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_shard_get_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.mf_shard_set_poses.argtypes = [C.c_void_p, C.c_void_p]
-    L.mf_shard_project.argtypes = [C.c_void_p]
-    L.mf_shard_projection_keys.restype = C.c_void_p; L.mf_shard_projection_keys.argtypes = [C.c_void_p]
-    L.mf_shard_frame_end.argtypes = [C.c_void_p, C.c_float]
-    L.mf_shard_attach_detector.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.mf_shard_frame_masks.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
-    L.mf_model_owner.argtypes = [C.c_void_p, C.c_int]
-    L.mf_shard_pick_owner.argtypes = [C.c_void_p, C.c_int]
+    for name, ret, params in _prototypes():
+        if not hasattr(L, name):
+            raise MFError(f"{path} lacks {name}, which the header declares: rebuild it (`python -m maskfusion_b200.build`)")
+        f = getattr(L, name)
+        f.restype = _ctype(ret, name)
+        f.argtypes = [_ctype(p, name) for p in params]
     _LIB = L
     return L
+
+
+def _error() -> MFError:
+    """the message of the calling thread's last failed call (mf_last_error)"""
+    return MFError(load_library().mf_last_error().decode())
 
 
 def default_config(width=640, height=480, **kw) -> Config:
@@ -353,11 +253,11 @@ class MaskFusion:
         self.W, self.H = self.cfg.width, self.cfg.height
         self.h = self.L.mf_create(C.byref(self.cfg), device, C.c_void_p(stream) if stream else None)
         if not self.h:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
 
     def _ck(self, r):
         if r < 0:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
         return r
 
     def close(self):
@@ -373,7 +273,6 @@ class MaskFusion:
 
     def exportPoses(self, exportDir: str) -> int:
         """MaskFusion::exportPoses: <exportDir>poses-<id>.txt per model"""
-        self.L.mf_export_poses.argtypes = [C.c_void_p, C.c_char_p]
         return self._ck(self.L.mf_export_poses(self.h, exportDir.encode()))
 
     def processFrame(self, rgb: np.ndarray, depth: np.ndarray, timestamp: int = 0, mask=None, inPose=None,
@@ -501,7 +400,7 @@ class KlgLogReader:
         self.W, self.H = width, height
         self.k = self.L.mf_klg_open(path.encode(), width, height, int(flipColors))
         if not self.k:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
 
     def getNumFrames(self):
         return self.L.mf_klg_num_frames(self.k)
@@ -513,7 +412,7 @@ class KlgLogReader:
         rgb = np.zeros((self.H, self.W, 3), np.uint8); depth = np.zeros((self.H, self.W), np.float32)
         ts = C.c_int64(0)
         if self.L.mf_klg_get_next(self.k, _p(rgb), _p(depth), C.byref(ts)) != 0:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
         return rgb, depth, ts.value
 
     def close(self):
@@ -526,10 +425,9 @@ def write_ply(path: str, surfels: np.ndarray, conf_threshold: float) -> int:
     """one model's cloud as MaskFusion::savePly writes it (MaskFusion.cpp:733-848); surfels = Model.downloadMap()"""
     L = load_library()
     a = np.ascontiguousarray(surfels, np.float32).reshape(-1, 12)
-    L.mf_write_ply.argtypes = [C.c_char_p, C.c_void_p, C.c_int, C.c_float]
     n = L.mf_write_ply(path.encode(), _p(a) if a.size else None, int(a.shape[0]), float(conf_threshold))
     if n < 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     return n
 
 
@@ -543,12 +441,10 @@ def generate_id_image(result: dict, min_score: float, class_filter=(), special_a
     rois = np.ascontiguousarray(result["rois"], np.int32).reshape(N, 4)
     cf = np.ascontiguousarray(list(class_filter), np.int32); sa = np.ascontiguousarray(list(special_assignments), np.int32)
     img = np.zeros((H, W), np.uint8); ec = np.zeros(max(N, 1), np.int32); er = np.zeros((max(N, 1), 4), np.int32)
-    L.mf_generate_id_image.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int,
-                                       C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     n = L.mf_generate_id_image(_p(masks), H, W, N, _p(scores), _p(cls), _p(rois), float(min_score), _p(cf) if cf.size else None, int(cf.size),
                                _p(sa) if sa.size else None, int(sa.size), _p(img), _p(ec), _p(er))
     if n < 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     return img, ec[:n].tolist(), er[:n].tolist()
 
 
@@ -562,12 +458,10 @@ def pre_segmentation(mask: np.ndarray, depth: np.ndarray, model_ids, next_model_
     assert mapping.dtype == np.uint8 and mapping.size == 256 and mapping.flags["C_CONTIGUOUS"]
     seg = np.zeros((H, W), np.uint8); has_new = C.c_int(0)
     spc = np.zeros(len(ids) + 1, np.uint32); mean = np.zeros(len(ids) + 1, np.float32); std = np.zeros(len(ids) + 1, np.float32)
-    L.mf_pre_segmentation.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                      C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p]
     n = L.mf_pre_segmentation(_p(m), _p(d), W, H, _p(ids), len(ids), int(next_model_id), int(bool(allow_new)), _p(mapping), _p(seg), C.byref(has_new),
                               _p(spc), _p(mean), _p(std))
     if n < 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     return seg, bool(has_new.value), spc[:n].copy(), mean[:n].copy(), std[:n].copy()
 
 
@@ -577,10 +471,10 @@ def decode_exr_depth(buf: bytes) -> np.ndarray:
     w, h = C.c_int(0), C.c_int(0)
     a = np.frombuffer(buf, np.uint8)
     if L.mf_decode_exr_depth(_p(a), int(a.shape[0]), None, 0, C.byref(w), C.byref(h)) != 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     out = np.zeros((h.value, w.value), np.float32)
     if L.mf_decode_exr_depth(_p(a), int(a.shape[0]), _p(out), out.size, C.byref(w), C.byref(h)) != 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     return out
 
 
@@ -590,10 +484,10 @@ def decode_jpeg(buf: bytes) -> np.ndarray:
     w, h = C.c_int(0), C.c_int(0)
     a = np.frombuffer(buf, np.uint8)
     if L.mf_decode_jpeg(_p(a), int(a.shape[0]), None, 0, C.byref(w), C.byref(h)) != 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     out = np.zeros((h.value, w.value, 3), np.uint8)
     if L.mf_decode_jpeg(_p(a), int(a.shape[0]), _p(out), out.size, C.byref(w), C.byref(h)) != 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
     return out
 
 
@@ -608,7 +502,7 @@ class ImageLogReader:
         self.r = self.L.mf_dir_open(colorDirectory.encode(), enc(depthDirectory), enc(maskDirectory), indexWidth, colorPrefix.encode(),
                                     depthPrefix.encode(), maskPrefix.encode())
         if not self.r:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
         w, h = C.c_int(0), C.c_int(0)
         self.L.mf_dir_size(self.r, C.byref(w), C.byref(h))
         self.W, self.H = w.value, h.value
@@ -631,7 +525,7 @@ class ImageLogReader:
         ids = np.zeros(256, np.int32); boxes = np.zeros((255, 4), np.int32); n = C.c_int(256); ts = C.c_int64(0)
         rc = self.L.mf_dir_get_next(self.r, _p(rgb), _p(depth), _p(mask), _p(ids), _p(boxes), C.byref(n), C.byref(ts))
         if rc < 0:
-            raise MFError(self.L.mf_last_error().decode())
+            raise _error()
         cls = ids[:n.value].copy() if n.value else None
         return rgb, depth, ts.value, (mask if rc == 1 else None), cls, (boxes[:n.value - 1].copy() if n.value > 1 else None)
 
@@ -648,17 +542,18 @@ def write_klg(path: str, timestamps, depth_mm: np.ndarray, rgb: np.ndarray):
     ts = np.ascontiguousarray(timestamps, np.int64)
     d = np.ascontiguousarray(depth_mm, np.uint16); c = np.ascontiguousarray(rgb, np.uint8)
     if L.mf_klg_write(path.encode(), W, H, n, _p(ts), _p(d), _p(c)) != 0:
-        raise MFError(L.mf_last_error().decode())
+        raise _error()
 
 
 class _CnnHandle:
-    """what the Mask R-CNN handles share: errors reported through mf_cnn_last_error, close() through their destroy function"""
+    """what the Mask R-CNN handles share: errors through mf_last_error (a None handle is a failed create), close() through their destroy
+    function"""
 
     _destroy = ""
 
     def _ck(self, r):
         if r is None or r < 0:
-            raise MFError(self.L.mf_cnn_last_error().decode())
+            raise _error()
         return r
 
     def close(self):
@@ -797,7 +692,7 @@ def roi_align(backbone: Backbone, boxes_ptr: int, n: int, pool: int, out_ptr: in
     enqueued on the backbone's stream"""
     L = load_library()
     if L.mf_roi_align_bf16(C.c_void_p(backbone.h), C.c_void_p(boxes_ptr) if n else None, int(n), int(pool), C.c_void_p(out_ptr) if n else None) != 0:
-        raise MFError(L.mf_cnn_last_error().decode())
+        raise _error()
 
 
 class Detector(_CnnHandle):
@@ -942,8 +837,8 @@ def read_mrcnn_layer(path: str, layer: str):
     L = load_library()
     dims = np.zeros(2, np.int32)
     if L.mf_mrcnn_read_layer(os.fsencode(path), layer.encode(), None, None, _p(dims)) != 0:
-        raise MFError(L.mf_cnn_last_error().decode())
+        raise _error()
     w = np.zeros((int(dims[0]), int(dims[1])), np.float32); b = np.zeros(int(dims[0]), np.float32)
     if L.mf_mrcnn_read_layer(os.fsencode(path), layer.encode(), _p(w), _p(b), _p(dims)) != 0:
-        raise MFError(L.mf_cnn_last_error().decode())
+        raise _error()
     return w, b

@@ -325,14 +325,13 @@ __global__ void k_mold_input(const uchar4* __restrict__ rgb, int W, int H, int S
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static PFN_encodeTiled g_encode = nullptr;
-static std::string g_cnn_err;
 
 static bool ensure_encode()
 {
     if (g_encode) return true;
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) { g_cnn_err = "cuTensorMapEncodeTiled not available"; return false; }
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) { mf_set_error("cuTensorMapEncodeTiled not available"); return false; }
     g_encode = (PFN_encodeTiled)fn;
     return true;
 }
@@ -345,7 +344,7 @@ static bool make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t K,
     cuuint32_t estr[2] = {1, 1};
     CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_cnn_err = "cuTensorMapEncodeTiled failed: " + std::to_string((int)r); return false; }
+    if (r != CUDA_SUCCESS) { mf_set_error("cuTensorMapEncodeTiled failed: " + std::to_string((int)r)); return false; }
     return true;
 }
 
@@ -358,7 +357,7 @@ static bool make_map_nhwc(CUtensorMap* m, const void* ptr, int C, int W, int H, 
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_cnn_err = "cuTensorMapEncodeTiled (3-D) failed: " + std::to_string((int)r); return false; }
+    if (r != CUDA_SUCCESS) { mf_set_error("cuTensorMapEncodeTiled (3-D) failed: " + std::to_string((int)r)); return false; }
     return true;
 }
 
@@ -387,8 +386,7 @@ static bool cached_map_nhwc(CUtensorMap* m, const void* ptr, int Cin, int Wimg, 
 template <int BN>
 static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 2 * GEMM_STAGES * 8 + 1024; }
 
-const char* cnn_last_error() { return g_cnn_err.c_str(); }
-int cnn_fail(const std::string& msg) { g_cnn_err = msg; return -1; }
+int cnn_fail(const std::string& msg) { mf_set_error(msg); return -1; }
 
 int cnn_check_launch(const char* what)
 {
@@ -421,14 +419,14 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
                      const int* conv3x3 /* Wimg, Himg, Cin */, bool outF32)
 {
     // every refusal comes before the first driver call
-    if (outF32 && residual) { g_cnn_err = "gemm: the fp32 output takes no residual"; return -2; }
+    if (outF32 && residual) { mf_set_error("gemm: the fp32 output takes no residual"); return -2; }
     ConvGeom geo; memset(&geo, 0, sizeof geo);
     if (conv3x3) {
         const int Wimg = conv3x3[0], Himg = conv3x3[1], Cin = conv3x3[2];
-        if (!cnn_conv_implicit(3, 1, 1, Cin, Himg, Wimg) || K != 9 * Cin || M != Wimg * Himg) { g_cnn_err = "conv3x3: unsupported geometry"; return -2; }
+        if (!cnn_conv_implicit(3, 1, 1, Cin, Himg, Wimg) || K != 9 * Cin || M != Wimg * Himg) { mf_set_error("conv3x3: unsupported geometry"); return -2; }
         geo.mode = 1; geo.Wimg = Wimg; geo.Himg = Himg; geo.Wbox = Wimg >= 128 ? 128 : Wimg; geo.Hbox = 128 / geo.Wbox; geo.cblocks = Cin / 64;
     }
-    if (K <= 0 || N <= 0 || M <= 0 || K % 64 || N % 64) { g_cnn_err = "gemm: need M > 0, and K > 0 and N > 0 multiples of 64"; return -2; }
+    if (K <= 0 || N <= 0 || M <= 0 || K % 64 || N % 64) { mf_set_error("gemm: need M > 0, and K > 0 and N > 0 multiples of 64"); return -2; }
     if (!ensure_encode()) return -1;
     const int mtiles = (M + GEMM_BM - 1) / GEMM_BM;
     // fill the machine: with few M tiles prefer the narrow N tile (twice the CTAs)
@@ -449,7 +447,7 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
         else launch_wgmma<64, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
     }
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_cnn_err = std::string("gemm launch: ") + cudaGetErrorString(e); return -4; }
+    if (e != cudaSuccess) { mf_set_error(std::string("gemm launch: ") + cudaGetErrorString(e)); return -4; }
     return 0;
 }
 
@@ -550,12 +548,11 @@ using namespace mfb;
 // ==========================================================================================
 struct mf_backbone : Backbone { using Backbone::Backbone; };
 
-extern "C" const char* mf_cnn_last_error(void) { return cnn_last_error(); }
-
 extern "C" int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, const void* dResidual, void* dOut, int M, int N, int K, int relu, void* stream)
 {
-    int rc = launch_gemm_bf16(dA, dB, dBias, dResidual, dOut, M, N, K, relu, (cudaStream_t)stream);
-    return rc;
+    MF_TRY
+    return launch_gemm_bf16(dA, dB, dBias, dResidual, dOut, M, N, K, relu, (cudaStream_t)stream);
+    MF_CATCH(-1)
 }
 
 // implicit-GEMM 3x3 / stride 1 / pad 1 convolution on an NHWC bf16 activation (weights [Cout][3][3][Cin] bf16); the geometry is
@@ -563,10 +560,12 @@ extern "C" int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, 
 extern "C" int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBias, const void* dResidual, void* dOut, int H, int W, int Cin, int Cout,
                                int relu, void* stream)
 {
+    MF_TRY
     int g3[3] = {W, H, Cin};
     // products in unsigned arithmetic: a refused geometry may overflow them, and the refusal does not read them
     return launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, (int)((unsigned)H * (unsigned)W), Cout, (int)(9u * (unsigned)Cin), relu, (cudaStream_t)stream,
                             g3);
+    MF_CATCH(-1)
 }
 
 // ResNet-101-FPN (mf_weights.cu has the layer table); throws CudaError
@@ -586,42 +585,42 @@ Backbone::Backbone(int S_, unsigned seed, cudaStream_t s) : S(S_), stream(s), w(
 
 extern "C" mf_backbone* mf_backbone_create(int input_size, unsigned seed, void* stream)
 {
+    MF_TRY
     if (input_size % 64) { cnn_fail("input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"); return nullptr; }
-    try {
-        return new mf_backbone(input_size, seed, (cudaStream_t)stream);
-    } catch (const CudaError& e) {
-        cnn_fail("backbone: " + e.what);
-        return nullptr;
-    }
+    return new mf_backbone(input_size, seed, (cudaStream_t)stream);
+    MF_CATCH_AS(nullptr, "backbone: ")
 }
 
 extern "C" void mf_backbone_destroy(mf_backbone* h) { delete h; }
 
-extern "C" int mf_backbone_num_layers(mf_backbone* h) { return h ? (int)h->layers.size() : cnn_fail("backbone: null handle"); }
+extern "C" int mf_backbone_num_layers(mf_backbone* h) { MF_TRY return h ? (int)h->layers.size() : cnn_fail("backbone: null handle"); MF_CATCH(-1) }
 // layer table: Cin Cout k stride pad Kpad
 extern "C" int mf_backbone_layer(mf_backbone* h, int i, int* out6)
 {
+    MF_TRY
     if (!h || i < 0 || i >= (int)h->layers.size() || !out6) return cnn_fail("backbone: bad layer index");
     const LayerGeom& L = h->layers[i];
     out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
     return 0;
+    MF_CATCH(-1)
 }
 // weights [Cout x Kpad] fp32 (bf16-representable), (ky,kx,cin) order along K; bias [Cout]
 extern "C" int mf_backbone_get_weights(mf_backbone* h, int i, float* w, float* bias)
 {
-    return h ? h->w.get(i, w, bias) : cnn_fail("backbone: null handle");
+    MF_TRY return h ? h->w.get(i, w, bias) : cnn_fail("backbone: null handle"); MF_CATCH(-1)
 }
 
 // pretrained weights (mf_weights.cu): every layer is read, checked and folded on the host before the device tables change; the copy is
 // ordered on the handle's stream and complete on return
 extern "C" int mf_backbone_load_weights(mf_backbone* h, const char* path)
 {
-    return h ? h->w.load(path, h->stream) : cnn_fail("backbone: null handle");
+    MF_TRY return h ? h->w.load(path, h->stream) : cnn_fail("backbone: null handle"); MF_CATCH(-1)
 }
 
 // forward on an already-moulded input (device, NHWC bf16 S x S x 3).  Outputs stay on the device (P2..P6, NHWC bf16).
 extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
 {
+    MF_TRY
     if (!h) return cnn_fail("backbone: null handle");
     Backbone* b = h; cudaStream_t s = h->stream;
     b->flops = 0; b->gemms = 0;
@@ -671,6 +670,7 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     }
     prof_mark(s, "k_subsample2"); k_subsample2<<<64, 256, 0, s>>>(b->P[3], fs[3], fs[3], 256, b->P[4]);       // P6
     return cnn_check_launch("backbone forward") ? -3 : 0;
+    MF_CATCH(-1)
 }
 extern "C" double mf_backbone_flops(mf_backbone* h) { return h ? h->flops : 0; }
 extern "C" int mf_backbone_num_gemms(mf_backbone* h) { return h ? h->gemms : 0; }
@@ -689,14 +689,17 @@ extern "C" void* mf_backbone_output(mf_backbone* h, int level, int* dims3)
 }
 extern "C" int mf_backbone_download(mf_backbone* h, int level, void* host_bf16)
 {
+    MF_TRY
     int d[3];
     void* p = mf_backbone_output(h, level, d);
     if (!p) return cnn_fail("backbone: no handle or level outside 0..8");
     return cnn_download(h->stream, host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2) ? -2 : 0;
+    MF_CATCH(-1)
 }
 // letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs; rule R-MOLD)
 extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H)
 {
+    MF_TRY
     if (!h) return cnn_fail("backbone: null handle");
     if (W <= 0 || H <= 0) return cnn_fail("mold: the image needs W > 0 and H > 0");
     Backbone* b = h; const int S = b->S;
@@ -707,4 +710,5 @@ extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H
     k_mold_input<<<dim3((S + 255) / 256, S), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, zoomx, zoomy, g.offx, g.offy, g.newW, g.newH,
                                                                    b->input);
     return cnn_check_launch("k_mold_input") ? -2 : 0;
+    MF_CATCH(-1)
 }

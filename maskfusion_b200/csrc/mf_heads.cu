@@ -323,22 +323,19 @@ mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed)
 
 extern "C" mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed)
 {
+    MF_TRY
     if (!rpn) { cnn_fail("detector: no region-proposal handle"); return nullptr; }
-    mf_detector* h;
-    try {
-        h = new mf_detector(rpn, seed);
-    } catch (const CudaError& e) {
-        cnn_fail("detector: " + e.what);
-        return nullptr;
-    }
+    mf_detector* h = new mf_detector(rpn, seed);
     if (set_image(h, h->S, h->S)) { delete h; return nullptr; }
     return h;
+    MF_CATCH_AS(nullptr, "detector: ")
 }
 
 extern "C" void mf_detector_destroy(mf_detector* h) { delete h; }
 
 extern "C" int mf_detector_run(mf_detector* h, int stages)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     const cudaStream_t s = h->s;
     if (stages & MF_DET_CLASSIFIER) {
@@ -361,29 +358,35 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
     }
     if ((stages & MF_DET_ID_IMAGE) && paste(h, h->dets, h->masks)) return -3;
     return 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_forward(mf_detector* h, int image_w, int image_h)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     if (set_image(h, image_w, image_h)) return -1;
     return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int H)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     if (!d_rgba || ((uintptr_t)d_rgba & 3)) return cnn_fail("detector: the image needs a 4-byte aligned device pointer");
     if (set_image(h, W, H)) return -1;
     if (mf_backbone_mold(h->bb, d_rgba, W, H) || mf_backbone_forward(h->bb, mf_backbone_input_buffer(h->bb)))
-        return cnn_fail(std::string("detector: backbone: ") + cnn_last_error());
+        return cnn_fail(std::string("detector: backbone: ") + mf_last_error());
     if (mf_rpn_forward(h->rpn)) return -3;
     return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const int32_t* class_filter, int n_filter, const int32_t* special_assignments,
                                       int n_special)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     if (n_filter < 0 || n_special < 0 || n_filter > EXPORT_CAP || n_special > EXPORT_CAP || (n_filter && !class_filter) || (n_special && !special_assignments))
         return cnn_fail("detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries");
@@ -394,62 +397,78 @@ extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const in
     for (int i = 0; i < n_special; ++i) ep.special[i] = special_assignments[i];
     h->ep = ep;
     return 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_refine(mf_detector* h, const float* d_rois, const float* d_logits, const float* d_deltas, int n)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     if (n < 1 || n > DET_ROIS) return cnn_fail("detector_refine: n = " + std::to_string(n) + " outside [1, 1000]");
     if (!d_rois || !d_logits || !d_deltas || ((uintptr_t)d_rois & 15) || ((uintptr_t)d_logits & 3) || ((uintptr_t)d_deltas & 3))
         return cnn_fail("detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer");
     return refine(h, d_rois, d_logits, NCLS, d_deltas, 4 * NCLS, n);
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_paste(mf_detector* h, const float* d_detections, const float* d_masks, int W, int H)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     if (!d_detections || !d_masks || ((uintptr_t)d_detections & 3) || ((uintptr_t)d_masks & 3))
         return cnn_fail("detector_paste: detections and masks need 4-byte aligned device pointers");
     if (set_image(h, W, H)) return -1;
     return paste(h, d_detections, d_masks);
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_num_layers(mf_detector* h) { return h ? N_LAYERS : -1; }
 
 extern "C" int mf_detector_layer(mf_detector* h, int i, int* out6)
 {
+    MF_TRY
     if (!h || i < 0 || i >= N_LAYERS || !out6) return cnn_fail("detector: bad layer index");
     const LayerGeom L = mrcnn_layer(MRCNN_DETECTOR, i);
     out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
     return 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* bias)
 {
+    MF_TRY
     return h ? h->w.get(i, w, bias) : cnn_fail("detector: bad layer index");
+    MF_CATCH(-1)
 }
 
 // pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
 extern "C" int mf_detector_load_weights(mf_detector* h, const char* path)
 {
+    MF_TRY
     return h ? h->w.load(path, h->s) : cnn_fail("detector: null handle");
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_fc(mf_detector* h, void* fc1_bf16, void* fc2_bf16)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     return cnn_download(h->s, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2) || cnn_download(h->s, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2) ? -1 : 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_head_outputs(mf_detector* h, float* logits, float* deltas)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     return cnn_download(h->s, logits, h->head, NCLS * 4, DET_ROIS, HEAD_N * 4) ||
                    cnn_download(h->s, deltas, h->head.p + NCLS, NCLS * 16, DET_ROIS, HEAD_N * 4) ? -1 : 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_mask_layer(mf_detector* h, int i, void* host)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     const size_t px = (size_t)DET_MAX * MPIX;
     switch (i) {
@@ -459,23 +478,29 @@ extern "C" int mf_detector_get_mask_layer(mf_detector* h, int i, void* host)
     case 6: return cnn_download(h->s, host, h->mlog, NCLS * 4, px * 4, MLOG_N * 4);
     default: return cnn_fail("detector: mask layer must be 0..6");
     }
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_detections(mf_detector* h, float* detections)
 {
+    MF_TRY
     int n = 0;
     if (!h) return cnn_fail("detector: null handle");
     if (cnn_download(h->s, detections, h->dets, DET_MAX * 6 * 4) || cnn_download(h->s, &n, h->count, 4)) return -1;
     return n;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_masks(mf_detector* h, float* masks)
 {
+    MF_TRY
     return h ? cnn_download(h->s, masks, h->masks, DET_MAX * MASK * MASK * 4) : cnn_fail("detector: null handle");
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32_t* class_ids, int32_t* rois)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     int info[2];
     if (cnn_download(h->s, info, h->einfo, 8)) return -1;
@@ -483,11 +508,14 @@ extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32
     if (cnn_download(h->s, id_image, h->idimg, (size_t)h->imgW * h->imgH) || cnn_download(h->s, class_ids, h->ecls, (size_t)info[0] * 4) ||
         cnn_download(h->s, rois, h->erois, (size_t)info[0] * 16)) return -1;
     return info[0];
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_image_size(mf_detector* h, int* w, int* hgt)
 {
+    MF_TRY
     if (!h) return cnn_fail("detector: null handle");
     *w = h->imgW; *hgt = h->imgH;
     return 0;
+    MF_CATCH(-1)
 }

@@ -794,7 +794,7 @@ void MaskFusion::attachNetwork(const char* who, bool asDetector, mf_detector* de
     if (!asDetector && (detector || detRank >= 0))
         throw CudaError{std::string(who) + ": a detector is attached (it runs its own backbone on the same stream); detach it first"};
     waitNetwork();
-    if (det && detector_reserve_image(det, W, H) != 0) throw CudaError{std::string(who) + ": " + cnn_last_error()};
+    if (det && detector_reserve_image(det, W, H) != 0) throw CudaError{std::string(who) + ": " + mf_last_error()};
     if (!netRGBA.p) netRGBA.alloc(P);
 }
 
@@ -882,7 +882,7 @@ void MaskFusion::runNetwork(int slot, bool runBackbone)
         if (mf_backbone_forward(bb, mf_backbone_input_buffer(bb)) != 0) throw CudaError{"backbone: forward failed"};
     } else {
         if (mf_detector_detect(detector, netRGBA, W, H) != 0 || detector_frame_masks(detector, slotMask(slot), slotHdr(slot)) != 0)
-            throw CudaError{std::string("detector: ") + cnn_last_error()};
+            throw CudaError{std::string("detector: ") + mf_last_error()};
         // one event for both guards: the slot may be reused, and its mask / header are written
         cudaCheck(cudaEventRecord(f.netDone, ns), "cudaEventRecord");
         f.netUsed = true; f.handoff = true;

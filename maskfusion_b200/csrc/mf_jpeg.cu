@@ -10,6 +10,7 @@
 //   colour conversion   jdcolor.c YCbCr -> RGB, 16-bit fixed-point tables with ONE_HALF rounding
 // Pinned against OpenCV's decoder (libjpeg-turbo, bit-compatible with libjpeg for these methods) in tests/test_cpu_loader.py.
 // Progressive, arithmetic-coded, 12-bit and CMYK files are refused.
+#include "mf_kernels.h"
 #include <stdint.h>
 #include <string.h>
 #include <string>
@@ -334,11 +335,10 @@ bool decodeJPEG(const uint8_t* data, size_t size, int& W, int& H, std::vector<ui
 }  // namespace mfb
 
 // test hook behind the C ABI: decode a JPEG byte stream to RGB (out must hold width*height*3 bytes; call with out == NULL for the size)
-extern void mf_set_error(const std::string& e);
 extern "C" int mf_decode_jpeg(const uint8_t* data, int size, uint8_t* out, int capacity, int* width, int* height)
 {
+    MF_TRY
     if (!data || size <= 0) { mf_set_error("decode_jpeg: empty input"); return -1; }
-    try {
     int W = 0, H = 0; std::vector<uint8_t> rgb; std::string err;
     if (!mfb::decodeJPEG(data, (size_t)size, W, H, rgb, err)) { mf_set_error(err); return -2; }
     if (width) *width = W;
@@ -348,6 +348,5 @@ extern "C" int mf_decode_jpeg(const uint8_t* data, int size, uint8_t* out, int c
         memcpy(out, rgb.data(), rgb.size());
     }
     return 0;
-    } catch (const std::exception& e) { mf_set_error(std::string("decode_jpeg: ") + e.what()); return -4; }
-    catch (...) { mf_set_error("decode_jpeg: unknown error"); return -4; }
+    MF_CATCH(-4)
 }

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <exception>
 #include <string>
 #include <vector>
 #include "mf_common.cuh"
@@ -11,6 +12,18 @@
 struct mf_backbone;
 struct mf_rpn;
 struct mf_detector;
+
+// the calling thread's error message, which mf_last_error() returns (mf_capi.cu); every C ABI entry point reports through it
+void mf_set_error(const std::string& msg);
+
+// the guard of every extern "C" function that can fail: nothing thrown below it unwinds into the caller's frames.  A CudaError's text is
+// stored after `cudaPrefix`, any other exception as "<entry point>: <what()>"; the function then returns `ret`.
+#define MF_TRY try {
+#define MF_CATCH_AS(ret, cudaPrefix)                                                                          \
+    } catch (const mfb::CudaError& e) { mf_set_error(cudaPrefix + e.what); return ret; }                      \
+    catch (const std::exception& e) { mf_set_error(std::string(__func__) + ": " + e.what()); return ret; }     \
+    catch (...) { mf_set_error(std::string(__func__) + ": unknown error"); return ret; }
+#define MF_CATCH(ret) MF_CATCH_AS(ret, std::string())
 
 namespace mfb {
 
@@ -170,7 +183,7 @@ void prof_mark(cudaStream_t s, const char* name);
 
 // ---- mf_cnn.cu ----
 // D[M x N] = relu?(A[M x K] * B[N x K]^T + bias + residual), bf16 operands; conv3x3 = {Wimg, Himg, Cin}: A is an NHWC activation and the GEMM is
-// the implicit 3x3/s1/p1 convolution; outF32: D is fp32 (no residual), else bf16.  Returns 0 or < 0 with the text in cnn_last_error()
+// the implicit 3x3/s1/p1 convolution; outF32: D is fp32 (no residual), else bf16.  Returns 0 or < 0 with the text in mf_last_error()
 int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
                      const int* conv3x3 = nullptr, bool outF32 = false);
 // one convolution (NHWC bf16, weights [Cout][Kpad] in (ky, kx, cin) order) through the backbone's conv path: the implicit 3x3 GEMM where its
@@ -183,8 +196,7 @@ void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout
 // the letter-box rule of mf_backbone_mold (mould_image): a W x H image is resized by `scale` to newW x newH and placed at (offx, offy) of S x S
 struct MoldGeom { float scale; int newW, newH, offx, offy; };
 MoldGeom cnn_mold_geometry(int S, int W, int H);
-const char* cnn_last_error();
-// what the backbone, RPN and detector handles share: the message into cnn_last_error() and -1; a failed launch; a read-back of `rows` rows
+// what the backbone, RPN and detector handles share: the message into mf_last_error() and -1; a failed launch; a read-back of `rows` rows
 // of `width` bytes, `pitch` bytes apart on the device (0: one block), packed into dst after `s` is drained.  dst NULL: nothing is copied
 int cnn_fail(const std::string& msg);
 int cnn_check_launch(const char* what);
@@ -212,7 +224,7 @@ struct WeightStore {
     // the seeded tables (one LCG stream, seed 0 taken as 1), uploaded on `s`; throws CudaError
     WeightStore(int part, unsigned seed, cudaStream_t s);
     // every layer read, checked and folded on the host, uploaded on `s` and complete on return; the tables change only on success.
-    // 0, or -1 with the message in cnn_last_error() naming the file and the tensor (-2: the upload failed)
+    // 0, or -1 with the message in mf_last_error() naming the file and the tensor (-2: the upload failed)
     int load(const char* path, cudaStream_t s);
     int get(int i, float* w, float* b, int rows = -1) const;    // the first `rows` rows (-1: all) of layer i; NULL skips
     const __nv_bfloat16* w(int i) const { return dW.p + wOff[i]; }

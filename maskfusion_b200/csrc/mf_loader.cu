@@ -12,6 +12,7 @@
 // The reference's background buffering thread (:203-220) is an I/O detail and is not reproduced: frames are decoded on demand.
 #include "../../include/maskfusion_b200.h"
 #include "mf_boxes.cuh"
+#include "mf_kernels.h"
 #include <dirent.h>
 #include <stdio.h>
 #include <stdint.h>
@@ -20,10 +21,10 @@
 #include <zlib.h>
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <string>
 #include <vector>
 
-extern void mf_set_error(const std::string& e);          // mf_capi.cu (thread-local message behind mf_last_error)
 #define MF_MAX_IMAGE_SIDE 16384          // decoders refuse larger headers before allocating (a crafted IHDR must not throw across the C ABI)
 namespace mfb { bool decodeJPEG(const uint8_t* data, size_t size, int& W, int& H, std::vector<uint8_t>& rgb, std::string& err); }   // mf_jpeg.cu
 
@@ -342,10 +343,9 @@ static int countFiles(const std::string& dir, const std::string& prefix, const s
 extern "C" mf_dir* mf_dir_open(const char* color_dir, const char* depth_dir, const char* mask_dir, int index_width, const char* color_prefix,
                                const char* depth_prefix, const char* mask_prefix)
 {
+    MF_TRY
     if (!color_dir) { mf_set_error("mf_dir_open: null colour directory"); return nullptr; }
-    mf_dir* r = nullptr;
-    try {
-    r = new mf_dir;
+    std::unique_ptr<mf_dir> r(new mf_dir);
     r->colorDir = withSlash(color_dir); r->depthDir = withSlash(depth_dir && *depth_dir ? depth_dir : color_dir);
     r->maskDir = withSlash(mask_dir && *mask_dir ? mask_dir : "");
     r->colorPre = color_prefix ? color_prefix : ""; r->depthPre = depth_prefix ? depth_prefix : ""; r->maskPre = mask_prefix ? mask_prefix : "";
@@ -358,22 +358,21 @@ extern "C" mf_dir* mf_dir_open(const char* color_dir, const char* depth_dir, con
     int nc = countFiles(r->colorDir, r->colorPre, {".jpg", ".png", ".ppm"}, r->colorExt, err);
     int nd = nc < 0 ? -1 : countFiles(r->depthDir, r->depthPre, {".exr", ".png"}, r->depthExt, err);
     int nm = (nd < 0 || noMaskDir) ? 0 : countFiles(r->maskDir, r->maskPre, {".png", ".pgm"}, r->maskExt, err);
-    if (nc < 0 || nd < 0 || nm < 0) { mf_set_error(err); delete r; return nullptr; }
+    if (nc < 0 || nd < 0 || nm < 0) { mf_set_error(err); return nullptr; }
     if (nm > 0) { r->hasMasks = true; r->maxMasks = (size_t)nm; }
-    if (nc != nd) { mf_set_error("Error: Number of RGB-frames != Depth-frames!"); delete r; return nullptr; }
-    if (r->hasMasks && nc != nm) { mf_set_error("Error: Number of RGB-frames != Mask-frames!"); delete r; return nullptr; }
+    if (nc != nd) { mf_set_error("Error: Number of RGB-frames != Depth-frames!"); return nullptr; }
+    if (r->hasMasks && nc != nm) { mf_set_error("Error: Number of RGB-frames != Mask-frames!"); return nullptr; }
     r->numFrames = nc;
     int index = 0;
     for (; index < 2; ++index)
         if (exists(r->colorDir + r->colorPre + indexString(r->indexW, (size_t)index) + r->colorExt)) { r->startIndex = (unsigned)index; break; }
-    if (index == 2) { mf_set_error("Error: Could not find start index."); delete r; return nullptr; }
+    if (index == 2) { mf_set_error("Error: Could not find start index."); return nullptr; }
     // image size from the first colour frame (the reference takes it from Resolution::getInstance())
     Image im;
-    if (!loadImage(r->colorDir + r->colorPre + indexString(r->indexW, r->startIndex) + r->colorExt, r->colorExt, im, err)) { mf_set_error(err); delete r; return nullptr; }
+    if (!loadImage(r->colorDir + r->colorPre + indexString(r->indexW, r->startIndex) + r->colorExt, r->colorExt, im, err)) { mf_set_error(err); return nullptr; }
     r->W = im.w; r->H = im.h;
-    return r;
-    } catch (const std::exception& e) { mf_set_error(std::string("mf_dir_open: ") + e.what()); delete r; return nullptr; }
-    catch (...) { mf_set_error("mf_dir_open: unknown error"); delete r; return nullptr; }
+    return r.release();
+    MF_CATCH(nullptr)
 }
 extern "C" void mf_dir_close(mf_dir* r) { delete r; }
 extern "C" int mf_dir_num_frames(mf_dir* r) { return r ? r->numFrames : -1; }
@@ -385,19 +384,18 @@ extern "C" int mf_dir_size(mf_dir* r, int* w, int* h) { if (!r) return -1; if (w
 // test hook behind the C ABI: an OpenEXR byte stream -> the float depth image the reader delivers (out == NULL: only the size)
 extern "C" int mf_decode_exr_depth(const uint8_t* data, int size, float* out, int capacity, int* width, int* height)
 {
+    MF_TRY
     if (!data || size <= 0) { mf_set_error("decode_exr_depth: empty input"); return -1; }
-    try {
-        std::vector<uint8_t> f(data, data + size); std::vector<float> d; int W = 0, H = 0; std::string err;
-        if (!decodeEXRDepth(f, W, H, d, err)) { mf_set_error(err); return -2; }
-        if (width) *width = W;
-        if (height) *height = H;
-        if (out) {
-            if ((size_t)capacity < d.size()) { mf_set_error("decode_exr_depth: output buffer too small"); return -3; }
-            memcpy(out, d.data(), d.size() * sizeof(float));
-        }
-        return 0;
-    } catch (const std::exception& e) { mf_set_error(std::string("decode_exr_depth: ") + e.what()); return -4; }
-    catch (...) { mf_set_error("decode_exr_depth: unknown error"); return -4; }
+    std::vector<uint8_t> f(data, data + size); std::vector<float> d; int W = 0, H = 0; std::string err;
+    if (!decodeEXRDepth(f, W, H, d, err)) { mf_set_error(err); return -2; }
+    if (width) *width = W;
+    if (height) *height = H;
+    if (out) {
+        if ((size_t)capacity < d.size()) { mf_set_error("decode_exr_depth: output buffer too small"); return -3; }
+        memcpy(out, d.data(), d.size() * sizeof(float));
+    }
+    return 0;
+    MF_CATCH(-4)
 }
 
 // ImageLogReader::getNext + loadFrameFromDrive (:222-288).  mask / class_ids / boxes may be NULL.  *n_class_ids: in = capacity of
@@ -406,9 +404,9 @@ extern "C" int mf_decode_exr_depth(const uint8_t* data, int size, float* out, in
 extern "C" int mf_dir_get_next(mf_dir* r, uint8_t* rgb, float* depth, uint8_t* mask, int32_t* class_ids, int32_t* boxes, int* n_class_ids,
                                int64_t* timestamp)
 {
+    MF_TRY
     if (!r) { mf_set_error("null reader"); return -1; }
     if (!rgb || !depth) { mf_set_error("mf_dir_get_next: null output buffer"); return -1; }
-    try {
     if (r->currentFrame + 1 >= r->numFrames) { mf_set_error("no more frames"); return -2; }
     const size_t index = (size_t)(r->currentFrame + 1);
     const std::string idx = indexString(r->indexW, index + r->startIndex);
@@ -479,8 +477,7 @@ extern "C" int mf_dir_get_next(mf_dir* r, uint8_t* rgb, float* depth, uint8_t* m
     if (timestamp) *timestamp = (int64_t)((float)index * 1000.0f / r->rateHz);        // :283 (float product truncated into the int64 field)
     r->currentFrame++;
     return gotMask;
-    } catch (const std::exception& e) { mf_set_error(std::string("mf_dir_get_next: ") + e.what()); return -9; }
-    catch (...) { mf_set_error("mf_dir_get_next: unknown error"); return -9; }
+    MF_CATCH(-9)
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -501,44 +498,44 @@ extern "C" int mf_pre_segmentation(const uint8_t* mask, const float* depth, int 
                                    int allow_new, uint8_t* mapping, uint8_t* full_segmentation, int* has_new_label, uint32_t* super_pixel_count,
                                    float* depth_mean, float* depth_std)
 {
+    MF_TRY
     if (!mask || !depth || !model_ids || !mapping || !full_segmentation || !super_pixel_count || !depth_mean || !depth_std || W <= 0 || H <= 0 ||
         n_models < 1 || n_models > 255 || next_model_id < 0 || next_model_id > 255) { mf_set_error("mf_pre_segmentation: bad arguments"); return -1; }
-    try {
-        const size_t P = (size_t)W * H;
-        unsigned char modelIdToIndex[256];
-        memset(modelIdToIndex, 0, sizeof modelIdToIndex);                 // (uninitialised in the reference; ids outside the list never occur in its output)
-        for (int i = 0; i < n_models; ++i) modelIdToIndex[model_ids[i]] = (unsigned char)i;
-        modelIdToIndex[next_model_id] = (unsigned char)n_models;
-        std::vector<unsigned> outIds(256, 0);
-        bool hasNew = false;
-        for (size_t i = 0; i < P; ++i) {
-            const unsigned char vIn = mask[i];
-            unsigned char vOut = 0;
-            if (vIn) {
-                if (mapping[vIn] != 0) { vOut = mapping[vIn]; outIds[vOut]++; }
-                else if (allow_new && !hasNew) { vOut = (unsigned char)next_model_id; mapping[vIn] = vOut; hasNew = true; outIds[vOut]++; }
-            } else outIds[0]++;
-            full_segmentation[i] = vOut;
-        }
-        const int n = n_models + (hasNew ? 1 : 0);
-        for (int i = 0; i < n_models; ++i) super_pixel_count[i] = outIds[model_ids[i]] / (16 * 16);
-        if (hasNew) { const float c = (float)(outIds[next_model_id] / (16 * 16)); super_pixel_count[n_models] = (unsigned)(c > 1.0f ? c : 1.0f); }
-        std::vector<unsigned> cnts(n, 0);
-        for (int i = 0; i < n; ++i) { depth_mean[i] = 0.f; depth_std[i] = 0.f; }
-        for (size_t i = 0; i < P; ++i) { const size_t k = modelIdToIndex[full_segmentation[i]]; if ((int)k < n) { depth_mean[k] += depth[i]; cnts[k]++; } }
-        for (int i = 0; i < n; ++i) depth_mean[i] /= cnts[i] ? cnts[i] : 1;
-        for (size_t i = 0; i < P; ++i) { const size_t k = modelIdToIndex[full_segmentation[i]]; if ((int)k < n) depth_std[k] += std::abs(depth_mean[k] - depth[i]); }
-        for (int i = 0; i < n; ++i) depth_std[i] /= cnts[i] ? cnts[i] : 1;
-        if (has_new_label) *has_new_label = hasNew ? 1 : 0;
-        return n;
-    } catch (const std::exception& e) { mf_set_error(std::string("mf_pre_segmentation: ") + e.what()); return -2; }
-    catch (...) { mf_set_error("mf_pre_segmentation: unknown error"); return -2; }
+    const size_t P = (size_t)W * H;
+    unsigned char modelIdToIndex[256];
+    memset(modelIdToIndex, 0, sizeof modelIdToIndex);                 // (uninitialised in the reference; ids outside the list never occur in its output)
+    for (int i = 0; i < n_models; ++i) modelIdToIndex[model_ids[i]] = (unsigned char)i;
+    modelIdToIndex[next_model_id] = (unsigned char)n_models;
+    std::vector<unsigned> outIds(256, 0);
+    bool hasNew = false;
+    for (size_t i = 0; i < P; ++i) {
+        const unsigned char vIn = mask[i];
+        unsigned char vOut = 0;
+        if (vIn) {
+            if (mapping[vIn] != 0) { vOut = mapping[vIn]; outIds[vOut]++; }
+            else if (allow_new && !hasNew) { vOut = (unsigned char)next_model_id; mapping[vIn] = vOut; hasNew = true; outIds[vOut]++; }
+        } else outIds[0]++;
+        full_segmentation[i] = vOut;
+    }
+    const int n = n_models + (hasNew ? 1 : 0);
+    for (int i = 0; i < n_models; ++i) super_pixel_count[i] = outIds[model_ids[i]] / (16 * 16);
+    if (hasNew) { const float c = (float)(outIds[next_model_id] / (16 * 16)); super_pixel_count[n_models] = (unsigned)(c > 1.0f ? c : 1.0f); }
+    std::vector<unsigned> cnts(n, 0);
+    for (int i = 0; i < n; ++i) { depth_mean[i] = 0.f; depth_std[i] = 0.f; }
+    for (size_t i = 0; i < P; ++i) { const size_t k = modelIdToIndex[full_segmentation[i]]; if ((int)k < n) { depth_mean[k] += depth[i]; cnts[k]++; } }
+    for (int i = 0; i < n; ++i) depth_mean[i] /= cnts[i] ? cnts[i] : 1;
+    for (size_t i = 0; i < P; ++i) { const size_t k = modelIdToIndex[full_segmentation[i]]; if ((int)k < n) depth_std[k] += std::abs(depth_mean[k] - depth[i]); }
+    for (int i = 0; i < n; ++i) depth_std[i] /= cnts[i] ? cnts[i] : 1;
+    if (has_new_label) *has_new_label = hasNew ? 1 : 0;
+    return n;
+    MF_CATCH(-2)
 }
 
 extern "C" int mf_generate_id_image(const uint8_t* masks, int H, int W, int N, const float* scores, const int32_t* class_ids, const int32_t* rois,
                                     double min_score, const int32_t* class_filter, int n_filter, const int32_t* special_assignments, int n_special,
                                     uint8_t* id_image, int32_t* exported_class_ids, int32_t* exported_rois)
 {
+    MF_TRY
     if (N > 256) { mf_set_error("Too many masks in image."); return -1; }                 // helpers.py:78-79
     if (!id_image || (N > 0 && (!masks || !scores || !class_ids || !rois))) { mf_set_error("generate_id_image: null argument"); return -2; }
     const size_t P = (size_t)H * W;
@@ -556,6 +553,7 @@ extern "C" int mf_generate_id_image(const uint8_t* masks, int H, int W, int N, c
         ++n;
     }
     return n;
+    MF_CATCH(-1)
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -565,6 +563,7 @@ extern "C" int mf_generate_id_image(const uint8_t* masks, int H, int W, int N, c
 // nx ny nz (float, NEGATED as the reference does) radius (float), binary little endian.  Returns the number of vertices written.
 extern "C" int mf_write_ply(const char* path, const float* surfels, int n, float conf_threshold)
 {
+    MF_TRY
     if (!path || (n > 0 && !surfels) || n < 0) { mf_set_error("write_ply: bad arguments"); return -1; }
     int valid = 0;
     for (int i = 0; i < n; ++i) if (surfels[(size_t)i * 12 + 3] > conf_threshold) ++valid;      // SurfelMap::countValid
@@ -585,4 +584,5 @@ extern "C" int mf_write_ply(const char* path, const float* surfels, int n, float
     }
     fclose(fp);
     return valid;
+    MF_CATCH(-1)
 }

@@ -342,19 +342,17 @@ mf_rpn::mf_rpn(mf_backbone* bb_, unsigned seed) : bb(bb_), s((cudaStream_t)mf_ba
 
 extern "C" mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed)
 {
+    MF_TRY
     if (!bb) { cnn_fail("rpn: no backbone"); return nullptr; }
-    try {
-        return new mf_rpn(bb, seed);
-    } catch (const CudaError& e) {
-        cnn_fail("rpn: " + e.what);
-        return nullptr;
-    }
+    return new mf_rpn(bb, seed);
+    MF_CATCH_AS(nullptr, "rpn: ")
 }
 
 extern "C" void mf_rpn_destroy(mf_rpn* h) { delete h; }
 
 extern "C" int mf_rpn_run(mf_rpn* h, int stages)
 {
+    MF_TRY
     if (!h) return cnn_fail("rpn: null handle");
     const cudaStream_t s = h->s;
     if (stages & MF_RPN_CONV)
@@ -372,72 +370,91 @@ extern "C" int mf_rpn_run(mf_rpn* h, int stages)
     if ((stages & MF_RPN_PROPOSALS) && propose(h, h->logits, h->deltas, h->anchors, h->A)) return -3;
     if ((stages & MF_RPN_ROI_ALIGN) && roi_align(h->bb, h->rois, RPN_POST_NMS, RPN_POOL, h->pooled, s)) return -3;
     return 0;
+    MF_CATCH(-1)
 }
 
-extern "C" int mf_rpn_forward(mf_rpn* h) { return mf_rpn_run(h, MF_RPN_CONV | MF_RPN_HEADS | MF_RPN_PROPOSALS | MF_RPN_ROI_ALIGN); }
+extern "C" int mf_rpn_forward(mf_rpn* h) { MF_TRY return mf_rpn_run(h, MF_RPN_CONV | MF_RPN_HEADS | MF_RPN_PROPOSALS | MF_RPN_ROI_ALIGN); MF_CATCH(-1) }
 
 extern "C" int mf_rpn_propose(mf_rpn* h, const float* d_logits, const float* d_deltas, const float* d_anchors, int n_anchors)
 {
+    MF_TRY
     if (!h) return cnn_fail("rpn: null handle");
     if (n_anchors < 1 || n_anchors > h->A)
         return cnn_fail("rpn_propose: n_anchors = " + std::to_string(n_anchors) + " outside [1, " + std::to_string(h->A) + "]");
     if (!d_logits || !d_deltas || !d_anchors || ((uintptr_t)d_logits & 7) || ((uintptr_t)d_deltas & 15) || ((uintptr_t)d_anchors & 15))
         return cnn_fail("rpn_propose: logits need 8-byte, deltas and anchors 16-byte aligned device pointers");
     return propose(h, d_logits, d_deltas, d_anchors, n_anchors) ? -3 : 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_roi_align_bf16(mf_backbone* bb, const float* d_boxes, int n, int pool, void* d_out)
 {
+    MF_TRY
     if (!bb) return cnn_fail("roi_align: no backbone");
     if (n < 0 || pool < 2 || pool > 64) return cnn_fail("roi_align: need n >= 0 and 2 <= pool <= 64");
     if (n > 0 && (!d_boxes || !d_out || ((uintptr_t)d_boxes & 15) || ((uintptr_t)d_out & 3)))
         return cnn_fail("roi_align: boxes need a 16-byte, out a 4-byte aligned device pointer");
     return roi_align(bb, d_boxes, n, pool, d_out, (cudaStream_t)mf_backbone_stream(bb)) ? -3 : 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_num_anchors(mf_rpn* h) { return h ? h->A : -1; }
 
 extern "C" int mf_rpn_get_weights(mf_rpn* h, float* conv_w, float* conv_b, float* head_w, float* head_b)
 {
+    MF_TRY
     if (!h) return cnn_fail("rpn: null handle");
     return h->w.get(0, conv_w, conv_b) || h->w.get(1, head_w, head_b, 18) ? -1 : 0;     // head rows 0..5 logits, 6..17 deltas
+    MF_CATCH(-1)
 }
 
 // pretrained weights (mf_weights.cu): read, checked and folded on the host first; the copy is ordered on the stream and complete on return
 extern "C" int mf_rpn_load_weights(mf_rpn* h, const char* path)
 {
+    MF_TRY
     return h ? h->w.load(path, h->s) : cnn_fail("rpn: null handle");
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_anchors(mf_rpn* h, float* anchors)
 {
+    MF_TRY
     return h ? cnn_download(h->s, anchors, h->anchors, (size_t)h->A * 16) : cnn_fail("rpn: null handle");
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_head_outputs(mf_rpn* h, float* logits, float* deltas)
 {
+    MF_TRY
     if (!h) return cnn_fail("rpn: null handle");
     return cnn_download(h->s, logits, h->logits, (size_t)h->A * 8) || cnn_download(h->s, deltas, h->deltas, (size_t)h->A * 16) ? -1 : 0;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_download_conv(mf_rpn* h, int level, void* host_bf16)
 {
+    MF_TRY
     if (!h) return cnn_fail("rpn: null handle");
     if (level < 0 || level > 4) return cnn_fail("rpn: level must be 0..4 (P2..P6)");
     return cnn_download(h->s, host_bf16, h->conv.p + (size_t)h->pixOff[level] * RPN_MID, (size_t)h->lh[level] * h->lh[level] * RPN_MID * 2);
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_proposals(mf_rpn* h, float* rois)
 {
+    MF_TRY
     int n = 0;
     if (!h) return cnn_fail("rpn: null handle");
     if (cnn_download(h->s, rois, h->rois, RPN_POST_NMS * 16) || cnn_download(h->s, &n, h->count, 4)) return -1;
     return n;
+    MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16)
 {
+    MF_TRY
     return h ? cnn_download(h->s, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) : cnn_fail("rpn: null handle");
+    MF_CATCH(-1)
 }
 
 // ---- what the detection heads (mf_heads.cu) read of the handle ----

@@ -451,6 +451,7 @@ int WeightStore::get(int i, float* w, float* b, int rows) const
 // one handle layer as the loaders fold it, without a CUDA device: dims = {rows, K}; w / bias NULL: only the dims
 extern "C" int mf_mrcnn_read_layer(const char* path, const char* layer, float* w_rows_K, float* bias_rows, int* dims)
 {
+    MF_TRY
     for (int part = 0; part < 3; ++part)
         for (const LayerSpec& s : specs(part)) {
             if (!layer || s.name != layer) continue;
@@ -461,4 +462,5 @@ extern "C" int mf_mrcnn_read_layer(const char* path, const char* layer, float* w
             return 0;
         }
     return mfb::cnn_fail(std::string("mrcnn_read_layer: no layer named '") + (layer ? layer : "(null)") + "'");
+    MF_CATCH(-1)
 }
