@@ -104,7 +104,7 @@ extern "C" int mf_sync(mf_context* ctx) { MF_TRY MF_NEED(ctx) ctx->mf->sync(); r
 extern "C" int mf_tick(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return ctx->mf->tick; }
 extern "C" int mf_set_frame_queue(mf_context* ctx, int length) { MF_TRY MF_NEED(ctx) ctx->mf->setFrameQueue(length); return 0; MF_CATCH(-1) }
 extern "C" int mf_frame_queue_size(mf_context* ctx) { MF_TRY if (!ctx || !ctx->mf) { mf_set_error("null context"); return -1; } return ctx->mf->queued; MF_CATCH(-1) }
-extern "C" int64_t mf_kernel_launches(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return ctx->mf->launches; }
+extern "C" int64_t mf_kernel_launches(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return ctx->mf->rec.launches; }
 
 extern "C" int mf_model_count(mf_context* ctx) { if (!ctx || !ctx->mf) return -1; return (int)ctx->mf->models.size(); }
 extern "C" int mf_model_id(mf_context* ctx, int i) { MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) return m->id; MF_CATCH(-1) }
@@ -121,7 +121,7 @@ extern "C" int mf_download_surfels(mf_context* ctx, int i, float* out, int max_s
     if ((int)n > max_surfels) n = (uint32_t)max_surfels;
     if (!n) return 0;
     DevBuf<float4> tmp; tmp.alloc((size_t)n * 3);
-    launch_planes_to_aos(m->current(), n, tmp, o->stream);
+    launch_planes_to_aos(m->current(), n, tmp, o->on());
     cudaCheck(cudaMemcpyAsync(out, tmp.p, (size_t)n * 48, cudaMemcpyDeviceToHost, o->stream), "surfel D2H");
     o->sync();
     return (int)n;
@@ -135,7 +135,7 @@ extern "C" int mf_upload_surfels(mf_context* ctx, int i, const float* in, int n)
     if (n) {
         DevBuf<float4> tmp; tmp.alloc((size_t)n * 3);
         cudaCheck(cudaMemcpyAsync(tmp.p, in, (size_t)n * 48, cudaMemcpyHostToDevice, o->stream), "surfel H2D");
-        launch_aos_to_planes(tmp, (uint32_t)n, m->current(), o->stream);
+        launch_aos_to_planes(tmp, (uint32_t)n, m->current(), o->on());
         o->sync();
     }
     uint32_t c = (uint32_t)n;
@@ -243,7 +243,7 @@ static void d2h(MaskFusion* o, void* dst, const T* src, size_t n)
 static void planarOut(MaskFusion* o, const float4* map, int P, float* out)
 {
     if (!out) return;
-    launch_map_to_planar(map, P, o->scratch, o->stream);
+    launch_map_to_planar(map, P, o->scratch, o->on());
     cudaCheck(cudaMemcpyAsync(out, o->scratch.p, (size_t)P * 3 * sizeof(float), cudaMemcpyDeviceToHost, o->stream), "D2H");
     o->sync();
 }
@@ -307,7 +307,7 @@ extern "C" int mf_download_association(mf_context* ctx, int i, uint8_t* flag, ui
     d2h(o, flag, m->aflag.p, o->P); d2h(o, best, m->abest.p, o->P);
     if (meas12) {
         DevBuf<float4> tmp; tmp.alloc((size_t)o->P * 3);
-        launch_planes_to_aos(SurfelPlanes{m->meas[0].p, m->meas[1].p, m->meas[2].p}, (uint32_t)o->P, tmp, o->stream);
+        launch_planes_to_aos(SurfelPlanes{m->meas[0].p, m->meas[1].p, m->meas[2].p}, (uint32_t)o->P, tmp, o->on());
         cudaCheck(cudaMemcpyAsync(meas12, tmp.p, (size_t)o->P * 48, cudaMemcpyDeviceToHost, o->stream), "D2H");
         o->sync();
     }
@@ -348,8 +348,8 @@ extern "C" int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int i
     MaskFusion* o = ctx->mf;
     DevBuf<uint8_t> a, b, c; a.alloc(o->P); b.alloc(o->P); c.alloc(o->P);
     cudaCheck(cudaMemcpyAsync(a.p, image, o->P, cudaMemcpyHostToDevice, o->stream), "H2D");
-    if (ellipse) o->launches += launch_morph_close_ellipse(a, b, o->W, o->H, radius, iterations, nullptr, o->stream);
-    else { launch_morph_close_invert(a, b, o->W, o->H, radius, iterations, c, o->stream); o->launches += 1 + 2 * iterations; }
+    if (ellipse) launch_morph_close_ellipse(a, b, o->W, o->H, radius, iterations, nullptr, o->on());
+    else launch_morph_close_invert(a, b, o->W, o->H, radius, iterations, c, o->on());
     d2h(o, image, a.p, o->P);
     if (inverted && !ellipse) d2h(o, inverted, c.p, o->P);
     o->sync(); return 0;
@@ -503,8 +503,9 @@ extern "C" int mf_set_profiling(mf_context* ctx, int on)
 {
     MF_TRY MF_NEED(ctx)
     ctx->mf->sync();
-    ctx->mf->prof.on = on != 0; ctx->mf->prof.used = 0;
-    if (on) ctx->mf->prof.acc.clear();
+    Profiler& p = ctx->mf->rec.prof;
+    p.on = on != 0; p.used = 0;
+    if (on) p.acc.clear();
     return 0;
     MF_CATCH(-1)
 }
@@ -514,7 +515,7 @@ extern "C" int mf_get_stage_times(mf_context* ctx, char* buf, int bufsize)
     ctx->mf->sync();
     std::string out;
     char line[256];
-    for (auto& kv : ctx->mf->prof.acc) { snprintf(line, sizeof line, "%s %ld %.6f\n", kv.first.c_str(), kv.second.first, kv.second.second); out += line; }
+    for (auto& kv : ctx->mf->rec.prof.acc) { snprintf(line, sizeof line, "%s %ld %.6f\n", kv.first.c_str(), kv.second.first, kv.second.second); out += line; }
     if ((int)out.size() + 1 > bufsize) { mf_set_error("buffer too small"); return -6; }
     memcpy(buf, out.c_str(), out.size() + 1);
     return (int)out.size();
@@ -547,8 +548,7 @@ extern "C" int mf_icp_step(mf_context* ctx, int i, int level, const float* Rcurr
     DevBuf<float> out; out.alloc(32);
     DevBuf<unsigned> ticket; ticket.alloc(1); ticket.zero(o->stream);
     launch_icp_only(o->vmap[level], o->nmap[level], m->vmapG[level], m->nmapG[level], o->W >> level, o->H >> level, camLevel(o->cam, level), pp,
-                    m->partial, ticket, out, o->numSMs, o->stream);
-    o->launches += 1;
+                    m->partial, ticket, out, o->numSMs, o->on());
     cudaCheck(cudaMemcpyAsync(out29, out.p, 29 * sizeof(float), cudaMemcpyDeviceToHost, o->stream), "D2H");
     o->sync();
     return 0;

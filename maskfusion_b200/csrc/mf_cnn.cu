@@ -438,11 +438,9 @@ int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void
     if (!cached_map(&mB, B, (uint64_t)N, (uint64_t)K, (uint32_t)BN)) return -3;
     dim3 grid(mtiles, N / BN);
     if (outF32) {
-        prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128_f32" : "k_gemm_bf16_wgmma_n64_f32");
         if (BN == 128) launch_wgmma<128, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
         else launch_wgmma<64, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
     } else {
-        prof_mark(s, BN == 128 ? "k_gemm_bf16_wgmma_n128" : "k_gemm_bf16_wgmma_n64");
         if (BN == 128) launch_wgmma<128, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
         else launch_wgmma<64, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
     }
@@ -491,9 +489,9 @@ static int conv_layer(const LayerGeom& L, const __nv_bfloat16* W, const float* B
     }
     if (!(L.k == 1 && L.stride == 1)) {
         if (L.k == 1 && L.stride == 2 && (L.cin % 8) == 0) {
-            prof_mark(s, "k_subsample2"); k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.cin, col);
+            k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.cin, col);
         } else {
-            prof_mark(s, "k_im2col"); k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.K, col);
+            k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.K, col);
         }
         A = col;
     }
@@ -516,7 +514,6 @@ static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int W
 
 void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int k, int stride, int pad, int Kpad, void* col, cudaStream_t s)
 {
-    prof_mark(s, "k_im2col");
     k_im2col<<<8 * num_sms(), 256, 0, s>>>((const __nv_bfloat16*)in, nimg, Hin, Win, Cin, Hout, Wout, k, k, stride, pad, Kpad, (__nv_bfloat16*)col);
 }
 
@@ -629,7 +626,7 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     int li = 0;                                      // the next layer of the table
     // C1: 7x7/2 + ReLU, max-pool 3x3/2
     if (run_conv(b, li++, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W)) return -2;
-    prof_mark(s, "k_maxpool3s2"); k_maxpool3s2<<<8 * num_sms(), 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
+    k_maxpool3s2<<<8 * num_sms(), 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
     H /= 2; W /= 2;
     __nv_bfloat16* x = b->bufB;                      // current block input
     const int nblocks[4] = {3, 4, 23, 3};
@@ -664,11 +661,11 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     for (int i = 2; i >= 0; --i) {
         if (run_conv(b, fpnLat + i, Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s)) return -2;
         __nv_bfloat16* nt = tdBuf[i & 1];
-        prof_mark(s, "k_upsample_add"); k_upsample_add<<<8 * num_sms(), 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
+        k_upsample_add<<<8 * num_sms(), 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
         top = nt;
         if (run_conv(b, fpnOut + i, top, fs[i], fs[i], b->P[i], nullptr, 0, s)) return -2;
     }
-    prof_mark(s, "k_subsample2"); k_subsample2<<<64, 256, 0, s>>>(b->P[3], fs[3], fs[3], 256, b->P[4]);       // P6
+    k_subsample2<<<64, 256, 0, s>>>(b->P[3], fs[3], fs[3], 256, b->P[4]);       // P6
     return cnn_check_launch("backbone forward") ? -3 : 0;
     MF_CATCH(-1)
 }
@@ -706,7 +703,6 @@ extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H
     const MoldGeom g = cnn_mold_geometry(S, W, H);
     const double zoomx = (double)W / (double)g.newW, zoomy = (double)H / (double)g.newH;     // in / out per axis (R-MOLD)
     if (S > 65535) return cnn_fail("mold: the input size exceeds the grid's 65535 rows");
-    prof_mark(h->stream, "k_mold_input");
     k_mold_input<<<dim3((S + 255) / 256, S), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, zoomx, zoomy, g.offx, g.offy, g.newW, g.newH,
                                                                    b->input);
     return cnn_check_launch("k_mold_input") ? -2 : 0;

@@ -418,61 +418,61 @@ __global__ void k_project_points3(Maps3 m, int W0, int H0, Cam cam0)
 // ------------------------------ host launchers ----------------------------------------
 static inline dim3 grid2(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y); }
 
-void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, cudaStream_t s) { k_unpack_rgb<<<(P + 255) / 256, 256, 0, s>>>(rgb3, out, P); }
-void launch_bilateral(const float* depth, float* out, int W, int H, cudaStream_t s)
+void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, Enq q) { launch(q, nullptr, k_unpack_rgb, (P + 255) / 256, 256, 0, rgb3, out, P); }
+void launch_bilateral(const float* depth, float* out, int W, int H, Enq q)
 {
     // the bulk copies need 16-byte aligned rows (MaskFusion rejects W % 4 != 0; the raw depth sits 16-byte aligned in its frame buffer)
     if (W % 4 != 0 || ((uintptr_t)depth & 15) != 0) throw CudaError{"bilateral filter: depth rows must be 16-byte aligned (W % 4 == 0, aligned image)"};
     dim3 b(BIL_BX, BIL_BY);
-    prof_mark(s, "k_bilateral"); k_bilateral<<<grid2(W, H, b), b, 0, s>>>(depth, out, W, H);
+    launch(q, "k_bilateral", k_bilateral, grid2(W, H, b), b, 0, depth, out, W, H);
 }
-void launch_pyrdown2_f(const float* src, int sw, int sh, float* dst1, float* dst2, cudaStream_t s)
+void launch_pyrdown2_f(const float* src, int sw, int sh, float* dst1, float* dst2, Enq q)
 {
     dim3 g((sw / 4 + PY_TX - 1) / PY_TX, (sh / 4 + PY_TY - 1) / PY_TY);
-    prof_mark(s, "k_pyrdown2_f"); k_pyrdown2<PyrF><<<g, 256, 0, s>>>(src, sw, sh, dst1, dst2);
+    launch(q, "k_pyrdown2_f", k_pyrdown2<PyrF>, g, 256, 0, src, sw, sh, dst1, dst2);
 }
-void launch_pyrdown2_pair(const float* srcF, float* dstF1, float* dstF2, const uint8_t* srcU, uint8_t* dstU1, uint8_t* dstU2, int sw, int sh, cudaStream_t s)
+void launch_pyrdown2_pair(const float* srcF, float* dstF1, float* dstF2, const uint8_t* srcU, uint8_t* dstU1, uint8_t* dstU2, int sw, int sh, Enq q)
 {
     dim3 g((sw / 4 + PY_TX - 1) / PY_TX, (sh / 4 + PY_TY - 1) / PY_TY, 2);
-    prof_mark(s, "k_pyrdown2_pair"); k_pyrdown2_pair<<<g, 256, 0, s>>>(srcF, dstF1, dstF2, srcU, dstU1, dstU2, sw, sh);
+    launch(q, "k_pyrdown2_pair", k_pyrdown2_pair, g, 256, 0, srcF, dstF1, dstF2, srcU, dstU1, dstU2, sw, sh);
 }
-void launch_pyrdown2_u8(const uint8_t* src, int sw, int sh, uint8_t* dst1, uint8_t* dst2, cudaStream_t s)
+void launch_pyrdown2_u8(const uint8_t* src, int sw, int sh, uint8_t* dst1, uint8_t* dst2, Enq q)
 {
     dim3 g((sw / 4 + PY_TX - 1) / PY_TX, (sh / 4 + PY_TY - 1) / PY_TY);
-    prof_mark(s, "k_pyrdown2_u8"); k_pyrdown2<PyrU8><<<g, 256, 0, s>>>(src, sw, sh, dst1, dst2);
+    launch(q, "k_pyrdown2_u8", k_pyrdown2<PyrU8>, g, 256, 0, src, sw, sh, dst1, dst2);
 }
-void launch_vmap_nmap3(const float* const* depth, int W, int H, Cam cam, float cutoff, float4* const* vmap, float4* const* nmap, cudaStream_t s)
+void launch_vmap_nmap3(const float* const* depth, int W, int H, Cam cam, float cutoff, float4* const* vmap, float4* const* nmap, Enq q)
 {
     Maps3 m = {};
     for (int l = 0; l < 3; ++l) { m.depth[l] = depth[l]; m.vmap[l] = vmap[l]; m.nmap[l] = nmap[l]; }
     dim3 b(32, 8), g = grid2(W, H, b); g.z = 3;
-    prof_mark(s, "k_vmap_nmap3"); k_vmap_nmap3<<<g, b, 0, s>>>(m, W, H, cam, cutoff);
+    launch(q, "k_vmap_nmap3", k_vmap_nmap3, g, b, 0, m, W, H, cam, cutoff);
 }
-void launch_sobel3(const uint8_t* const* img, int W, int H, short2* const* grad, uint8_t* const* rgbValid, cudaStream_t s)
+void launch_sobel3(const uint8_t* const* img, int W, int H, short2* const* grad, uint8_t* const* rgbValid, Enq q)
 {
     Maps3 m = {};
     for (int l = 0; l < 3; ++l) { m.img[l] = img[l]; m.grad[l] = grad[l]; m.valid[l] = rgbValid[l]; m.minScale[l] = track_min_scale(l); }
     dim3 b(32, 8), g = grid2(W, H, b); g.z = 3;
-    prof_mark(s, "k_sobel3"); k_sobel3<<<g, b, 0, s>>>(m, W, H);
+    launch(q, "k_sobel3", k_sobel3, g, b, 0, m, W, H);
 }
-void launch_project_points3(const float* const* depth, int W, int H, Cam cam, float4* const* cloud, cudaStream_t s)
+void launch_project_points3(const float* const* depth, int W, int H, Cam cam, float4* const* cloud, Enq q)
 {
     Maps3 m = {};
     for (int l = 0; l < 3; ++l) { m.depth[l] = depth[l]; m.cloud[l] = cloud[l]; }
     dim3 b(32, 8), g = grid2(W, H, b); g.z = 3;
-    prof_mark(s, "k_project_points3"); k_project_points3<<<g, b, 0, s>>>(m, W, H, cam);
+    launch(q, "k_project_points3", k_project_points3, g, b, 0, m, W, H, cam);
 }
-void launch_intensity(const uchar4* img, int P, uint8_t* out, cudaStream_t s) { k_intensity<<<(P + 255) / 256, 256, 0, s>>>(img, P, out); }
-void launch_intensity_select(const uchar4* imgPred, const uchar4* imgFill, const uint32_t* nonBlack, float denom, int forceFill, int P, uint8_t* out, cudaStream_t s)
+void launch_intensity(const uchar4* img, int P, uint8_t* out, Enq q) { launch(q, nullptr, k_intensity, (P + 255) / 256, 256, 0, img, P, out); }
+void launch_intensity_select(const uchar4* imgPred, const uchar4* imgFill, const uint32_t* nonBlack, float denom, int forceFill, int P, uint8_t* out, Enq q)
 {
-    prof_mark(s, "k_intensity_select"); k_intensity_select<<<(P + 255) / 256, 256, 0, s>>>(imgPred, imgFill, nonBlack, denom, forceFill, P, out);
+    launch(q, "k_intensity_select", k_intensity_select, (P + 255) / 256, 256, 0, imgPred, imgFill, nonBlack, denom, forceFill, P, out);
 }
 void launch_model_maps(const float4* srcVp, const float4* srcNp, const float4* srcVf, const float4* srcNf, const uint32_t* nonBlack, float denom,
-                       int W, int H, const DevPose* pose, float maxDepthRGB, float4* const* v, float4* const* n, float* depth0, cudaStream_t s)
+                       int W, int H, const DevPose* pose, float maxDepthRGB, float4* const* v, float4* const* n, float* depth0, Enq q)
 {
     int threads = (W / 4) * (H / 4) * 4;
-    prof_mark(s, "k_model_maps"); k_model_maps<<<(threads + 127) / 128, 128, 0, s>>>(srcVp, srcNp, srcVf, srcNf, nonBlack, denom, W, H, pose, maxDepthRGB,
-                                                       v[0], n[0], v[1], n[1], v[2], n[2], depth0);
+    launch(q, "k_model_maps", k_model_maps, (threads + 127) / 128, 128, 0, srcVp, srcNp, srcVf, srcNf, nonBlack, denom, W, H, pose, maxDepthRGB,
+           v[0], n[0], v[1], n[1], v[2], n[2], depth0);
 }
 // validity bitmask of a model's normal maps, three levels in one launch (blockIdx.y = level): the tracker tests the bit of the pixel a
 // frame vertex projects to BEFORE gathering the model vertex / normal there.  An object model covers a few per cent of the image, so
@@ -491,12 +491,12 @@ __global__ void k_valid_bits3(const float4* __restrict__ n0, const float4* __res
     const unsigned m = __ballot_sync(0xffffffffu, ok);
     if ((threadIdx.x & 31) == 0) b[i >> 5] = m;
 }
-void launch_valid_bits3(const float4* const* nmap, int W, int H, uint32_t* const* bits, cudaStream_t s)
+void launch_valid_bits3(const float4* const* nmap, int W, int H, uint32_t* const* bits, Enq q)
 {
     const int N0 = W * H;
     dim3 g((N0 + 255) / 256, 3);
-    prof_mark(s, "k_valid_bits3"); k_valid_bits3<<<g, 256, 0, s>>>(nmap[0], nmap[1], nmap[2], N0, bits[0], bits[1], bits[2]);
+    launch(q, "k_valid_bits3", k_valid_bits3, g, 256, 0, nmap[0], nmap[1], nmap[2], N0, bits[0], bits[1], bits[2]);
 }
-void launch_map_to_planar(const float4* m, int P, float* out, cudaStream_t s) { k_map_to_planar<<<(P + 255) / 256, 256, 0, s>>>(m, P, out); }
+void launch_map_to_planar(const float4* m, int P, float* out, Enq q) { launch(q, nullptr, k_map_to_planar, (P + 255) / 256, 256, 0, m, P, out); }
 
 }  // namespace mfb

@@ -264,7 +264,6 @@ int detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr)
     const size_t P = (size_t)h->imgW * h->imgH;
     if (P % 16 || ((uintptr_t)mask & 15)) return cnn_fail("detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer");
     const int n16 = (int)(P / 16);
-    prof_mark(h->s, "k_frame_masks");
     k_frame_masks<<<(n16 + 255) / 256, 256, 0, h->s>>>((const uint4*)h->idimg.p, h->einfo, h->ecls, n16, (uint4*)mask, hdr);
     return cnn_check_launch("k_frame_masks");
 }
@@ -278,18 +277,14 @@ static int gemm(mf_detector* h, int layer, const void* A, void* out, int M, int 
 
 static int refine(mf_detector* h, const float* rois, const float* logits, int lstride, const float* deltas, int dstride, int n)
 {
-    prof_mark(h->s, "k_det_refine");
     k_det_refine<<<(n + 127) / 128, 128, 0, h->s>>>((const float4*)rois, logits, lstride, deltas, dstride, n, h->win, h->keys, h->boxes, h->scores);
-    prof_mark(h->s, "k_det_select");
     k_det_select<<<1, SEL_N, 0, h->s>>>(h->keys, n, h->boxes, h->scores, h->dets, h->dboxes, h->count);
     return cnn_check_launch("detection layer") ? -3 : 0;
 }
 
 static int paste(mf_detector* h, const float* dets, const float* masks)
 {
-    prof_mark(h->s, "k_unmold");
     k_unmold<<<1, 1, 0, h->s>>>(dets, h->win, h->imgW, h->imgH, h->ep, h->ebox, h->eid, h->ecls, h->erois, h->einfo);
-    prof_mark(h->s, "k_paste");
     k_paste<<<(h->imgW * h->imgH + 255) / 256, 256, 0, h->s>>>(masks, h->ebox, h->eid, h->einfo, h->imgW, h->imgH, h->idimg);
     return cnn_check_launch("id image") ? -3 : 0;
 }
@@ -352,7 +347,6 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
             x = h->mconv[i];
         }
         if (gemm(h, L_DECONV, x, h->dec, DET_MAX * MPIX, 1, false) || gemm(h, L_MLOG, h->dec, h->mlog, DET_MAX * MPIX * 4, 0, true)) return -2;
-        prof_mark(s, "k_mask_select");
         k_mask_select<<<(DET_MAX * MASK * MASK + 255) / 256, 256, 0, s>>>(h->mlog, h->dets, h->masks);
         if (cnn_check_launch("k_mask_select")) return -3;
     }

@@ -24,13 +24,18 @@ Mat4 rigidInverse(const Mat4& T);
 Mat4 mul(const Mat4& A, const Mat4& B);
 Rt toRt(const Mat4& T);
 
+// in-stream stage timer: one CUDA event per mark; the interval up to the next mark is attributed to the mark's name.  Off by default.
 struct Profiler {
     bool on = false; int used = 0;
     std::vector<cudaEvent_t> events; std::vector<const char*> names;
     std::map<std::string, std::pair<long, double>> acc;      // name -> (count, total ms)
     void resolve();
 };
-extern Profiler* g_prof;
+// what a context records about the kernels it enqueues through its Enq (MaskFusion::on)
+struct LaunchRecord {
+    int64_t launches = 0;               // mf_kernel_launches
+    Profiler prof;
+};
 
 class MaskFusion;
 
@@ -44,9 +49,9 @@ struct ShardComm {
     void allReduceMinU64(uint64_t* buf, size_t count, cudaStream_t s);                               // ID-projection keys (GlobalProjection.cpp:66-95)
 };
 void shardUniqueId(unsigned char* out128);
-void launch_pack_rows(const LifeParams& lp, float* table, cudaStream_t s);
-void launch_lifecycle(const LifeParams& lp, const float* gathered, FrameResult* res, cudaStream_t s);
-void launch_set_count(uint32_t* c, uint32_t v, cudaStream_t s);
+void launch_pack_rows(const LifeParams& lp, float* table, Enq q);
+void launch_lifecycle(const LifeParams& lp, const float* gathered, FrameResult* res, Enq q);
+void launch_set_count(uint32_t* c, uint32_t v, Enq q);
 
 class Model {
 public:
@@ -210,7 +215,8 @@ public:
     mf_config cfg; Cam cam; int W, H, P; int device; cudaStream_t stream; bool ownStream;
     int numSMs = 132;
     int tick = 1;
-    int64_t launches = 0;
+    LaunchRecord rec;
+    Enq on(cudaStream_t s = nullptr) { return Enq{s ? s : stream, &rec}; }     // where this context's launches go (nullptr: the main stream)
     std::vector<std::unique_ptr<Model>> models;
     unsigned char nextID = 0;
     // frame
@@ -262,7 +268,6 @@ public:
     DevBuf<float> scratch;                  // read-back staging
     DevBuf<float4> rayTab;                  // viewing ray of every pixel centre (camera constant): read by the splat rasteriser
     bool frameMapsValid = false, intensityValid = false;
-    Profiler prof;
     // multi-model state
     std::vector<int32_t> classIDs;          // of the frame being processed
     int spawnOffset = 0;

@@ -255,7 +255,6 @@ static int roi_align(mf_backbone* bb, const float* boxes, int n, int pool, void*
     mf_backbone_output(bb, 4, d);
     const int S = d[0] * 4;
     const float areaScale = (float)((double)S * (double)S / (224.0 * 224.0));
-    prof_mark(s, "k_roi_align");
     k_roi_align<<<dim3(n, pool), RPN_CH / 2, 0, s>>>((const float4*)boxes, pool, roi_levels(bb), areaScale, (__nv_bfloat16*)out);
     return cnn_check_launch("k_roi_align");
 }
@@ -266,7 +265,6 @@ static int propose(mf_rpn* h, const float* logits, const float* deltas, const fl
     const cudaStream_t s = h->s;
     const int k = n < RPN_PRE_NMS ? n : RPN_PRE_NMS;
     const int grid = (n + 255) / 256, histGrid = std::min((n + 2047) / 2048, 2 * num_sms());
-    prof_mark(s, "k_rpn_keys");
     k_rpn_keys<<<grid, 256, 0, s>>>((const float2*)logits, n, k, h->keys, h->st);
     int shifts[8], np = 0;
     for (int sh = 56; sh >= 32; sh -= 8) shifts[np++] = sh;
@@ -275,19 +273,13 @@ static int propose(mf_rpn* h, const float* logits, const float* deltas, const fl
     for (int sh = 24; sh >= 0; sh -= 8)
         if (sh < idxBits) shifts[np++] = sh;
     for (int p = 0; p < np; ++p) {
-        prof_mark(s, "k_sel_hist");
         k_sel_hist<<<histGrid, 256, 0, s>>>(h->keys, n, h->st, shifts[p]);
-        prof_mark(s, "k_sel_pick");
         k_sel_pick<<<1, 256, 0, s>>>(h->st, shifts[p]);
     }
-    prof_mark(s, "k_sel_compact");
     k_sel_compact<<<grid, 256, 0, s>>>(h->keys, n, h->st, h->sel);
-    prof_mark(s, "k_sort_decode");
     k_sort_decode<<<1, 1024, SORT_CAP * sizeof(unsigned long long), s>>>(h->sel, k, (const float4*)deltas, (const float4*)anchors, h->boxes);
     const int words = (k + 63) / 64;
-    prof_mark(s, "k_nms_mask");
     k_nms_mask<<<dim3(words, words), 64, 0, s>>>(h->boxes, k, words, h->mask);
-    prof_mark(s, "k_nms_scan");
     k_nms_scan<<<1, 32, 0, s>>>(h->boxes, h->mask, k, words, (float4*)h->rois.p, h->count);
     return cnn_check_launch("proposal layer");
 }
@@ -363,7 +355,6 @@ extern "C" int mf_rpn_run(mf_rpn* h, int stages)
         }
     if (stages & MF_RPN_HEADS) {
         if (launch_gemm_bf16(h->conv, h->w.w(1), h->w.b(1), nullptr, h->head, h->pixels, RPN_HEAD_N, RPN_MID, 0, s, nullptr, true)) return -2;
-        prof_mark(s, "k_rpn_split");
         k_rpn_split<<<std::min((h->pixels * 18 + 255) / 256, 8 * num_sms()), 256, 0, s>>>(h->head, h->pixels, h->logits, h->deltas);
         if (cnn_check_launch("k_rpn_split")) return -3;
     }

@@ -66,13 +66,13 @@ __global__ void k_lifecycle(LifeParams lp, const float* __restrict__ gathered, F
     for (int k = 0; k < 16; ++k) { res->poses[i][k] = pose[k]; res->poses[i][16 + k] = last[k]; }
 }
 
-void launch_pack_rows(const LifeParams& lp, float* table, cudaStream_t s) { prof_mark(s, "k_pack_rows"); k_pack_rows<<<MF_MAX_MODELS, 32, 0, s>>>(lp, table); }
-void launch_lifecycle(const LifeParams& lp, const float* gathered, FrameResult* res, cudaStream_t s)
+void launch_pack_rows(const LifeParams& lp, float* table, Enq q) { launch(q, "k_pack_rows", k_pack_rows, MF_MAX_MODELS, 32, 0, lp, table); }
+void launch_lifecycle(const LifeParams& lp, const float* gathered, FrameResult* res, Enq q)
 {
-    prof_mark(s, "k_lifecycle"); k_lifecycle<<<1, MF_MAX_MODELS, 0, s>>>(lp, gathered, res);
+    launch(q, "k_lifecycle", k_lifecycle, 1, MF_MAX_MODELS, 0, lp, gathered, res);
 }
 __global__ void k_set_count(uint32_t* c, uint32_t v) { if (threadIdx.x == 0 && blockIdx.x == 0) *c = v; }
-void launch_set_count(uint32_t* c, uint32_t v, cudaStream_t s) { k_set_count<<<1, 32, 0, s>>>(c, v); }
+void launch_set_count(uint32_t* c, uint32_t v, Enq q) { launch(q, nullptr, k_set_count, 1, 32, 0, c, v); }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // NCCL, opened at run time.  Only the handful of entry points the exchange needs; types follow nccl.h (ABI-stable across 2.x).

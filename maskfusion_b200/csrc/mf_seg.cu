@@ -87,9 +87,9 @@ __global__ void k_morph_ellipse(const uint8_t* __restrict__ in, uint8_t* __restr
     out[y * W + x] = (uint8_t)best;
 }
 // closes `data` in place (buf: scratch of the same size): dilate x iterations, then erode x iterations
-int launch_morph_close_ellipse(uint8_t* data, uint8_t* buf, int W, int H, int radius, int iterations, const FrameHdr* onlyIfMasks, cudaStream_t s)
+void launch_morph_close_ellipse(uint8_t* data, uint8_t* buf, int W, int H, int radius, int iterations, const FrameHdr* onlyIfMasks, Enq q)
 {
-    if (iterations <= 0) return 0;
+    if (iterations <= 0) return;
     if (radius < 0 || radius > 16) throw CudaError{"morphMaskRadius must be in 0..16"};
     EllipseRows e; e.r = radius;
     const double inv_r2 = radius ? 1.0 / ((double)radius * radius) : 0.0;
@@ -101,26 +101,25 @@ int launch_morph_close_ellipse(uint8_t* data, uint8_t* buf, int W, int H, int ra
     uint8_t* src = data; uint8_t* dst = buf;
     for (int pass = 0; pass < 2; ++pass)
         for (int i = 0; i < iterations; ++i) {
-            prof_mark(s, "k_morph_ellipse"); k_morph_ellipse<<<g, b, 0, s>>>(src, dst, W, H, e, pass == 0, onlyIfMasks);
+            launch(q, "k_morph_ellipse", k_morph_ellipse, g, b, 0, src, dst, W, H, e, pass == 0, onlyIfMasks);
             uint8_t* t = src; src = dst; dst = t;
         }
-    // 2 * iterations launches: the result is back in `data`
-    return 2 * iterations;
+    // an even number of passes: the result is back in `data`
 }
 
-void launch_geometric_edges(const float4* vmap, const float4* nmap, int W, int H, float wD, float wC, float thr, float* edge, uint8_t* binary, cudaStream_t s)
+void launch_geometric_edges(const float4* vmap, const float4* nmap, int W, int H, float wD, float wC, float thr, float* edge, uint8_t* binary, Enq q)
 {
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
-    prof_mark(s, "k_geometric_edges"); k_geometric_edges<<<g, b, 0, s>>>(vmap, nmap, W, H, wD, wC, thr, edge, binary);
+    launch(q, "k_geometric_edges", k_geometric_edges, g, b, 0, vmap, nmap, W, H, wD, wC, thr, edge, binary);
 }
-void launch_morph_close_invert(uint8_t* data, uint8_t* buf, int W, int H, int radius, int iterations, uint8_t* inverted, cudaStream_t s)
+void launch_morph_close_invert(uint8_t* data, uint8_t* buf, int W, int H, int radius, int iterations, uint8_t* inverted, Enq q)
 {
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
     for (int i = 0; i < iterations; ++i) {
-        prof_mark(s, "k_morph"); k_morph<<<g, b, 0, s>>>(data, buf, W, H, radius, 1);
-        prof_mark(s, "k_morph"); k_morph<<<g, b, 0, s>>>(buf, data, W, H, radius, 0);
+        launch(q, "k_morph", k_morph, g, b, 0, data, buf, W, H, radius, 1);
+        launch(q, "k_morph", k_morph, g, b, 0, buf, data, W, H, radius, 0);
     }
-    prof_mark(s, "k_invert"); k_invert<<<(W * H + 255) / 256, 256, 0, s>>>(data, W * H, inverted);
+    launch(q, "k_invert", k_invert, (W * H + 255) / 256, 256, 0, data, W * H, inverted);
 }
 
 }  // namespace mfb
@@ -388,71 +387,71 @@ __global__ void k_proj_resolve(unsigned long long* __restrict__ key, int P, cons
     out[i] = id;
 }
 
-void launch_cc(const uint8_t* img, int W, int H, int* L, int* dense, int* lab, int* area, int* box, uint32_t* counter, cudaStream_t s)
+void launch_cc(const uint8_t* img, int W, int H, int* L, int* dense, int* lab, int* area, int* box, uint32_t* counter, Enq q)
 {
     int P = W * H;
     dim3 gt((W + CC_TW - 1) / CC_TW, (H + CC_TH - 1) / CC_TH);
-    prof_mark(s, "k_cc_tile"); k_cc_tile<<<gt, CC_TW * CC_TH, 0, s>>>(img, W, H, L, area, counter);
+    launch(q, "k_cc_tile", k_cc_tile, gt, CC_TW * CC_TH, 0, img, W, H, L, area, counter);
     const int nEdge = ((W - 1) / CC_TW) * H + ((H - 1) / CC_TH) * W;
-    if (nEdge > 0) { prof_mark(s, "k_cc_border"); k_cc_border<<<(nEdge + 255) / 256, 256, 0, s>>>(img, W, H, L); }
-    prof_mark(s, "k_cc_number"); k_cc_number<<<(P + 255) / 256, 256, 0, s>>>(L, P, dense, counter, box);
-    prof_mark(s, "k_cc_relabel"); k_cc_relabel<<<(P + 255) / 256, 256, 0, s>>>(L, dense, P, W, lab, area, box);
+    if (nEdge > 0) launch(q, "k_cc_border", k_cc_border, (nEdge + 255) / 256, 256, 0, img, W, H, L);
+    launch(q, "k_cc_number", k_cc_number, (P + 255) / 256, 256, 0, L, P, dense, counter, box);
+    launch(q, "k_cc_relabel", k_cc_relabel, (P + 255) / 256, 256, 0, L, dense, P, W, lab, area, box);
 }
-void launch_remove_edges(int* labA, int* labB, const float* depth, const int* area, int W, int H, int iterations, cudaStream_t s)
+void launch_remove_edges(int* labA, int* labB, const float* depth, const int* area, int W, int H, int iterations, Enq q)
 {
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
     for (int i = 0; i < iterations; ++i) {          // caller guarantees an even ping-pong ends in labA when iterations is odd -> see host
-        prof_mark(s, "k_remove_edges"); k_remove_edges<<<g, b, 0, s>>>(i % 2 == 0 ? labA : labB, i % 2 == 0 ? labB : labA, depth, area, W, H);
+        launch(q, "k_remove_edges", k_remove_edges, g, b, 0, i % 2 == 0 ? labA : labB, i % 2 == 0 ? labB : labA, depth, area, W, H);
     }
 }
 void launch_seg_hist(const int* lab, const uint8_t* projID, const uint8_t* mask, int P, const uint8_t* idToIndex, int nModels, const FrameHdr* hdr,
-                     int* compModel, int* compMask, cudaStream_t s)
+                     int* compModel, int* compMask, Enq q)
 {
-    prof_mark(s, "k_seg_hist"); k_seg_hist<<<(P + 255) / 256, 256, 0, s>>>(lab, projID, mask, P, idToIndex, nModels, hdr, compModel, compMask);
+    launch(q, "k_seg_hist", k_seg_hist, (P + 255) / 256, 256, 0, lab, projID, mask, P, idToIndex, nModels, hdr, compModel, compMask);
 }
-void launch_clear_hist(const uint32_t* ccCounter, const FrameHdr* hdr, int nModels, int* compModel, int* compMask, cudaStream_t s)
+void launch_clear_hist(const uint32_t* ccCounter, const FrameHdr* hdr, int nModels, int* compModel, int* compMask, Enq q)
 {
-    prof_mark(s, "k_clear_hist"); k_clear_hist<<<num_sms(), 256, 0, s>>>(ccCounter, hdr, nModels, compModel, compMask);
+    launch(q, "k_clear_hist", k_clear_hist, num_sms(), 256, 0, ccCounter, hdr, nModels, compModel, compMask);
 }
 void launch_component_map(const uint32_t* ccCounter, const int* area, const int* compModel, const int* compMask, int nModels, const FrameHdr* hdr,
-                          const uint8_t* indexToId, int minMapped, int* mapToMask, int* absorb, int* maskPixels, cudaStream_t s)
+                          const uint8_t* indexToId, int minMapped, int* mapToMask, int* absorb, int* maskPixels, Enq q)
 {
-    prof_mark(s, "k_component_map"); k_component_map<<<num_sms(), 128, 0, s>>>(ccCounter, area, compModel, compMask, nModels, hdr, indexToId, minMapped, mapToMask, absorb, maskPixels);
+    launch(q, "k_component_map", k_component_map, num_sms(), 128, 0, ccCounter, area, compModel, compMask, nModels, hdr, indexToId, minMapped, mapToMask, absorb, maskPixels);
 }
 void launch_vote(const FrameHdr* hdr, const VoteParams& vp, const int* maskPixels, const unsigned* maskOverlap, const uint32_t* ccCounter,
-                 uint8_t* maskToID, FrameResult* res, cudaStream_t s)
+                 uint8_t* maskToID, FrameResult* res, Enq q)
 {
-    prof_mark(s, "k_vote"); k_vote<<<1, 32, 0, s>>>(hdr, vp, maskPixels, maskOverlap, ccCounter, maskToID, res);
+    launch(q, "k_vote", k_vote, 1, 32, 0, hdr, vp, maskPixels, maskOverlap, ccCounter, maskToID, res);
 }
-void launch_seg_tables(const SegTables& t, uint8_t* idToIndex, uint8_t* indexToId, uint8_t* isModel, cudaStream_t s)
+void launch_seg_tables(const SegTables& t, uint8_t* idToIndex, uint8_t* indexToId, uint8_t* isModel, Enq q)
 {
-    prof_mark(s, "k_seg_tables"); k_seg_tables<<<1, 256, 0, s>>>(t, idToIndex, indexToId, isModel);
+    launch(q, "k_seg_tables", k_seg_tables, 1, 256, 0, t, idToIndex, indexToId, isModel);
 }
-void launch_frame_header(const FrameHdr& h, FrameHdr* d, cudaStream_t s) { prof_mark(s, "k_frame_header"); k_frame_header<<<1, 256, 0, s>>>(h, d); }
-void launch_person_table(const FrameHdr* hdr, int personClassID, uint8_t* isPerson, cudaStream_t s)
+void launch_frame_header(const FrameHdr& h, FrameHdr* d, Enq q) { launch(q, "k_frame_header", k_frame_header, 1, 256, 0, h, d); }
+void launch_person_table(const FrameHdr* hdr, int personClassID, uint8_t* isPerson, Enq q)
 {
-    prof_mark(s, "k_person_table"); k_person_table<<<1, 256, 0, s>>>(hdr, personClassID, isPerson);
+    launch(q, "k_person_table", k_person_table, 1, 256, 0, hdr, personClassID, isPerson);
 }
-void launch_seg_assign(const int* lab, const int* mapToMask, const uint8_t* ignore, int P, uint8_t* seg, cudaStream_t s)
+void launch_seg_assign(const int* lab, const int* mapToMask, const uint8_t* ignore, int P, uint8_t* seg, Enq q)
 {
-    prof_mark(s, "k_seg_assign"); k_seg_assign<<<(P + 255) / 256, 256, 0, s>>>(lab, mapToMask, ignore, P, seg);
+    launch(q, "k_seg_assign", k_seg_assign, (P + 255) / 256, 256, 0, lab, mapToMask, ignore, P, seg);
 }
-void launch_mask_overlap(const uint8_t* seg, const uint8_t* projID, const uint8_t* idToIndex, const uint8_t* isModelId, int P, unsigned* maskOverlap, cudaStream_t s)
+void launch_mask_overlap(const uint8_t* seg, const uint8_t* projID, const uint8_t* idToIndex, const uint8_t* isModelId, int P, unsigned* maskOverlap, Enq q)
 {
-    prof_mark(s, "k_mask_overlap"); k_mask_overlap<<<(P + 255) / 256, 256, 0, s>>>(seg, projID, idToIndex, isModelId, P, maskOverlap);
+    launch(q, "k_mask_overlap", k_mask_overlap, (P + 255) / 256, 256, 0, seg, projID, idToIndex, isModelId, P, maskOverlap);
 }
 void launch_seg_final(const uint8_t* seg, const int* lab, const int* mapToMask, const int* absorb, const uint8_t* maskToID, const int* box, int P, int W,
-                      uint8_t* out, cudaStream_t s)
+                      uint8_t* out, Enq q)
 {
-    prof_mark(s, "k_seg_final"); k_seg_final<<<(P + 255) / 256, 256, 0, s>>>(seg, lab, mapToMask, absorb, maskToID, box, P, W, out);
+    launch(q, "k_seg_final", k_seg_final, (P + 255) / 256, 256, 0, seg, lab, mapToMask, absorb, maskToID, box, P, W, out);
 }
-void launch_apply_ignore(const uint8_t* mask, const uint8_t* isPerson, const FrameHdr* hdr, int P, uint8_t* ignore, uint8_t* edges, cudaStream_t s)
+void launch_apply_ignore(const uint8_t* mask, const uint8_t* isPerson, const FrameHdr* hdr, int P, uint8_t* ignore, uint8_t* edges, Enq q)
 {
-    prof_mark(s, "k_apply_ignore"); k_apply_ignore<<<(P + 255) / 256, 256, 0, s>>>(mask, isPerson, hdr, P, ignore, edges);
+    launch(q, "k_apply_ignore", k_apply_ignore, (P + 255) / 256, 256, 0, mask, isPerson, hdr, P, ignore, edges);
 }
-void launch_proj_resolve(uint64_t* key, int P, const uint8_t* indexToId, uint8_t* out, cudaStream_t s)
+void launch_proj_resolve(uint64_t* key, int P, const uint8_t* indexToId, uint8_t* out, Enq q)
 {
-    prof_mark(s, "k_proj_resolve"); k_proj_resolve<<<(P + 255) / 256, 256, 0, s>>>((unsigned long long*)key, P, indexToId, out);
+    launch(q, "k_proj_resolve", k_proj_resolve, (P + 255) / 256, 256, 0, (unsigned long long*)key, P, indexToId, out);
 }
 
 }  // namespace mfb

@@ -1097,45 +1097,45 @@ __global__ void k_set_pose(DevPose* d, Pose2 in)
 {
     if (threadIdx.x == 0 && blockIdx.x == 0) derivePose(d, in.p, in.l);
 }
-void launch_set_pose(DevPose* d, const float* pose16, const float* lastPose16, cudaStream_t s)
+void launch_set_pose(DevPose* d, const float* pose16, const float* lastPose16, Enq q)
 {
     Pose2 in;
     for (int k = 0; k < 16; ++k) { in.p[k] = pose16[k]; in.l[k] = lastPose16[k]; }
-    k_set_pose<<<1, 32, 0, s>>>(d, in);
+    launch(q, nullptr, k_set_pose, 1, 32, 0, d, in);
 }
 
-void launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t s) { if (n) k_fill_u32<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p, v, n); }
-void launch_fill_u64(uint64_t* p, uint64_t v, size_t n, cudaStream_t s) { if (n) k_fill_u64<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((unsigned long long*)p, v, n); }
+void launch_fill_u32(uint32_t* p, uint32_t v, size_t n, Enq q) { if (n) launch(q, nullptr, k_fill_u32, (unsigned)((n + 255) / 256), 256, 0, p, v, n); }
+void launch_fill_u64(uint64_t* p, uint64_t v, size_t n, Enq q) { if (n) launch(q, nullptr, k_fill_u64, (unsigned)((n + 255) / 256), 256, 0, (unsigned long long*)p, v, n); }
 
 void launch_predict_indices(const SurfelPlanes& sp, const uint32_t* count, const DevPose* tinv, Cam cam, int W, int H, float maxDepth, int time,
-                            int timeDelta, uint64_t* key, uint32_t* idx, float4* vertConf, float4* colorTime, float4* normRad, float4* cleanTex, float cleanConf, cudaStream_t s)
+                            int timeDelta, uint64_t* key, uint32_t* idx, float4* vertConf, float4* colorTime, float4* normRad, float4* cleanTex, float cleanConf, Enq q)
 {
-    prof_mark(s, "k_index_project"); k_index_project<<<persistentBlocks(8), 256, 0, s>>>(sp.pos, sp.col, count, tinv, cam, W, H, maxDepth, (float)time, (float)timeDelta,
-                                                        (unsigned long long*)key);
+    launch(q, "k_index_project", k_index_project, persistentBlocks(8), 256, 0, sp.pos, sp.col, count, tinv, cam, W, H, maxDepth, (float)time, (float)timeDelta,
+           (unsigned long long*)key);
     int P = W * H;
-    prof_mark(s, "k_index_resolve"); k_index_resolve<<<(P + 255) / 256, 256, 0, s>>>(sp.pos, sp.col, sp.nrm, tinv, P, (unsigned long long*)key, idx, vertConf, colorTime, normRad, cleanTex, cleanConf, (float)time);
+    launch(q, "k_index_resolve", k_index_resolve, (P + 255) / 256, 256, 0, sp.pos, sp.col, sp.nrm, tinv, P, (unsigned long long*)key, idx, vertConf, colorTime, normRad, cleanTex, cleanConf, (float)time);
 }
 
 void launch_associate(const uchar4* rgb, const float* depthRaw, const float* depthFilt, const uint8_t* mask, const uint32_t* idx,
                       const float4* vertConf, const float4* normRad, const DevPose* pose, Cam cam, int W, int H, float maxDepth, int time,
-                      float weighting, uint8_t maskID, uint8_t* flag, uint32_t* best, float4* const* meas, uint32_t* slot, cudaStream_t s)
+                      float weighting, uint8_t maskID, uint8_t* flag, uint32_t* best, float4* const* meas, uint32_t* slot, Enq q)
 {
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
-    prof_mark(s, "k_associate"); k_associate<<<g, b, 0, s>>>(rgb, depthRaw, depthFilt, mask, idx, vertConf, normRad, pose, cam, W, H, maxDepth, time, weighting, maskID,
-                                flag, best, meas[0], meas[1], meas[2], slot);
+    launch(q, "k_associate", k_associate, g, b, 0, rgb, depthRaw, depthFilt, mask, idx, vertConf, normRad, pose, cam, W, H, maxDepth, time, weighting, maskID,
+           flag, best, meas[0], meas[1], meas[2], slot);
 }
 
 void launch_fuse_update(const uint8_t* flag, const uint32_t* best, float4* const* meas, uint32_t* slot, int P, int time,
-                        const SurfelPlanes& sp, cudaStream_t s)
+                        const SurfelPlanes& sp, Enq q)
 {
-    prof_mark(s, "k_fuse_update"); k_fuse_update<<<(P + 255) / 256, 256, 0, s>>>(flag, best, meas[0], meas[1], meas[2], slot, P, time, sp.pos, sp.col, sp.nrm);
-    prof_mark(s, "k_slot_release"); k_slot_release<<<(P + 255) / 256, 256, 0, s>>>(flag, best, P, slot);
+    launch(q, "k_fuse_update", k_fuse_update, (P + 255) / 256, 256, 0, flag, best, meas[0], meas[1], meas[2], slot, P, time, sp.pos, sp.col, sp.nrm);
+    launch(q, "k_slot_release", k_slot_release, (P + 255) / 256, 256, 0, flag, best, P, slot);
 }
 
 void launch_clean(const SurfelPlanes& src, const SurfelPlanes& dst, const uint32_t* count, uint32_t* newCount, uint32_t capacity,
                   const uint8_t* aflag, float4* const* meas, const DevPose* tinv, Cam cam, int W, int H, int time, int timeDelta, float confThreshold,
                   float outlierCoeff, uint8_t maskID, const CleanWindowImages& win,
-                  const float* depthFilt, const uint8_t* mask, uint8_t* keep, uint32_t* blockSums, uint32_t* cand, uint32_t* candCount, cudaStream_t s,
+                  const float* depthFilt, const uint8_t* mask, uint8_t* keep, uint32_t* blockSums, uint32_t* cand, uint32_t* candCount, Enq q,
                   const CleanInPlace& inplace, const IndexFused* fused)
 {
     const CleanTexels texels{win.packed, win.vertConf, win.colorTime, win.idx};
@@ -1145,30 +1145,29 @@ void launch_clean(const SurfelPlanes& src, const SurfelPlanes& dst, const uint32
     P.outlierCoeff = outlierCoeff; P.maskID = maskID;
     int Ppix = W * H;
     int blocks = persistentBlocks(4);
-    prof_mark(s, "k_clean_p1"); k_clean_p1<<<persistentBlocks(8), 256, 0, s>>>(src.pos, src.col, count, aflag, meas[0], meas[1], Ppix, P, tinv, depthFilt, mask, keep, cand, candCount,
-                                                                               fused ? (unsigned long long*)fused->key : nullptr, fused ? fused->maxDepth : 0.f);
+    launch(q, "k_clean_p1", k_clean_p1, persistentBlocks(8), 256, 0, src.pos, src.col, count, aflag, meas[0], meas[1], Ppix, P, tinv, depthFilt, mask, keep, cand, candCount,
+           fused ? (unsigned long long*)fused->key : nullptr, fused ? fused->maxDepth : 0.f);
     if (fused) {           // Model::predictIndices, second half: the index map of the store as clean sees it
-        prof_mark(s, "k_index_resolve"); k_index_resolve<<<(Ppix + 255) / 256, 256, 0, s>>>(src.pos, src.col, src.nrm, tinv, Ppix, (unsigned long long*)fused->key, fused->idx, fused->vertConf,
-                                                                                          fused->colorTime, fused->normRad, fused->cleanTex, confThreshold, (float)time);
+        launch(q, "k_index_resolve", k_index_resolve, (Ppix + 255) / 256, 256, 0, src.pos, src.col, src.nrm, tinv, Ppix, (unsigned long long*)fused->key, fused->idx,
+               fused->vertConf, fused->colorTime, fused->normRad, fused->cleanTex, confThreshold, (float)time);
     }
-    prof_mark(s, "k_clean_p2");
-    if (texels.packed) k_clean_p2<true><<<persistentBlocks(8), 256, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], P, tinv, texels, depthFilt, mask, keep, cand, candCount);
-    else k_clean_p2<false><<<persistentBlocks(8), 256, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], P, tinv, texels, depthFilt, mask, keep, cand, candCount);
-    prof_mark(s, "k_keep_block_sums"); k_keep_block_sums<<<persistentBlocks(8), 256, 0, s>>>(keep, count, Ppix, blockSums, candCount, inplace.ticket);
-    prof_mark(s, "k_scan_block_sums"); k_scan_block_sums<<<1, 1024, 0, s>>>(blockSums, count, Ppix, capacity, newCount, inplace.firstMoved);
+    launch(q, "k_clean_p2", texels.packed ? k_clean_p2<true> : k_clean_p2<false>, persistentBlocks(8), 256, 0, src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2],
+           P, tinv, texels, depthFilt, mask, keep, cand, candCount);
+    launch(q, "k_keep_block_sums", k_keep_block_sums, persistentBlocks(8), 256, 0, keep, count, Ppix, blockSums, candCount, inplace.ticket);
+    launch(q, "k_scan_block_sums", k_scan_block_sums, 1, 1024, 0, blockSums, count, Ppix, capacity, newCount, inplace.firstMoved);
     if (!inplace.pingPong) {
-        prof_mark(s, "k_clean_compact"); k_clean_compact<<<blocks, SCAN_BLOCK, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
-                                                      inplace.ticket, inplace.loaded, inplace.firstMoved, inplace.epoch);
+        launch(q, "k_clean_compact", k_clean_compact, blocks, SCAN_BLOCK, 0, src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
+               inplace.ticket, inplace.loaded, inplace.firstMoved, inplace.epoch);
     } else {
-        prof_mark(s, "k_clean_scatter"); k_clean_scatter<<<blocks, SCAN_BLOCK, 0, s>>>(src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
-                                                      dst.pos, dst.col, dst.nrm);
+        launch(q, "k_clean_scatter", k_clean_scatter, blocks, SCAN_BLOCK, 0, src.pos, src.col, src.nrm, count, meas[0], meas[1], meas[2], Ppix, keep, blockSums, capacity,
+               dst.pos, dst.col, dst.nrm);
     }
 }
 
-void launch_ray_table(Cam cam, int W, int H, float4* tab, cudaStream_t s)
+void launch_ray_table(Cam cam, int W, int H, float4* tab, Enq q)
 {
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
-    k_ray_table<<<g, b, 0, s>>>(cam, W, H, tab);
+    launch(q, nullptr, k_ray_table, g, b, 0, cam, W, H, tab);
 }
 
 // grid of the splat rasteriser: for large stores a persistent grid of as many blocks as the SMs hold at once; for a small store (an object
@@ -1191,41 +1190,40 @@ static dim3 splatGrid(uint32_t capacity, int W, int H)
 void launch_combined_predict(const SurfelPlanes& sp, const uint32_t* count, const DevPose* tinv, Cam cam, int W, int H, float maxDepth,
                              float confThreshold, int time, int maxTime, int timeDelta, const float4* rayTab, uint64_t* key, uchar4* image, float4* vertexConf,
                              float4* normalRad, uint16_t* timeTex, int doFill, const float* depthFilt, const uchar4* rgb, int ptVN, int ptImg,
-                             uchar4* fillImage, float4* fillVertex, float4* fillNormal, uint32_t* nonBlackSamples, cudaStream_t s, uint32_t capacity)
+                             uchar4* fillImage, float4* fillVertex, float4* fillNormal, uint32_t* nonBlackSamples, Enq q, uint32_t capacity)
 {
-    prof_mark(s, "k_splat_project"); k_splat_project<<<splatGrid(capacity, W, H), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
-                                                        (float)maxTime, (float)timeDelta, 0u, rayTab, (unsigned long long*)key);
-    if (nonBlackSamples) cudaMemsetAsync(nonBlackSamples, 0, sizeof(uint32_t), s);
+    launch(q, "k_splat_project", k_splat_project, splatGrid(capacity, W, H), SPLAT_BS, 0, sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
+           (float)maxTime, (float)timeDelta, 0u, rayTab, (unsigned long long*)key);
+    if (nonBlackSamples) cudaMemsetAsync(nonBlackSamples, 0, sizeof(uint32_t), q.s);
     dim3 b(32, 8), g((W + 31) / 32, (H + 7) / 8);
-    prof_mark(s, "k_splat_resolve"); k_splat_resolve<<<g, b, 0, s>>>(sp.pos, sp.col, sp.nrm, tinv, cam, W, H, maxDepth, confThreshold, (float)time, (float)maxTime,
-                                    (float)timeDelta, rayTab, (unsigned long long*)key, image, vertexConf, normalRad, timeTex, doFill, depthFilt, rgb,
-                                    ptVN, ptImg, fillImage, fillVertex, fillNormal, nonBlackSamples);
+    launch(q, "k_splat_resolve", k_splat_resolve, g, b, 0, sp.pos, sp.col, sp.nrm, tinv, cam, W, H, maxDepth, confThreshold, (float)time, (float)maxTime,
+           (float)timeDelta, rayTab, (unsigned long long*)key, image, vertexConf, normalRad, timeTex, doFill, depthFilt, rgb,
+           ptVN, ptImg, fillImage, fillVertex, fillNormal, nonBlackSamples);
 }
 
 void launch_init_model(const uchar4* rgb, const float* depthRaw, const float* depthFilt, Cam cam, int W, int H, int time, float maxDepth,
                        uint8_t* fr, uint8_t* ff, uint32_t* sumR, uint32_t* sumF, uint32_t capacity, const SurfelPlanes& sp, uint32_t* count,
-                       cudaStream_t s)
+                       Enq q)
 {
     int P = W * H, nb = (P + SCAN_BLOCK - 1) / SCAN_BLOCK;
-    prof_mark(s, "k_zero_f4"); k_zero_f4<<<(P + 255) / 256, 256, 0, s>>>(sp.nrm, 0, (uint32_t)(P < (int)capacity ? P : (int)capacity));
-    prof_mark(s, "k_init_flags"); k_init_flags<<<nb, SCAN_BLOCK, 0, s>>>(depthRaw, depthFilt, W, H, maxDepth, fr, ff, sumR, sumF);
-    prof_mark(s, "k_scan_small"); k_scan_small<<<1, 1024, 0, s>>>(sumR, nb, capacity, count);
-    prof_mark(s, "k_scan_small"); k_scan_small<<<1, 1024, 0, s>>>(sumF, nb, capacity, nullptr);
-    prof_mark(s, "k_init_scatter"); k_init_scatter<<<nb, SCAN_BLOCK, 0, s>>>(rgb, depthRaw, depthFilt, cam, W, H, time, fr, ff, sumR, sumF, capacity, sp.pos, sp.col, sp.nrm);
+    launch(q, "k_zero_f4", k_zero_f4, (P + 255) / 256, 256, 0, sp.nrm, 0, (uint32_t)(P < (int)capacity ? P : (int)capacity));
+    launch(q, "k_init_flags", k_init_flags, nb, SCAN_BLOCK, 0, depthRaw, depthFilt, W, H, maxDepth, fr, ff, sumR, sumF);
+    launch(q, "k_scan_small", k_scan_small, 1, 1024, 0, sumR, nb, capacity, count);
+    launch(q, "k_scan_small", k_scan_small, 1, 1024, 0, sumF, nb, capacity, nullptr);
+    launch(q, "k_init_scatter", k_init_scatter, nb, SCAN_BLOCK, 0, rgb, depthRaw, depthFilt, cam, W, H, time, fr, ff, sumR, sumF, capacity, sp.pos, sp.col, sp.nrm);
 }
 
-void launch_planes_to_aos(const SurfelPlanes& sp, uint32_t n, float4* out, cudaStream_t s) { if (n) k_planes_to_aos<<<(n + 255) / 256, 256, 0, s>>>(sp.pos, sp.col, sp.nrm, n, out); }
-void launch_aos_to_planes(const float4* in, uint32_t n, const SurfelPlanes& sp, cudaStream_t s) { if (n) k_aos_to_planes<<<(n + 255) / 256, 256, 0, s>>>(in, n, sp.pos, sp.col, sp.nrm); }
+void launch_planes_to_aos(const SurfelPlanes& sp, uint32_t n, float4* out, Enq q) { if (n) launch(q, nullptr, k_planes_to_aos, (n + 255) / 256, 256, 0, sp.pos, sp.col, sp.nrm, n, out); }
+void launch_aos_to_planes(const float4* in, uint32_t n, const SurfelPlanes& sp, Enq q) { if (n) launch(q, nullptr, k_aos_to_planes, (n + 255) / 256, 256, 0, in, n, sp.pos, sp.col, sp.nrm); }
 
 }  // namespace mfb
 
 namespace mfb {
 // splat projection into a caller-owned key image (GlobalProjection: all models share one key image)
 void launch_splat_project_only(const SurfelPlanes& sp, const uint32_t* count, const DevPose* tinv, Cam cam, int W, int H, float maxDepth, float confThreshold,
-                               int time, int maxTime, int timeDelta, uint32_t drawBase, const float4* rayTab, uint64_t* key, cudaStream_t s, uint32_t capacity)
+                               int time, int maxTime, int timeDelta, uint32_t drawBase, const float4* rayTab, uint64_t* key, Enq q, uint32_t capacity)
 {
-    prof_mark(s, "k_splat_project_ids");
-    k_splat_project<<<splatGrid(capacity, W, H), SPLAT_BS, 0, s>>>(sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold, (float)time,
-                                                        (float)maxTime, (float)timeDelta, drawBase, rayTab, (unsigned long long*)key);
+    launch(q, "k_splat_project_ids", k_splat_project, splatGrid(capacity, W, H), SPLAT_BS, 0, sp.pos, sp.col, sp.nrm, count, tinv, cam, W, H, maxDepth, confThreshold,
+           (float)time, (float)maxTime, (float)timeDelta, drawBase, rayTab, (unsigned long long*)key);
 }
 }  // namespace mfb

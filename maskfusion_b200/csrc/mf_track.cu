@@ -1235,8 +1235,8 @@ void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* 
     for (int j = 0; j < nJobs; ++j) G[j] = ((lightMask >> j) & 1u) ? Glight : Gheavy;
 }
 
-int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
-                    bool pyramid, bool fastOdom, bool so3, int numSMs, cudaStream_t s, unsigned lightMask)
+void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
+                     bool pyramid, bool fastOdom, bool so3, int numSMs, Enq q, unsigned lightMask)
 {
     const bool anyValidBits = lightMask != 0;          // bit j: job j is an object model with a validity bitmask (nearly all of its pixels are rejected early)
     // per-device launch limits (several contexts on different GPUs may live in one process): occupancy and the opt-in
@@ -1299,11 +1299,11 @@ int launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgb
     if (cacheOn < 0) { const char* e = getenv("MFB200_TRACK_CACHE"); cacheOn = e ? (e[0] != '0') : MFB200_DEFAULT_TRACK_CACHE; }
     tp.cacheRounds = cacheOn ? (int)std::min<size_t>((size_t)rounds0, (dynMaxDev[dev] - dyn - (tp.bitWords ? bitBytes : 0)) / ((size_t)PT_THREADS * CACHE_BYTES_PER_SLOT)) : 0;
     dyn += (size_t)tp.cacheRounds * PT_THREADS * CACHE_BYTES_PER_SLOT + (tp.bitWords ? bitBytes : 0);
-    prof_mark(s, "k_track_persistent");
+    q.mark("k_track_persistent");
     const TrackJob* jp = d_jobs;
     void* args[] = {(void*)&jp, (void*)&tp};
-    cudaCheck(cudaLaunchCooperativeKernel((const void*)k_track_persistent, dim3(gridCTAs), dim3(PT_THREADS), args, dyn, s), "cooperative launch (tracking)");
-    return 1;
+    cudaLaunchCooperativeKernel((const void*)k_track_persistent, dim3(gridCTAs), dim3(PT_THREADS), args, dyn, q.s);    // a failure is the runtime's last error
+    q.launched((const void*)k_track_persistent);
 }
 
 // (tag, clock64) pairs of the last tracking launch (A/B build -DMF_TRACK_TIMING only); returns the number of int64 values written
@@ -1323,10 +1323,11 @@ int debug_track_timing(long long* out, int cap)
 }
 
 void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
-                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, int numSMs, cudaStream_t s)
+                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, int numSMs, Enq q)
 {
     const float angleThres = (float)sin(20.f * 3.14159254f / 180.f);
-    prof_mark(s, "k_icp_only"); k_icp_only<<<trackBlocks(W * H, numSMs), TRK_THREADS, 0, s>>>(vmapC, nmapC, vmapG, nmapG, W, H, cam, pp, 0.10f, angleThres, reinterpret_cast<double*>(partial), ticket, out29);
+    launch(q, "k_icp_only", k_icp_only, trackBlocks(W * H, numSMs), TRK_THREADS, 0, vmapC, nmapC, vmapG, nmapG, W, H, cam, pp, 0.10f, angleThres,
+           reinterpret_cast<double*>(partial), ticket, out29);
 }
 
 }  // namespace mfb
