@@ -235,7 +235,9 @@ int mf_debug_set_poses(mf_context* ctx, int i, const float pose16[16], const flo
 int mf_icp_step(mf_context* ctx, int i, int level, const float Rcurr9[9], const float tcurr3[3], float out29[29]);  /* icpStep, reduce.cu:446-525 */
 
 /* ---- Mask R-CNN backbone: ResNet-101 + FPN as wgmma GEMMs (replaces the dense part of the Keras/TF sidecar,
- *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded unless loaded with mf_*_load_weights) ---- */
+ *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded unless loaded with mf_*_load_weights).
+ *      The Mask R-CNN functions (mf_backbone_*, mf_rpn_*, mf_detector_*, mf_roi_align_bf16) report a refusal or a CUDA failure by returning
+ *      -1, a creator by returning NULL, and mf_gemm_bf16 and mf_conv3x3_bf16 by returning -2; mf_last_error() has the text. ---- */
 typedef struct mf_backbone mf_backbone;
 const char* mf_cnn_last_error(void);      /* the same text as mf_last_error(), under the name kept for existing bindings */
 /* Pretrained weights (the reference's model.load_weights(COCO_MODEL_PATH, by_name=True)): a safetensors file of matterport's Keras

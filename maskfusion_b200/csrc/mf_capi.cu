@@ -361,7 +361,7 @@ extern "C" int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int i
 extern "C" int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k)
 {
     MF_TRY MF_NEED(ctx)
-    ctx->mf->attachBackbone(backbone, every_k); return 0;
+    ctx->mf->attachBackbone((mf_backbone*)backbone, every_k); return 0;
     MF_CATCH(-1)
 }
 

@@ -28,6 +28,8 @@
 #include <stdlib.h>
 #include <string.h>
 #include <map>
+#include <mutex>
+#include <set>
 #include <array>
 #include <type_traits>
 
@@ -324,129 +326,102 @@ __global__ void k_mold_input(const uchar4* __restrict__ rgb, int W, int H, int S
 // ------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_encodeTiled g_encode = nullptr;
 
-static bool ensure_encode()
+// The GEMM launcher's process-wide state, behind one lock (handles may run on several threads and devices): the driver's
+// cuTensorMapEncodeTiled, looked up once; the tensor maps, which are pure functions of (pointer, geometry) -- the backbone's buffers never
+// move, so every map is encoded once (first forward) and reused by all later launches; and, per kernel instantiation, the devices on which
+// its dynamic shared-memory attribute is set (the attribute belongs to a (function, device) pair).
+static std::mutex g_gemmLock;
+static PFN_encodeTiled g_encode = nullptr;
+static std::map<std::array<uint64_t, 6>, CUtensorMap> g_mapCache;
+
+static PFN_encodeTiled encode_fn()
 {
-    if (g_encode) return true;
+    if (g_encode) return g_encode;
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) { mf_set_error("cuTensorMapEncodeTiled not available"); return false; }
-    g_encode = (PFN_encodeTiled)fn;
-    return true;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) throw CudaError{"cuTensorMapEncodeTiled not available"};
+    return g_encode = (PFN_encodeTiled)fn;
 }
-// 2-D row-major [rows x K] bf16, box = {64, boxRows}, SWIZZLE_128B
-static bool make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t K, uint32_t boxRows)
+// rank 2: row-major [rows x K] bf16, dims {K, rows}, box {64, boxRows}; rank 3: an NHWC activation, dims {C, W, H}, box {64, Wbox, Hbox}.
+// SWIZZLE_128B.  Encoded on first use, then from the cache; under g_gemmLock
+static CUtensorMap cached_map(const void* ptr, int rank, const cuuint64_t* dims, const cuuint32_t* box)
 {
-    cuuint64_t dims[2] = {K, rows};
-    cuuint64_t strides[1] = {K * 2};
-    cuuint32_t box[2] = {64, boxRows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { mf_set_error("cuTensorMapEncodeTiled failed: " + std::to_string((int)r)); return false; }
-    return true;
-}
-
-// 3-D map over an NHWC activation (C, W, H), box = {64, Wbox, Hbox}, SWIZZLE_128B
-static bool make_map_nhwc(CUtensorMap* m, const void* ptr, int C, int W, int H, int Wbox, int Hbox)
-{
-    cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
-    cuuint64_t strides[2] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)Wbox, (cuuint32_t)Hbox};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { mf_set_error("cuTensorMapEncodeTiled (3-D) failed: " + std::to_string((int)r)); return false; }
-    return true;
-}
-
-// Tensor maps are pure functions of (pointer, geometry): the backbone's buffers never move, so every map is encoded ONCE (first forward) and
-// reused by all later launches (round 1 encoded two maps per GEMM per forward on the host: 224 driver calls in front of 112 launches).
-static std::map<std::array<uint64_t, 6>, CUtensorMap> g_mapCache;
-static bool cached_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t K, uint32_t boxRows)
-{
-    const std::array<uint64_t, 6> key = {(uint64_t)(uintptr_t)ptr, rows, K, boxRows, 0, 0};
+    const bool r3 = rank == 3;
+    const std::array<uint64_t, 6> key = {(uint64_t)(uintptr_t)ptr, dims[0], dims[1], r3 ? dims[2] : 0, box[1], r3 ? box[2] : 0};
     auto it = g_mapCache.find(key);
-    if (it != g_mapCache.end()) { *m = it->second; return true; }
-    if (!make_map(m, ptr, rows, K, boxRows)) return false;
-    if (g_mapCache.size() < 4096) g_mapCache[key] = *m;
-    return true;
-}
-static bool cached_map_nhwc(CUtensorMap* m, const void* ptr, int Cin, int Wimg, int Himg, int Wbox, int Hbox)
-{
-    const std::array<uint64_t, 6> key = {(uint64_t)(uintptr_t)ptr, (uint64_t)Cin, (uint64_t)Wimg, (uint64_t)Himg, (uint64_t)Wbox, (uint64_t)Hbox + 1};
-    auto it = g_mapCache.find(key);
-    if (it != g_mapCache.end()) { *m = it->second; return true; }
-    if (!make_map_nhwc(m, ptr, Cin, Wimg, Himg, Wbox, Hbox)) return false;
-    if (g_mapCache.size() < 4096) g_mapCache[key] = *m;
-    return true;
+    if (it != g_mapCache.end()) return it->second;
+    const cuuint64_t strides[2] = {dims[0] * 2, dims[0] * dims[1] * 2};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    CUtensorMap m;
+    CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) throw CudaError{std::string(r3 ? "cuTensorMapEncodeTiled (3-D) failed: " : "cuTensorMapEncodeTiled failed: ") + std::to_string((int)r)};
+    if (g_mapCache.size() < 4096) g_mapCache[key] = m;
+    return m;
 }
 
 template <int BN>
 static size_t gemm_smem_bytes() { return (size_t)GEMM_STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 2 * GEMM_STAGES * 8 + 1024; }
 
-int cnn_fail(const std::string& msg) { mf_set_error(msg); return -1; }
-
-int cnn_check_launch(const char* what)
+void cnn_read_back(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows, size_t pitch)
 {
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cnn_fail(std::string(what) + ": " + cudaGetErrorString(e));
-}
-
-int cnn_download(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows, size_t pitch)
-{
-    if (!dst) return 0;
+    if (!dst) return;
     cudaError_t e = cudaStreamSynchronize(s);
     if (e == cudaSuccess)
         e = rows == 1 ? cudaMemcpy(dst, src, width, cudaMemcpyDeviceToHost) : cudaMemcpy2D(dst, width, src, pitch, width, rows, cudaMemcpyDeviceToHost);
-    return e == cudaSuccess ? 0 : cnn_fail(std::string("download: ") + cudaGetErrorString(e));
+    cudaCheck(e, "download");
 }
 
 template <int BN, typename OutT>
-static void launch_wgmma(dim3 grid, cudaStream_t s, const CUtensorMap& mA, const CUtensorMap& mB, const float* bias, const void* residual, void* out,
-                         int M, int N, int K, int relu, const ConvGeom& geo)
+static void launch_wgmma(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu,
+                         cudaStream_t s, const ConvGeom& geo, int Cin)
 {
-    static bool attr = false;
-    if (!attr) { cudaFuncSetAttribute(k_gemm_bf16_wgmma<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<BN>()); attr = true; }
-    k_gemm_bf16_wgmma<BN, OutT><<<grid, GEMM_THREADS, gemm_smem_bytes<BN>(), s>>>(mA, mB, bias, (const __nv_bfloat16*)residual, (OutT*)out, M, N, K, relu, geo);
+    static std::set<int> attrSet;                             // devices with this instantiation's attribute set (under g_gemmLock)
+    int dev = 0;
+    cudaCheck(cudaGetDevice(&dev), "cudaGetDevice");
+    const cuuint64_t dimsA[3] = {(cuuint64_t)(geo.mode ? Cin : K), (cuuint64_t)(geo.mode ? geo.Wimg : M), (cuuint64_t)geo.Himg}, dimsB[2] = {(cuuint64_t)K, (cuuint64_t)N};
+    const cuuint32_t boxA[3] = {64, (cuuint32_t)(geo.mode ? geo.Wbox : GEMM_BM), (cuuint32_t)geo.Hbox}, boxB[2] = {64, BN};
+    CUtensorMap mA, mB;
+    {
+        std::lock_guard<std::mutex> lock(g_gemmLock);
+        if (!attrSet.count(dev)) {
+            cudaCheck(cudaFuncSetAttribute(k_gemm_bf16_wgmma<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<BN>()),
+                      "cudaFuncSetAttribute");
+            attrSet.insert(dev);
+        }
+        mA = cached_map(A, geo.mode ? 3 : 2, dimsA, boxA);
+        mB = cached_map(B, 2, dimsB, boxB);
+    }
+    launch(Enq{s, nullptr}, nullptr, k_gemm_bf16_wgmma<BN, OutT>, dim3((M + GEMM_BM - 1) / GEMM_BM, N / BN), dim3(GEMM_THREADS), gemm_smem_bytes<BN>(),
+           mA, mB, bias, (const __nv_bfloat16*)residual, (OutT*)out, M, N, K, relu, geo);
 }
 
 // D = relu?(A * B^T + bias + residual); all device pointers; K % 64 == 0, N % 64 == 0
 // conv3x3 != nullptr: A is an NHWC activation [Himg x Wimg x Cin] and the GEMM is the implicit 3x3/s1/p1 convolution (K = 9*Cin)
 // outF32: D is written as fp32 (residual must then be null), else as bf16
-int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
-                     const int* conv3x3 /* Wimg, Himg, Cin */, bool outF32)
+void launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
+                      const int* conv3x3 /* Wimg, Himg, Cin */, bool outF32)
 {
     // every refusal comes before the first driver call
-    if (outF32 && residual) { mf_set_error("gemm: the fp32 output takes no residual"); return -2; }
+    if (outF32 && residual) throw CudaError{"gemm: the fp32 output takes no residual"};
     ConvGeom geo; memset(&geo, 0, sizeof geo);
     if (conv3x3) {
         const int Wimg = conv3x3[0], Himg = conv3x3[1], Cin = conv3x3[2];
-        if (!cnn_conv_implicit(3, 1, 1, Cin, Himg, Wimg) || K != 9 * Cin || M != Wimg * Himg) { mf_set_error("conv3x3: unsupported geometry"); return -2; }
+        if (!cnn_conv_implicit(3, 1, 1, Cin, Himg, Wimg) || K != 9 * Cin || M != Wimg * Himg) throw CudaError{"conv3x3: unsupported geometry"};
         geo.mode = 1; geo.Wimg = Wimg; geo.Himg = Himg; geo.Wbox = Wimg >= 128 ? 128 : Wimg; geo.Hbox = 128 / geo.Wbox; geo.cblocks = Cin / 64;
     }
-    if (K <= 0 || N <= 0 || M <= 0 || K % 64 || N % 64) { mf_set_error("gemm: need M > 0, and K > 0 and N > 0 multiples of 64"); return -2; }
-    if (!ensure_encode()) return -1;
-    const int mtiles = (M + GEMM_BM - 1) / GEMM_BM;
+    if (K <= 0 || N <= 0 || M <= 0 || K % 64 || N % 64) throw CudaError{"gemm: need M > 0, and K > 0 and N > 0 multiples of 64"};
+    const int mtiles = (M + GEMM_BM - 1) / GEMM_BM, Cin = conv3x3 ? conv3x3[2] : 0;
     // fill the machine: with few M tiles prefer the narrow N tile (twice the CTAs)
-    const int BN = (N % 128 == 0 && mtiles * (N / 128) >= num_sms()) ? 128 : 64;
-    CUtensorMap mA, mB;
-    if (conv3x3) {
-        if (!cached_map_nhwc(&mA, A, conv3x3[2], geo.Wimg, geo.Himg, geo.Wbox, geo.Hbox)) return -3;
-    } else if (!cached_map(&mA, A, (uint64_t)M, (uint64_t)K, GEMM_BM)) return -3;
-    if (!cached_map(&mB, B, (uint64_t)N, (uint64_t)K, (uint32_t)BN)) return -3;
-    dim3 grid(mtiles, N / BN);
+    const bool wide = N % 128 == 0 && mtiles * (N / 128) >= num_sms();
     if (outF32) {
-        if (BN == 128) launch_wgmma<128, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
-        else launch_wgmma<64, float>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
+        if (wide) launch_wgmma<128, float>(A, B, bias, residual, out, M, N, K, relu, s, geo, Cin);
+        else launch_wgmma<64, float>(A, B, bias, residual, out, M, N, K, relu, s, geo, Cin);
     } else {
-        if (BN == 128) launch_wgmma<128, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
-        else launch_wgmma<64, __nv_bfloat16>(grid, s, mA, mB, bias, residual, out, M, N, K, relu, geo);
+        if (wide) launch_wgmma<128, __nv_bfloat16>(A, B, bias, residual, out, M, N, K, relu, s, geo, Cin);
+        else launch_wgmma<64, __nv_bfloat16>(A, B, bias, residual, out, M, N, K, relu, s, geo, Cin);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { mf_set_error(std::string("gemm launch: ") + cudaGetErrorString(e)); return -4; }
-    return 0;
 }
 
 // ---- backbone ---------------------------------------------------------------------------
@@ -475,8 +450,8 @@ bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win)
 }
 
 // runs convolution L (weights W [rows x K], bias B) on in[Hin x Win x cin] -> out[Hout x Wout x rows]; col: im2col scratch
-static int conv_layer(const LayerGeom& L, const __nv_bfloat16* W, const float* B, __nv_bfloat16* col, const __nv_bfloat16* in, int Hin, int Win,
-                      __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s, int* HoutP, int* WoutP)
+static void conv_layer(const LayerGeom& L, const __nv_bfloat16* W, const float* B, __nv_bfloat16* col, const __nv_bfloat16* in, int Hin, int Win,
+                       __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s, int* HoutP, int* WoutP)
 {
     const int Hout = (Hin + 2 * L.pad - L.k) / L.stride + 1, Wout = (Win + 2 * L.pad - L.k) / L.stride + 1;
     const int M = Hout * Wout;
@@ -485,36 +460,36 @@ static int conv_layer(const LayerGeom& L, const __nv_bfloat16* W, const float* B
     if (WoutP) *WoutP = Wout;
     if (cnn_conv_implicit(L.k, L.stride, L.pad, L.cin, Hin, Win)) {
         int g3[3] = {Win, Hin, L.cin};
-        return launch_gemm_bf16(in, W, B, residual, out, M, L.rows, L.K, relu, s, g3);
+        launch_gemm_bf16(in, W, B, residual, out, M, L.rows, L.K, relu, s, g3);
+        return;
     }
     if (!(L.k == 1 && L.stride == 1)) {
-        if (L.k == 1 && L.stride == 2 && (L.cin % 8) == 0) {
-            k_subsample2<<<4 * num_sms(), 256, 0, s>>>(in, Hin, Win, L.cin, col);
-        } else {
-            k_im2col<<<8 * num_sms(), 256, 0, s>>>(in, 1, Hin, Win, L.cin, Hout, Wout, L.k, L.k, L.stride, L.pad, L.K, col);
-        }
+        if (L.k == 1 && L.stride == 2 && (L.cin % 8) == 0)
+            launch(Enq{s, nullptr}, nullptr, k_subsample2, 4 * num_sms(), 256, 0, in, Hin, Win, L.cin, col);
+        else
+            launch_im2col(in, 1, Hin, Win, L.cin, Hout, Wout, L.k, L.stride, L.pad, L.K, col, s);
         A = col;
     }
-    return launch_gemm_bf16(A, W, B, residual, out, M, L.rows, L.K, relu, s);
+    launch_gemm_bf16(A, W, B, residual, out, M, L.rows, L.K, relu, s);
 }
 
 // runs backbone layer li on in[Hin x Win x Cin] -> out[Hout x Wout x Cout]
-static int run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int Win, __nv_bfloat16* out, const __nv_bfloat16* residual, int relu, cudaStream_t s,
-                    int* HoutP = nullptr, int* WoutP = nullptr)
+static void run_conv(Backbone* b, int li, const __nv_bfloat16* in, int Hin, int Win, __nv_bfloat16* out, const __nv_bfloat16* residual, int relu,
+                     cudaStream_t s, int* HoutP = nullptr, int* WoutP = nullptr)
 {
     const LayerGeom& L = b->layers[li];
     int Hout, Wout;
-    const int rc = conv_layer(L, b->w.w(li), b->w.b(li), b->col, in, Hin, Win, out, residual, relu, s, &Hout, &Wout);
+    conv_layer(L, b->w.w(li), b->w.b(li), b->col, in, Hin, Win, out, residual, relu, s, &Hout, &Wout);
     b->flops += 2.0 * Hout * Wout * (double)L.rows * (double)(L.k * L.k * L.cin);
     b->gemms++;
     if (HoutP) *HoutP = Hout;
     if (WoutP) *WoutP = Wout;
-    return rc;
 }
 
 void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int k, int stride, int pad, int Kpad, void* col, cudaStream_t s)
 {
-    k_im2col<<<8 * num_sms(), 256, 0, s>>>((const __nv_bfloat16*)in, nimg, Hin, Win, Cin, Hout, Wout, k, k, stride, pad, Kpad, (__nv_bfloat16*)col);
+    launch(Enq{s, nullptr}, nullptr, k_im2col, 8 * num_sms(), 256, 0, (const __nv_bfloat16*)in, nimg, Hin, Win, Cin, Hout, Wout, k, k, stride, pad, Kpad,
+           (__nv_bfloat16*)col);
 }
 
 // mould_image's letter box as mf_backbone_mold applies it (the detection heads map boxes back through the same geometry)
@@ -528,12 +503,12 @@ MoldGeom cnn_mold_geometry(int S, int W, int H)
 }
 
 // a convolution whose weights are not in the backbone's table (the RPN's shared 3x3): the same path as the backbone's layers
-int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
-             cudaStream_t s)
+void cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
+              cudaStream_t s)
 {
     const LayerGeom L = {Cin, Cout, k, stride, pad, (k * k * Cin + 63) / 64 * 64};
-    return conv_layer(L, (const __nv_bfloat16*)W, B, (__nv_bfloat16*)col, (const __nv_bfloat16*)in, Hin, Win, (__nv_bfloat16*)out, nullptr, relu, s,
-                      nullptr, nullptr);
+    conv_layer(L, (const __nv_bfloat16*)W, B, (__nv_bfloat16*)col, (const __nv_bfloat16*)in, Hin, Win, (__nv_bfloat16*)out, nullptr, relu, s, nullptr,
+               nullptr);
 }
 
 }  // namespace mfb
@@ -541,29 +516,9 @@ int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int str
 using namespace mfb;
 
 // ==========================================================================================
-// C ABI (declared in include/maskfusion_b200.h)
+// the backbone handle
 // ==========================================================================================
 struct mf_backbone : Backbone { using Backbone::Backbone; };
-
-extern "C" int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, const void* dResidual, void* dOut, int M, int N, int K, int relu, void* stream)
-{
-    MF_TRY
-    return launch_gemm_bf16(dA, dB, dBias, dResidual, dOut, M, N, K, relu, (cudaStream_t)stream);
-    MF_CATCH(-1)
-}
-
-// implicit-GEMM 3x3 / stride 1 / pad 1 convolution on an NHWC bf16 activation (weights [Cout][3][3][Cin] bf16); the geometry is
-// cnn_conv_implicit's, anything else returns -2 before a driver call
-extern "C" int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBias, const void* dResidual, void* dOut, int H, int W, int Cin, int Cout,
-                               int relu, void* stream)
-{
-    MF_TRY
-    int g3[3] = {W, H, Cin};
-    // products in unsigned arithmetic: a refused geometry may overflow them, and the refusal does not read them
-    return launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, (int)((unsigned)H * (unsigned)W), Cout, (int)(9u * (unsigned)Cin), relu, (cudaStream_t)stream,
-                            g3);
-    MF_CATCH(-1)
-}
 
 // ResNet-101-FPN (mf_weights.cu has the layer table); throws CudaError
 Backbone::Backbone(int S_, unsigned seed, cudaStream_t s) : S(S_), stream(s), w(MRCNN_BACKBONE, seed, s)
@@ -580,53 +535,43 @@ Backbone::Backbone(int S_, unsigned seed, cudaStream_t s) : S(S_), stream(s), w(
     lat.alloc((size_t)fs[0] * fs[0] * 256); td.alloc((size_t)fs[0] * fs[0] * 256);
 }
 
-extern "C" mf_backbone* mf_backbone_create(int input_size, unsigned seed, void* stream)
+namespace mfb {
+cudaStream_t backbone_stream(mf_backbone* h) { return h->stream; }
+const void* backbone_input(mf_backbone* h) { return h->input; }
+
+void* backbone_level(mf_backbone* h, int level, int* dims3)
 {
-    MF_TRY
-    if (input_size % 64) { cnn_fail("input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"); return nullptr; }
-    return new mf_backbone(input_size, seed, (cudaStream_t)stream);
-    MF_CATCH_AS(nullptr, "backbone: ")
+    const int S = h->S;
+    const int fs[5] = {S / 4, S / 8, S / 16, S / 32, S / 64};
+    const int cdim[4] = {256, 512, 1024, 2048};
+    if (level >= 0 && level < 4) { dims3[0] = dims3[1] = fs[level]; dims3[2] = cdim[level]; __nv_bfloat16* c[4] = {h->C2, h->C3, h->C4, h->C5}; return c[level]; }
+    if (level >= 4 && level < 9) { dims3[0] = dims3[1] = fs[level - 4]; dims3[2] = 256; return h->P[level - 4]; }
+    return nullptr;
 }
 
-extern "C" void mf_backbone_destroy(mf_backbone* h) { delete h; }
-
-extern "C" int mf_backbone_num_layers(mf_backbone* h) { MF_TRY return h ? (int)h->layers.size() : cnn_fail("backbone: null handle"); MF_CATCH(-1) }
-// layer table: Cin Cout k stride pad Kpad
-extern "C" int mf_backbone_layer(mf_backbone* h, int i, int* out6)
+// letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs; rule R-MOLD)
+void backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H)
 {
-    MF_TRY
-    if (!h || i < 0 || i >= (int)h->layers.size() || !out6) return cnn_fail("backbone: bad layer index");
-    const LayerGeom& L = h->layers[i];
-    out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
-    return 0;
-    MF_CATCH(-1)
-}
-// weights [Cout x Kpad] fp32 (bf16-representable), (ky,kx,cin) order along K; bias [Cout]
-extern "C" int mf_backbone_get_weights(mf_backbone* h, int i, float* w, float* bias)
-{
-    MF_TRY return h ? h->w.get(i, w, bias) : cnn_fail("backbone: null handle"); MF_CATCH(-1)
-}
-
-// pretrained weights (mf_weights.cu): every layer is read, checked and folded on the host before the device tables change; the copy is
-// ordered on the handle's stream and complete on return
-extern "C" int mf_backbone_load_weights(mf_backbone* h, const char* path)
-{
-    MF_TRY return h ? h->w.load(path, h->stream) : cnn_fail("backbone: null handle"); MF_CATCH(-1)
+    const int S = h->S;
+    const MoldGeom g = cnn_mold_geometry(S, W, H);
+    const double zoomx = (double)W / (double)g.newW, zoomy = (double)H / (double)g.newH;     // in / out per axis (R-MOLD)
+    if (S > 65535) throw CudaError{"mold: the input size exceeds the grid's 65535 rows"};
+    launch(Enq{h->stream, nullptr}, nullptr, k_mold_input, dim3((S + 255) / 256, S), 256, 0, (const uchar4*)d_rgba, W, H, S, zoomx, zoomy, g.offx,
+           g.offy, g.newW, g.newH, h->input.p);
 }
 
 // forward on an already-moulded input (device, NHWC bf16 S x S x 3).  Outputs stay on the device (P2..P6, NHWC bf16).
-extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
+void backbone_forward(mf_backbone* h, const void* d_input)
 {
-    MF_TRY
-    if (!h) return cnn_fail("backbone: null handle");
     Backbone* b = h; cudaStream_t s = h->stream;
+    const Enq q{s, nullptr};
     b->flops = 0; b->gemms = 0;
     const int S = b->S;
     int H, W;
     int li = 0;                                      // the next layer of the table
     // C1: 7x7/2 + ReLU, max-pool 3x3/2
-    if (run_conv(b, li++, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W)) return -2;
-    k_maxpool3s2<<<8 * num_sms(), 256, 0, s>>>(b->bufA, H, W, 64, H / 2, W / 2, b->bufB);
+    run_conv(b, li++, (const __nv_bfloat16*)d_input, S, S, b->bufA, nullptr, 1, s, &H, &W);
+    launch(q, nullptr, k_maxpool3s2, 8 * num_sms(), 256, 0, b->bufA.p, H, W, 64, H / 2, W / 2, b->bufB.p);
     H /= 2; W /= 2;
     __nv_bfloat16* x = b->bufB;                      // current block input
     const int nblocks[4] = {3, 4, 23, 3};
@@ -640,13 +585,13 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
             __nv_bfloat16* all[4] = {b->bufA, b->bufB, b->bufC, b->bufS};
             for (int k = 0; k < 4 && n < 3; ++k) if (all[k] != x) t[n++] = all[k];
             int H1, W1;
-            if (run_conv(b, c1, x, H, W, t[0], nullptr, 1, s, &H1, &W1)) return -2;
-            if (run_conv(b, c2, t[0], H1, W1, t[1], nullptr, 1, s)) return -2;
+            run_conv(b, c1, x, H, W, t[0], nullptr, 1, s, &H1, &W1);
+            run_conv(b, c2, t[0], H1, W1, t[1], nullptr, 1, s);
             const __nv_bfloat16* shortcut = x;
-            if (sc >= 0) { if (run_conv(b, sc, x, H, W, t[2], nullptr, 0, s)) return -2; shortcut = t[2]; }
+            if (sc >= 0) { run_conv(b, sc, x, H, W, t[2], nullptr, 0, s); shortcut = t[2]; }
             const bool last = blk == nblocks[st] - 1;
             __nv_bfloat16* y = last ? stageOut[st] : t[0];
-            if (run_conv(b, c3, t[1], H1, W1, y, shortcut, 1, s)) return -2;
+            run_conv(b, c3, t[1], H1, W1, y, shortcut, 1, s);
             x = y; H = H1; W = W1;
         }
     // FPN
@@ -654,19 +599,99 @@ extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
     __nv_bfloat16* Cs[4] = {b->C2, b->C3, b->C4, b->C5};
     const int fpnLat = li, fpnOut = li + 4;
     // P5 lateral
-    if (run_conv(b, fpnLat + 3, Cs[3], fs[3], fs[3], b->td, nullptr, 0, s)) return -2;
+    run_conv(b, fpnLat + 3, Cs[3], fs[3], fs[3], b->td, nullptr, 0, s);
     __nv_bfloat16* top = b->td;                       // running top-down map (pre-3x3)
     __nv_bfloat16* tdBuf[2] = {b->bufA, b->bufB};
-    if (run_conv(b, fpnOut + 3, top, fs[3], fs[3], b->P[3], nullptr, 0, s)) return -2;
+    run_conv(b, fpnOut + 3, top, fs[3], fs[3], b->P[3], nullptr, 0, s);
     for (int i = 2; i >= 0; --i) {
-        if (run_conv(b, fpnLat + i, Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s)) return -2;
+        run_conv(b, fpnLat + i, Cs[i], fs[i], fs[i], b->lat, nullptr, 0, s);
         __nv_bfloat16* nt = tdBuf[i & 1];
-        k_upsample_add<<<8 * num_sms(), 256, 0, s>>>(b->lat, top, fs[i], fs[i], 256, nt);
+        launch(q, nullptr, k_upsample_add, 8 * num_sms(), 256, 0, b->lat.p, top, fs[i], fs[i], 256, nt);
         top = nt;
-        if (run_conv(b, fpnOut + i, top, fs[i], fs[i], b->P[i], nullptr, 0, s)) return -2;
+        run_conv(b, fpnOut + i, top, fs[i], fs[i], b->P[i], nullptr, 0, s);
     }
-    k_subsample2<<<64, 256, 0, s>>>(b->P[3], fs[3], fs[3], 256, b->P[4]);       // P6
-    return cnn_check_launch("backbone forward") ? -3 : 0;
+    launch(q, nullptr, k_subsample2, 64, 256, 0, b->P[3].p, fs[3], fs[3], 256, b->P[4].p);       // P6
+}
+}  // namespace mfb
+
+// ==========================================================================================
+// C ABI (declared in include/maskfusion_b200.h)
+// ==========================================================================================
+extern "C" int mf_gemm_bf16(const void* dA, const void* dB, const float* dBias, const void* dResidual, void* dOut, int M, int N, int K, int relu, void* stream)
+{
+    MF_TRY
+    launch_gemm_bf16(dA, dB, dBias, dResidual, dOut, M, N, K, relu, (cudaStream_t)stream);
+    return 0;
+    MF_CATCH(-2)
+}
+
+// implicit-GEMM 3x3 / stride 1 / pad 1 convolution on an NHWC bf16 activation (weights [Cout][3][3][Cin] bf16); the geometry is
+// cnn_conv_implicit's, anything else returns -2 before a driver call
+extern "C" int mf_conv3x3_bf16(const void* dIn, const void* dW, const float* dBias, const void* dResidual, void* dOut, int H, int W, int Cin, int Cout,
+                               int relu, void* stream)
+{
+    MF_TRY
+    int g3[3] = {W, H, Cin};
+    // products in unsigned arithmetic: a refused geometry may overflow them, and the refusal does not read them
+    launch_gemm_bf16(dIn, dW, dBias, dResidual, dOut, (int)((unsigned)H * (unsigned)W), Cout, (int)(9u * (unsigned)Cin), relu, (cudaStream_t)stream, g3);
+    return 0;
+    MF_CATCH(-2)
+}
+
+extern "C" mf_backbone* mf_backbone_create(int input_size, unsigned seed, void* stream)
+{
+    MF_TRY
+    if (input_size % 64) { mf_set_error("input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"); return nullptr; }
+    return new mf_backbone(input_size, seed, (cudaStream_t)stream);
+    MF_CATCH_AS(nullptr, "backbone: ")
+}
+
+extern "C" void mf_backbone_destroy(mf_backbone* h) { delete h; }
+
+extern "C" int mf_backbone_num_layers(mf_backbone* h)
+{
+    MF_TRY
+    if (!h) throw CudaError{"backbone: null handle"};
+    return (int)h->layers.size();
+    MF_CATCH(-1)
+}
+// layer table: Cin Cout k stride pad Kpad
+extern "C" int mf_backbone_layer(mf_backbone* h, int i, int* out6)
+{
+    MF_TRY
+    if (!h || i < 0 || i >= (int)h->layers.size() || !out6) throw CudaError{"backbone: bad layer index"};
+    const LayerGeom& L = h->layers[i];
+    out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
+    return 0;
+    MF_CATCH(-1)
+}
+// weights [Cout x Kpad] fp32 (bf16-representable), (ky,kx,cin) order along K; bias [Cout]
+extern "C" int mf_backbone_get_weights(mf_backbone* h, int i, float* w, float* bias)
+{
+    MF_TRY
+    if (!h) throw CudaError{"backbone: null handle"};
+    h->w.get(i, w, bias);
+    return 0;
+    MF_CATCH(-1)
+}
+
+// pretrained weights (mf_weights.cu): every layer is read, checked and folded on the host before the device tables change; the copy is
+// ordered on the handle's stream and complete on return
+extern "C" int mf_backbone_load_weights(mf_backbone* h, const char* path)
+{
+    MF_TRY
+    if (!h) throw CudaError{"backbone: null handle"};
+    h->w.load(path, h->stream);
+    return 0;
+    MF_CATCH(-1)
+}
+
+extern "C" int mf_backbone_forward(mf_backbone* h, const void* d_input)
+{
+    MF_TRY
+    if (!h) throw CudaError{"backbone: null handle"};
+    backbone_forward(h, d_input);
+    return 0;
     MF_CATCH(-1)
 }
 extern "C" double mf_backbone_flops(mf_backbone* h) { return h ? h->flops : 0; }
@@ -674,37 +699,23 @@ extern "C" int mf_backbone_num_gemms(mf_backbone* h) { return h ? h->gemms : 0; 
 extern "C" void* mf_backbone_input_buffer(mf_backbone* h) { return h ? h->input.p : nullptr; }
 extern "C" void* mf_backbone_stream(mf_backbone* h) { return h ? (void*)h->stream : nullptr; }
 // level 0..3 = C2..C5, 4..8 = P2..P6; returns device pointer, fills dims (H, W, C)
-extern "C" void* mf_backbone_output(mf_backbone* h, int level, int* dims3)
-{
-    if (!h) return nullptr;
-    Backbone* b = h; const int S = b->S;
-    const int fs[5] = {S / 4, S / 8, S / 16, S / 32, S / 64};
-    const int cdim[4] = {256, 512, 1024, 2048};
-    if (level >= 0 && level < 4) { dims3[0] = dims3[1] = fs[level]; dims3[2] = cdim[level]; __nv_bfloat16* c[4] = {b->C2, b->C3, b->C4, b->C5}; return c[level]; }
-    if (level >= 4 && level < 9) { dims3[0] = dims3[1] = fs[level - 4]; dims3[2] = 256; return b->P[level - 4]; }
-    return nullptr;
-}
+extern "C" void* mf_backbone_output(mf_backbone* h, int level, int* dims3) { return h ? backbone_level(h, level, dims3) : nullptr; }
 extern "C" int mf_backbone_download(mf_backbone* h, int level, void* host_bf16)
 {
     MF_TRY
     int d[3];
-    void* p = mf_backbone_output(h, level, d);
-    if (!p) return cnn_fail("backbone: no handle or level outside 0..8");
-    return cnn_download(h->stream, host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2) ? -2 : 0;
+    const void* p = h ? backbone_level(h, level, d) : nullptr;
+    if (!p) throw CudaError{"backbone: no handle or level outside 0..8"};
+    cnn_read_back(h->stream, host_bf16, p, (size_t)d[0] * d[1] * d[2] * 2);
+    return 0;
     MF_CATCH(-1)
 }
-// letter-box + normalise a 640x480 (or any) RGBA8 device image into the network input (MaskRCNN.py.in mold_inputs; rule R-MOLD)
 extern "C" int mf_backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H)
 {
     MF_TRY
-    if (!h) return cnn_fail("backbone: null handle");
-    if (W <= 0 || H <= 0) return cnn_fail("mold: the image needs W > 0 and H > 0");
-    Backbone* b = h; const int S = b->S;
-    const MoldGeom g = cnn_mold_geometry(S, W, H);
-    const double zoomx = (double)W / (double)g.newW, zoomy = (double)H / (double)g.newH;     // in / out per axis (R-MOLD)
-    if (S > 65535) return cnn_fail("mold: the input size exceeds the grid's 65535 rows");
-    k_mold_input<<<dim3((S + 255) / 256, S), 256, 0, h->stream>>>((const uchar4*)d_rgba, W, H, S, zoomx, zoomy, g.offx, g.offy, g.newW, g.newH,
-                                                                   b->input);
-    return cnn_check_launch("k_mold_input") ? -2 : 0;
+    if (!h) throw CudaError{"backbone: null handle"};
+    if (W <= 0 || H <= 0) throw CudaError{"mold: the image needs W > 0 and H > 0"};
+    backbone_mold(h, d_rgba, W, H);
+    return 0;
     MF_CATCH(-1)
 }

@@ -236,72 +236,55 @@ struct mf_detector {
 };
 
 // the image geometry: the letter-box window of a W x H image in the S x S input, normalised as norm_boxes does (float64 divide, float32)
-static int set_image(mf_detector* h, int W, int H)
+static void set_image(mf_detector* h, int W, int H)
 {
-    if (W < 1 || H < 1 || W > 16384 || H > 16384) return cnn_fail("detector: image size " + std::to_string(W) + "x" + std::to_string(H) + " outside [1, 16384]");
+    if (W < 1 || H < 1 || W > 16384 || H > 16384)
+        throw CudaError{"detector: image size " + std::to_string(W) + "x" + std::to_string(H) + " outside [1, 16384]"};
     if ((size_t)W * H > h->idimg.n) {
-        if (cudaStreamSynchronize(h->s) != cudaSuccess) return cnn_fail("detector: id image free failed");
+        if (cudaStreamSynchronize(h->s) != cudaSuccess) throw CudaError{"detector: id image free failed"};
         try {
             h->idimg.alloc((size_t)W * H);
         } catch (const CudaError& e) {
-            return cnn_fail("detector: id image " + e.what);
+            throw CudaError{"detector: id image " + e.what};
         }
     }
     const MoldGeom g = cnn_mold_geometry(h->S, W, H);
     const double s1 = (double)(h->S - 1);
     h->win = make_float4((float)(g.offy / s1), (float)(g.offx / s1), (float)((g.offy + g.newH - 1) / s1), (float)((g.offx + g.newW - 1) / s1));
     h->imgW = W; h->imgH = H;
-    return 0;
 }
 
-namespace mfb {
-cudaStream_t detector_stream(mf_detector* h) { return h->s; }
-
-int detector_reserve_image(mf_detector* h, int W, int H) { return set_image(h, W, H); }
-
-int detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr)
-{
-    const size_t P = (size_t)h->imgW * h->imgH;
-    if (P % 16 || ((uintptr_t)mask & 15)) return cnn_fail("detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer");
-    const int n16 = (int)(P / 16);
-    k_frame_masks<<<(n16 + 255) / 256, 256, 0, h->s>>>((const uint4*)h->idimg.p, h->einfo, h->ecls, n16, (uint4*)mask, hdr);
-    return cnn_check_launch("k_frame_masks");
-}
-}  // namespace mfb
-
-static int gemm(mf_detector* h, int layer, const void* A, void* out, int M, int relu, bool f32)
+static void gemm(mf_detector* h, int layer, const void* A, void* out, int M, int relu, bool f32)
 {
     const LayerGeom L = mrcnn_layer(MRCNN_DETECTOR, layer);
-    return launch_gemm_bf16(A, h->w.w(layer), h->w.b(layer), nullptr, out, M, L.rows, L.K, relu, h->s, nullptr, f32) ? -2 : 0;
+    launch_gemm_bf16(A, h->w.w(layer), h->w.b(layer), nullptr, out, M, L.rows, L.K, relu, h->s, nullptr, f32);
 }
 
-static int refine(mf_detector* h, const float* rois, const float* logits, int lstride, const float* deltas, int dstride, int n)
+static void refine(mf_detector* h, const float* rois, const float* logits, int lstride, const float* deltas, int dstride, int n)
 {
-    k_det_refine<<<(n + 127) / 128, 128, 0, h->s>>>((const float4*)rois, logits, lstride, deltas, dstride, n, h->win, h->keys, h->boxes, h->scores);
-    k_det_select<<<1, SEL_N, 0, h->s>>>(h->keys, n, h->boxes, h->scores, h->dets, h->dboxes, h->count);
-    return cnn_check_launch("detection layer") ? -3 : 0;
+    const Enq q{h->s, nullptr};
+    launch(q, nullptr, k_det_refine, (n + 127) / 128, 128, 0, (const float4*)rois, logits, lstride, deltas, dstride, n, h->win, h->keys.p, h->boxes.p,
+           h->scores.p);
+    launch(q, nullptr, k_det_select, 1, SEL_N, 0, h->keys.p, n, h->boxes.p, h->scores.p, h->dets.p, h->dboxes.p, h->count.p);
 }
 
-static int paste(mf_detector* h, const float* dets, const float* masks)
+static void paste(mf_detector* h, const float* dets, const float* masks)
 {
-    k_unmold<<<1, 1, 0, h->s>>>(dets, h->win, h->imgW, h->imgH, h->ep, h->ebox, h->eid, h->ecls, h->erois, h->einfo);
-    k_paste<<<(h->imgW * h->imgH + 255) / 256, 256, 0, h->s>>>(masks, h->ebox, h->eid, h->einfo, h->imgW, h->imgH, h->idimg);
-    return cnn_check_launch("id image") ? -3 : 0;
+    const Enq q{h->s, nullptr};
+    launch(q, nullptr, k_unmold, 1, 1, 0, dets, h->win, h->imgW, h->imgH, h->ep, h->ebox.p, h->eid.p, h->ecls.p, h->erois.p, h->einfo.p);
+    launch(q, nullptr, k_paste, (h->imgW * h->imgH + 255) / 256, 256, 0, masks, h->ebox.p, h->eid.p, h->einfo.p, h->imgW, h->imgH, h->idimg.p);
 }
 
-// ==========================================================================================
-// C ABI (declared in include/maskfusion_b200.h)
-// ==========================================================================================
-mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed)
-    : rpn(rpn_), bb(rpn_backbone(rpn_)), s((cudaStream_t)mf_backbone_stream(bb)), w(MRCNN_DETECTOR, seed, s)
+mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed) : rpn(rpn_), bb(rpn_backbone(rpn_)), s(backbone_stream(bb)), w(MRCNN_DETECTOR, seed, s)
 {
     const LayerGeom fc1L = mrcnn_layer(MRCNN_DETECTOR, L_FC1), headL = mrcnn_layer(MRCNN_DETECTOR, L_HEAD), m1 = mrcnn_layer(MRCNN_DETECTOR, L_M1),
                     decL = mrcnn_layer(MRCNN_DETECTOR, L_DECONV), mlogL = mrcnn_layer(MRCNN_DETECTOR, L_MLOG);
     assert(mrcnn_num_layers(MRCNN_DETECTOR) == N_LAYERS && fc1L.rows == FC_N && fc1L.K == POOL * POOL * CH && headL.rows == HEAD_N &&
            m1.rows == CH && m1.K == MCONV_K && decL.rows == 4 * CH && mlogL.rows == MLOG_N);     // the shapes the buffers and kernels assume
     int d[3];
-    mf_backbone_output(bb, 4, d);
+    backbone_level(bb, 4, d);
     S = d[0] * 4;
+    imgW = imgH = S;                                          // the S x S image: its letter-box window is the whole input, `win`'s default
     memset(&ep, 0, sizeof ep);
     ep.min_score = 0.55;
     const size_t mrows = (size_t)DET_MAX * MPIX;
@@ -309,6 +292,7 @@ mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed)
     boxes.alloc(DET_ROIS); scores.alloc(DET_ROIS); dets.alloc(DET_MAX * 6); dboxes.alloc(DET_MAX); count.alloc(1);
     mpool.alloc(mrows * CH); col.alloc(mrows * MCONV_K); dec.alloc(mrows * 4 * CH); mlog.alloc(mrows * 4 * MLOG_N);
     masks.alloc(DET_MAX * MASK * MASK); ebox.alloc(DET_MAX * 5); ecls.alloc(DET_MAX); erois.alloc(DET_MAX * 4); einfo.alloc(2); eid.alloc(DET_MAX);
+    idimg.alloc((size_t)S * S);
     for (int i = 0; i < 4; ++i) mconv[i].alloc(mrows * CH);
     cudaCheck(cudaMemset(dets, 0, DET_MAX * 6 * 4), "cudaMemset");
     cudaCheck(cudaMemset(count, 0, 4), "cudaMemset");
@@ -316,13 +300,61 @@ mf_detector::mf_detector(mf_rpn* rpn_, unsigned seed)
     cudaCheck(cudaMemset(einfo, 0, 8), "cudaMemset");
 }
 
+namespace mfb {
+cudaStream_t detector_stream(mf_detector* h) { return h->s; }
+
+void detector_reserve_image(mf_detector* h, int W, int H) { set_image(h, W, H); }
+
+void detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr)
+{
+    const size_t P = (size_t)h->imgW * h->imgH;
+    if (P % 16 || ((uintptr_t)mask & 15)) throw CudaError{"detector: the frame mask needs W x H % 16 == 0 and a 16-byte aligned buffer"};
+    const int n16 = (int)(P / 16);
+    launch(Enq{h->s, nullptr}, nullptr, k_frame_masks, (n16 + 255) / 256, 256, 0, (const uint4*)h->idimg.p, h->einfo.p, h->ecls.p, n16, (uint4*)mask,
+           hdr);
+}
+
+void detector_run(mf_detector* h, int stages)
+{
+    if (stages & MF_DET_CLASSIFIER) {
+        gemm(h, L_FC1, rpn_pooled(h->rpn), h->fc1, DET_ROIS, 1, false);
+        gemm(h, L_FC2, h->fc1, h->fc2, DET_ROIS, 1, false);
+        gemm(h, L_HEAD, h->fc2, h->head, DET_ROIS, 0, true);
+    }
+    if (stages & MF_DET_DETECTIONS) refine(h, rpn_rois(h->rpn), h->head, HEAD_N, h->head + NCLS, HEAD_N, DET_ROIS);
+    if (stages & MF_DET_MASKS) {
+        roi_align(h->bb, (const float*)h->dboxes.p, DET_MAX, MPOOL, h->mpool);
+        const __nv_bfloat16* x = h->mpool;
+        for (int i = 0; i < 4; ++i) {
+            launch_im2col(x, DET_MAX, MPOOL, MPOOL, CH, MPOOL, MPOOL, 3, 1, 1, MCONV_K, h->col, h->s);
+            gemm(h, L_M1 + i, h->col, h->mconv[i], DET_MAX * MPIX, 1, false);
+            x = h->mconv[i];
+        }
+        gemm(h, L_DECONV, x, h->dec, DET_MAX * MPIX, 1, false);
+        gemm(h, L_MLOG, h->dec, h->mlog, DET_MAX * MPIX * 4, 0, true);
+        launch(Enq{h->s, nullptr}, nullptr, k_mask_select, (DET_MAX * MASK * MASK + 255) / 256, 256, 0, h->mlog.p, h->dets.p, h->masks.p);
+    }
+    if (stages & MF_DET_ID_IMAGE) paste(h, h->dets, h->masks);
+}
+
+void detector_detect(mf_detector* h, const void* d_rgba, int W, int H)
+{
+    set_image(h, W, H);
+    backbone_mold(h->bb, d_rgba, W, H);
+    backbone_forward(h->bb, backbone_input(h->bb));
+    rpn_run(h->rpn, MF_RPN_CONV | MF_RPN_HEADS | MF_RPN_PROPOSALS | MF_RPN_ROI_ALIGN);
+    detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+}
+}  // namespace mfb
+
+// ==========================================================================================
+// C ABI (declared in include/maskfusion_b200.h)
+// ==========================================================================================
 extern "C" mf_detector* mf_detector_create(mf_rpn* rpn, unsigned seed)
 {
     MF_TRY
-    if (!rpn) { cnn_fail("detector: no region-proposal handle"); return nullptr; }
-    mf_detector* h = new mf_detector(rpn, seed);
-    if (set_image(h, h->S, h->S)) { delete h; return nullptr; }
-    return h;
+    if (!rpn) { mf_set_error("detector: no region-proposal handle"); return nullptr; }
+    return new mf_detector(rpn, seed);
     MF_CATCH_AS(nullptr, "detector: ")
 }
 
@@ -331,26 +363,8 @@ extern "C" void mf_detector_destroy(mf_detector* h) { delete h; }
 extern "C" int mf_detector_run(mf_detector* h, int stages)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    const cudaStream_t s = h->s;
-    if (stages & MF_DET_CLASSIFIER) {
-        if (gemm(h, L_FC1, rpn_pooled(h->rpn), h->fc1, DET_ROIS, 1, false) || gemm(h, L_FC2, h->fc1, h->fc2, DET_ROIS, 1, false) ||
-            gemm(h, L_HEAD, h->fc2, h->head, DET_ROIS, 0, true)) return -2;
-    }
-    if ((stages & MF_DET_DETECTIONS) && refine(h, rpn_rois(h->rpn), h->head, HEAD_N, h->head + NCLS, HEAD_N, DET_ROIS)) return -3;
-    if (stages & MF_DET_MASKS) {
-        if (mf_roi_align_bf16(h->bb, (const float*)h->dboxes.p, DET_MAX, MPOOL, h->mpool)) return -3;
-        const __nv_bfloat16* x = h->mpool;
-        for (int i = 0; i < 4; ++i) {
-            launch_im2col(x, DET_MAX, MPOOL, MPOOL, CH, MPOOL, MPOOL, 3, 1, 1, MCONV_K, h->col, s);
-            if (gemm(h, L_M1 + i, h->col, h->mconv[i], DET_MAX * MPIX, 1, false)) return -2;
-            x = h->mconv[i];
-        }
-        if (gemm(h, L_DECONV, x, h->dec, DET_MAX * MPIX, 1, false) || gemm(h, L_MLOG, h->dec, h->mlog, DET_MAX * MPIX * 4, 0, true)) return -2;
-        k_mask_select<<<(DET_MAX * MASK * MASK + 255) / 256, 256, 0, s>>>(h->mlog, h->dets, h->masks);
-        if (cnn_check_launch("k_mask_select")) return -3;
-    }
-    if ((stages & MF_DET_ID_IMAGE) && paste(h, h->dets, h->masks)) return -3;
+    if (!h) throw CudaError{"detector: null handle"};
+    detector_run(h, stages);
     return 0;
     MF_CATCH(-1)
 }
@@ -358,22 +372,20 @@ extern "C" int mf_detector_run(mf_detector* h, int stages)
 extern "C" int mf_detector_forward(mf_detector* h, int image_w, int image_h)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    if (set_image(h, image_w, image_h)) return -1;
-    return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+    if (!h) throw CudaError{"detector: null handle"};
+    set_image(h, image_w, image_h);
+    detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_detect(mf_detector* h, const void* d_rgba, int W, int H)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    if (!d_rgba || ((uintptr_t)d_rgba & 3)) return cnn_fail("detector: the image needs a 4-byte aligned device pointer");
-    if (set_image(h, W, H)) return -1;
-    if (mf_backbone_mold(h->bb, d_rgba, W, H) || mf_backbone_forward(h->bb, mf_backbone_input_buffer(h->bb)))
-        return cnn_fail(std::string("detector: backbone: ") + mf_last_error());
-    if (mf_rpn_forward(h->rpn)) return -3;
-    return mf_detector_run(h, MF_DET_CLASSIFIER | MF_DET_DETECTIONS | MF_DET_MASKS | MF_DET_ID_IMAGE);
+    if (!h) throw CudaError{"detector: null handle"};
+    if (!d_rgba || ((uintptr_t)d_rgba & 3)) throw CudaError{"detector: the image needs a 4-byte aligned device pointer"};
+    detector_detect(h, d_rgba, W, H);
+    return 0;
     MF_CATCH(-1)
 }
 
@@ -381,9 +393,9 @@ extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const in
                                       int n_special)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
     if (n_filter < 0 || n_special < 0 || n_filter > EXPORT_CAP || n_special > EXPORT_CAP || (n_filter && !class_filter) || (n_special && !special_assignments))
-        return cnn_fail("detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries");
+        throw CudaError{"detector_set_export: lists of 0.." + std::to_string(EXPORT_CAP) + " entries"};
     ExportParams ep;
     memset(&ep, 0, sizeof ep);
     ep.min_score = min_score; ep.n_filter = n_filter; ep.n_special = n_special;
@@ -397,22 +409,24 @@ extern "C" int mf_detector_set_export(mf_detector* h, double min_score, const in
 extern "C" int mf_detector_refine(mf_detector* h, const float* d_rois, const float* d_logits, const float* d_deltas, int n)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    if (n < 1 || n > DET_ROIS) return cnn_fail("detector_refine: n = " + std::to_string(n) + " outside [1, 1000]");
+    if (!h) throw CudaError{"detector: null handle"};
+    if (n < 1 || n > DET_ROIS) throw CudaError{"detector_refine: n = " + std::to_string(n) + " outside [1, 1000]"};
     if (!d_rois || !d_logits || !d_deltas || ((uintptr_t)d_rois & 15) || ((uintptr_t)d_logits & 3) || ((uintptr_t)d_deltas & 3))
-        return cnn_fail("detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer");
-    return refine(h, d_rois, d_logits, NCLS, d_deltas, 4 * NCLS, n);
+        throw CudaError{"detector_refine: rois need a 16-byte, logits and deltas a 4-byte aligned device pointer"};
+    refine(h, d_rois, d_logits, NCLS, d_deltas, 4 * NCLS, n);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_paste(mf_detector* h, const float* d_detections, const float* d_masks, int W, int H)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
     if (!d_detections || !d_masks || ((uintptr_t)d_detections & 3) || ((uintptr_t)d_masks & 3))
-        return cnn_fail("detector_paste: detections and masks need 4-byte aligned device pointers");
-    if (set_image(h, W, H)) return -1;
-    return paste(h, d_detections, d_masks);
+        throw CudaError{"detector_paste: detections and masks need 4-byte aligned device pointers"};
+    set_image(h, W, H);
+    paste(h, d_detections, d_masks);
+    return 0;
     MF_CATCH(-1)
 }
 
@@ -421,7 +435,7 @@ extern "C" int mf_detector_num_layers(mf_detector* h) { return h ? N_LAYERS : -1
 extern "C" int mf_detector_layer(mf_detector* h, int i, int* out6)
 {
     MF_TRY
-    if (!h || i < 0 || i >= N_LAYERS || !out6) return cnn_fail("detector: bad layer index");
+    if (!h || i < 0 || i >= N_LAYERS || !out6) throw CudaError{"detector: bad layer index"};
     const LayerGeom L = mrcnn_layer(MRCNN_DETECTOR, i);
     out6[0] = L.cin; out6[1] = L.rows; out6[2] = L.k; out6[3] = L.stride; out6[4] = L.pad; out6[5] = L.K;
     return 0;
@@ -431,7 +445,9 @@ extern "C" int mf_detector_layer(mf_detector* h, int i, int* out6)
 extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* bias)
 {
     MF_TRY
-    return h ? h->w.get(i, w, bias) : cnn_fail("detector: bad layer index");
+    if (!h) throw CudaError{"detector: bad layer index"};
+    h->w.get(i, w, bias);
+    return 0;
     MF_CATCH(-1)
 }
 
@@ -439,48 +455,55 @@ extern "C" int mf_detector_get_weights(mf_detector* h, int i, float* w, float* b
 extern "C" int mf_detector_load_weights(mf_detector* h, const char* path)
 {
     MF_TRY
-    return h ? h->w.load(path, h->s) : cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
+    h->w.load(path, h->s);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_fc(mf_detector* h, void* fc1_bf16, void* fc2_bf16)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    return cnn_download(h->s, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2) || cnn_download(h->s, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2) ? -1 : 0;
+    if (!h) throw CudaError{"detector: null handle"};
+    cnn_read_back(h->s, fc1_bf16, h->fc1, (size_t)DET_ROIS * FC_N * 2);
+    cnn_read_back(h->s, fc2_bf16, h->fc2, (size_t)DET_ROIS * FC_N * 2);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_head_outputs(mf_detector* h, float* logits, float* deltas)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
-    return cnn_download(h->s, logits, h->head, NCLS * 4, DET_ROIS, HEAD_N * 4) ||
-                   cnn_download(h->s, deltas, h->head.p + NCLS, NCLS * 16, DET_ROIS, HEAD_N * 4) ? -1 : 0;
+    if (!h) throw CudaError{"detector: null handle"};
+    cnn_read_back(h->s, logits, h->head, NCLS * 4, DET_ROIS, HEAD_N * 4);
+    cnn_read_back(h->s, deltas, h->head.p + NCLS, NCLS * 16, DET_ROIS, HEAD_N * 4);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_mask_layer(mf_detector* h, int i, void* host)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
     const size_t px = (size_t)DET_MAX * MPIX;
     switch (i) {
-    case 0: return cnn_download(h->s, host, h->mpool, px * CH * 2);
-    case 1: case 2: case 3: case 4: return cnn_download(h->s, host, h->mconv[i - 1], px * CH * 2);
-    case 5: return cnn_download(h->s, host, h->dec, px * 4 * CH * 2);
-    case 6: return cnn_download(h->s, host, h->mlog, NCLS * 4, px * 4, MLOG_N * 4);
-    default: return cnn_fail("detector: mask layer must be 0..6");
+    case 0: cnn_read_back(h->s, host, h->mpool, px * CH * 2); break;
+    case 1: case 2: case 3: case 4: cnn_read_back(h->s, host, h->mconv[i - 1], px * CH * 2); break;
+    case 5: cnn_read_back(h->s, host, h->dec, px * 4 * CH * 2); break;
+    case 6: cnn_read_back(h->s, host, h->mlog, NCLS * 4, px * 4, MLOG_N * 4); break;
+    default: throw CudaError{"detector: mask layer must be 0..6"};
     }
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_detections(mf_detector* h, float* detections)
 {
     MF_TRY
+    if (!h) throw CudaError{"detector: null handle"};
     int n = 0;
-    if (!h) return cnn_fail("detector: null handle");
-    if (cnn_download(h->s, detections, h->dets, DET_MAX * 6 * 4) || cnn_download(h->s, &n, h->count, 4)) return -1;
+    cnn_read_back(h->s, detections, h->dets, DET_MAX * 6 * 4);
+    cnn_read_back(h->s, &n, h->count, 4);
     return n;
     MF_CATCH(-1)
 }
@@ -488,19 +511,22 @@ extern "C" int mf_detector_get_detections(mf_detector* h, float* detections)
 extern "C" int mf_detector_get_masks(mf_detector* h, float* masks)
 {
     MF_TRY
-    return h ? cnn_download(h->s, masks, h->masks, DET_MAX * MASK * MASK * 4) : cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
+    cnn_read_back(h->s, masks, h->masks, DET_MAX * MASK * MASK * 4);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32_t* class_ids, int32_t* rois)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
     int info[2];
-    if (cnn_download(h->s, info, h->einfo, 8)) return -1;
-    if (info[1]) return cnn_fail("generate_id_image: special_assignments[class_id] out of range");
-    if (cnn_download(h->s, id_image, h->idimg, (size_t)h->imgW * h->imgH) || cnn_download(h->s, class_ids, h->ecls, (size_t)info[0] * 4) ||
-        cnn_download(h->s, rois, h->erois, (size_t)info[0] * 16)) return -1;
+    cnn_read_back(h->s, info, h->einfo, 8);
+    if (info[1]) throw CudaError{"generate_id_image: special_assignments[class_id] out of range"};
+    cnn_read_back(h->s, id_image, h->idimg, (size_t)h->imgW * h->imgH);
+    cnn_read_back(h->s, class_ids, h->ecls, (size_t)info[0] * 4);
+    cnn_read_back(h->s, rois, h->erois, (size_t)info[0] * 16);
     return info[0];
     MF_CATCH(-1)
 }
@@ -508,7 +534,7 @@ extern "C" int mf_detector_get_id_image(mf_detector* h, uint8_t* id_image, int32
 extern "C" int mf_detector_image_size(mf_detector* h, int* w, int* hgt)
 {
     MF_TRY
-    if (!h) return cnn_fail("detector: null handle");
+    if (!h) throw CudaError{"detector: null handle"};
     *w = h->imgW; *hgt = h->imgH;
     return 0;
     MF_CATCH(-1)

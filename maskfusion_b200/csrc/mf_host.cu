@@ -758,11 +758,6 @@ void MaskFusion::initShardComm(const unsigned char* id128, int rank_, int world_
     shardNccl = true;
 }
 
-extern "C" int mf_backbone_mold(struct mf_backbone* h, const void* d_rgba, int W, int H);
-extern "C" int mf_backbone_forward(struct mf_backbone* h, const void* d_input);
-extern "C" void* mf_backbone_input_buffer(struct mf_backbone* h);
-extern "C" void* mf_backbone_stream(struct mf_backbone* h);
-
 // after the entry point's own checks: a backbone, or (asDetector) a detector on some rank of the run; `det` is its handle where it runs
 void MaskFusion::attachNetwork(const char* who, bool asDetector, mf_detector* det)
 {
@@ -771,11 +766,11 @@ void MaskFusion::attachNetwork(const char* who, bool asDetector, mf_detector* de
     if (!asDetector && (detector || detRank >= 0))
         throw CudaError{std::string(who) + ": a detector is attached (it runs its own backbone on the same stream); detach it first"};
     waitNetwork();
-    if (det && detector_reserve_image(det, W, H) != 0) throw CudaError{std::string(who) + ": " + mf_last_error()};
+    if (det) detector_reserve_image(det, W, H);
     if (!netRGBA.p) netRGBA.alloc(P);
 }
 
-void MaskFusion::attachBackbone(void* bb, int everyK)
+void MaskFusion::attachBackbone(mf_backbone* bb, int everyK)
 {
     if (bb) {
         if (!cfg.enableMultipleModels) throw CudaError{"attachBackbone: a -static context runs no segmentation to feed"};
@@ -848,18 +843,17 @@ bool MaskFusion::shardFrameMasks(void** ptr, size_t* bytes)
 void MaskFusion::runNetwork(int slot, bool runBackbone)
 {
     FrameSlot& f = *ring[slot];
-    mf_backbone* bb = (mf_backbone*)backbone;
-    cudaStream_t ns = runBackbone ? (cudaStream_t)mf_backbone_stream(bb) : detector_stream(detector);
+    cudaStream_t ns = runBackbone ? backbone_stream(backbone) : detector_stream(detector);
     cudaCheck(cudaStreamWaitEvent(ns, f.uploaded, 0), "cudaStreamWaitEvent");
     launch_unpack_rgb(f.packet.p, netRGBA, P, Enq{ns, nullptr});
     if (runBackbone) {
-        if (mf_backbone_mold(bb, netRGBA, W, H) != 0) throw CudaError{"backbone: mold_inputs failed"};
+        backbone_mold(backbone, netRGBA, W, H);
         cudaCheck(cudaEventRecord(f.netDone, ns), "cudaEventRecord");               // the slot is free again once the input is molded
         f.netUsed = true;
-        if (mf_backbone_forward(bb, mf_backbone_input_buffer(bb)) != 0) throw CudaError{"backbone: forward failed"};
+        backbone_forward(backbone, backbone_input(backbone));
     } else {
-        if (mf_detector_detect(detector, netRGBA, W, H) != 0 || detector_frame_masks(detector, slotMask(slot), slotHdr(slot)) != 0)
-            throw CudaError{std::string("detector: ") + mf_last_error()};
+        detector_detect(detector, netRGBA, W, H);
+        detector_frame_masks(detector, slotMask(slot), slotHdr(slot));
         // one event for both guards: the slot may be reused, and its mask / header are written
         cudaCheck(cudaEventRecord(f.netDone, ns), "cudaEventRecord");
         f.netUsed = true; f.handoff = true;

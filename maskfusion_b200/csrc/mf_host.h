@@ -177,8 +177,8 @@ public:
     // Mask R-CNN backbone on the frame path (MaskRCNN::executeSequential, MaskRCNN.cpp:147-151, is called from MfSegmentation.cpp:130):
     // every k-th frame the RGB image is letter-boxed into the backbone's input and the ResNet-101-FPN forward is enqueued on the
     // backbone's own stream, next to the dense pipeline of the same GPU (the reference runs its network as a ~5 Hz sidecar)
-    void* backbone = nullptr; int backboneEvery = 0;
-    void attachBackbone(void* bb, int everyK);
+    mf_backbone* backbone = nullptr; int backboneEvery = 0;
+    void attachBackbone(mf_backbone* bb, int everyK);
     // Mask R-CNN detector on the frame path (MfSegmentation.cpp:128-131): a segmentation frame that the caller gave no mask runs the
     // detector every k-th tick on the detector's (= its backbone's) stream; k_frame_masks writes the id image and class list into the
     // frame's mask / header in its slot; the main stream waits (the slot's netDone) just before segmentation reads them.

@@ -191,7 +191,7 @@ struct Enq {
     // after a launch: throws CudaError naming `kernel` if the runtime's last error is set, else counts the launch
     void launched(const void* kernel) const;
 };
-// the one launch of a dense-pipeline kernel: mark (name non-null), launch on q.s, check, count
+// the one launch of a kernel: mark (name non-null), launch on q.s, check, count (a null record: check only)
 template <typename... P, typename... A>
 inline void launch(const Enq& q, const char* name, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args)
 {
@@ -201,27 +201,38 @@ inline void launch(const Enq& q, const char* name, void (*kernel)(P...), dim3 gr
 }
 
 // ---- mf_cnn.cu ----
+// The Mask R-CNN handles (backbone, RPN, detector) belong to no context: every kernel of theirs goes through launch() with Enq{stream,
+// nullptr}, which checks the launch and throws, and counts and times nothing.  Below their extern "C" entry points everything throws
+// CudaError; only the entry points turn it into a return code.
 // D[M x N] = relu?(A[M x K] * B[N x K]^T + bias + residual), bf16 operands; conv3x3 = {Wimg, Himg, Cin}: A is an NHWC activation and the GEMM is
-// the implicit 3x3/s1/p1 convolution; outF32: D is fp32 (no residual), else bf16.  Returns 0 or < 0 with the text in mf_last_error()
-int launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
-                     const int* conv3x3 = nullptr, bool outF32 = false);
+// the implicit 3x3/s1/p1 convolution; outF32: D is fp32 (no residual), else bf16.  Every shape refusal throws before the first driver call
+void launch_gemm_bf16(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu, cudaStream_t s,
+                      const int* conv3x3 = nullptr, bool outF32 = false);
 // one convolution (NHWC bf16, weights [Cout][Kpad] in (ky, kx, cin) order) through the backbone's conv path: the implicit 3x3 GEMM where its
 // geometry guard admits the shape, else im2col into `col` (Hout*Wout*Kpad bf16) + GEMM
-int cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
-             cudaStream_t s);
+void cnn_conv(const void* in, int Hin, int Win, int Cin, int Cout, int k, int stride, int pad, const void* W, const float* B, void* col, void* out, int relu,
+              cudaStream_t s);
 bool cnn_conv_implicit(int k, int stride, int pad, int Cin, int Hin, int Win);     // does cnn_conv take the implicit path (no im2col)?
 // im2col of `nimg` stacked NHWC images (each padded on its own): A[(img, oy, ox)][(ky, kx, cin)], K zero-padded to Kpad
 void launch_im2col(const void* in, int nimg, int Hin, int Win, int Cin, int Hout, int Wout, int k, int stride, int pad, int Kpad, void* col, cudaStream_t s);
 // the letter-box rule of mf_backbone_mold (mould_image): a W x H image is resized by `scale` to newW x newH and placed at (offx, offy) of S x S
 struct MoldGeom { float scale; int newW, newH, offx, offy; };
 MoldGeom cnn_mold_geometry(int S, int W, int H);
-// what the backbone, RPN and detector handles share: the message into mf_last_error() and -1; a failed launch; a read-back of `rows` rows
-// of `width` bytes, `pitch` bytes apart on the device (0: one block), packed into dst after `s` is drained.  dst NULL: nothing is copied
-int cnn_fail(const std::string& msg);
-int cnn_check_launch(const char* what);
-int cnn_download(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows = 1, size_t pitch = 0);
+// the handles' read-back: `rows` rows of `width` bytes, `pitch` bytes apart on the device (0: one block), packed into dst after `s` is
+// drained.  dst NULL: nothing is copied
+void cnn_read_back(cudaStream_t s, void* dst, const void* src, size_t width, size_t rows = 1, size_t pitch = 0);
+// the backbone handle: its stream; its input buffer (where backbone_mold writes); level 0..3 = C2..C5, 4..8 = P2..P6 as a device pointer
+// with dims (H, W, C), nullptr for another level; the letter-boxed input of a W x H RGBA8 device image (W, H > 0); the forward on d_input
+cudaStream_t backbone_stream(mf_backbone* h);
+const void* backbone_input(mf_backbone* h);
+void* backbone_level(mf_backbone* h, int level, int* dims3);
+void backbone_mold(mf_backbone* h, const void* d_rgba, int W, int H);
+void backbone_forward(mf_backbone* h, const void* d_input);
 
-// ---- mf_rpn.cu: what the detection heads read of the RPN handle ----
+// ---- mf_rpn.cu: the RPN handle, and what the detection heads read of it ----
+void rpn_run(mf_rpn* h, int stages);              // MF_RPN_* bits, in order
+// pyramid ROI Align of n boxes on bb's P2..P5, on bb's stream
+void roi_align(mf_backbone* bb, const float* boxes, int n, int pool, void* out);
 mf_backbone* rpn_backbone(mf_rpn* h);
 const float* rpn_rois(mf_rpn* h);                 // [1000][4] proposals, zero padded
 const void* rpn_pooled(mf_rpn* h);                // [1000][7][7][256] bf16
@@ -243,20 +254,23 @@ struct WeightStore {
     // the seeded tables (one LCG stream, seed 0 taken as 1), uploaded on `s`; throws CudaError
     WeightStore(int part, unsigned seed, cudaStream_t s);
     // every layer read, checked and folded on the host, uploaded on `s` and complete on return; the tables change only on success.
-    // 0, or -1 with the message in mf_last_error() naming the file and the tensor (-2: the upload failed)
-    int load(const char* path, cudaStream_t s);
-    int get(int i, float* w, float* b, int rows = -1) const;    // the first `rows` rows (-1: all) of layer i; NULL skips
+    // Throws CudaError naming the file and the tensor, or the failed upload
+    void load(const char* path, cudaStream_t s);
+    void get(int i, float* w, float* b, int rows = -1) const;   // the first `rows` rows (-1: all) of layer i; NULL skips; throws on a bad i
     const __nv_bfloat16* w(int i) const { return dW.p + wOff[i]; }
     const float* b(int i) const { return dB.p + bOff[i]; }
 };
 
 // ---- mf_heads.cu: the detector on the frame path (mf_attach_detector) ----
 cudaStream_t detector_stream(mf_detector* h);
-int detector_reserve_image(mf_detector* h, int W, int H);      // id image sized for W x H once: mf_detector_detect at W x H then never reallocates
+void detector_reserve_image(mf_detector* h, int W, int H);     // id image sized for W x H once: detector_detect at W x H then never reallocates
+void detector_run(mf_detector* h, int stages);                 // MF_DET_* bits, in order
+// what MaskRCNN.execute() does on a W x H RGBA8 device image (4-byte aligned): mould, backbone, RPN and every head stage, on one stream
+void detector_detect(mf_detector* h, const void* d_rgba, int W, int H);
 // FrameData::mask / classIDs from the last id image (MaskRCNN.cpp:98-112, 147-151), enqueued on the detector's stream: the id image into
 // `mask` (W x H of the last detect), hdr->nMasks = exported + 1, hdr->classIDs = {0, exported class ids...}.  The count and ids stay on the
 // device.  A failed export rule gives nMasks = 0 and hdr->detectError = 1.
-int detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr);
+void detector_frame_masks(mf_detector* h, uint8_t* mask, FrameHdr* hdr);
 
 // ---- mf_frame.cu ----
 void launch_unpack_rgb(const uint8_t* rgb3, uchar4* out, int P, Enq q);

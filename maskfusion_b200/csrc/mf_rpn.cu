@@ -242,30 +242,30 @@ static RoiLevels roi_levels(mf_backbone* bb)
     RoiLevels lv;
     for (int i = 0; i < 4; ++i) {
         int d[3];
-        lv.P[i] = (const __nv_bfloat16*)mf_backbone_output(bb, 4 + i, d);
+        lv.P[i] = (const __nv_bfloat16*)backbone_level(bb, 4 + i, d);
         lv.H[i] = d[0]; lv.W[i] = d[1];
     }
     return lv;
 }
 
-static int roi_align(mf_backbone* bb, const float* boxes, int n, int pool, void* out, cudaStream_t s)
+void mfb::roi_align(mf_backbone* bb, const float* boxes, int n, int pool, void* out)
 {
-    if (n == 0) return 0;
+    if (n == 0) return;
     int d[3];
-    mf_backbone_output(bb, 4, d);
+    backbone_level(bb, 4, d);
     const int S = d[0] * 4;
     const float areaScale = (float)((double)S * (double)S / (224.0 * 224.0));
-    k_roi_align<<<dim3(n, pool), RPN_CH / 2, 0, s>>>((const float4*)boxes, pool, roi_levels(bb), areaScale, (__nv_bfloat16*)out);
-    return cnn_check_launch("k_roi_align");
+    launch(Enq{backbone_stream(bb), nullptr}, nullptr, k_roi_align, dim3(n, pool), RPN_CH / 2, 0, (const float4*)boxes, pool, roi_levels(bb), areaScale,
+           (__nv_bfloat16*)out);
 }
 
 // the proposal layer on logits [n][2], deltas [n][4], anchors [n][4] (device) -> h->rois [1000][4], h->count
-static int propose(mf_rpn* h, const float* logits, const float* deltas, const float* anchors, int n)
+static void propose(mf_rpn* h, const float* logits, const float* deltas, const float* anchors, int n)
 {
-    const cudaStream_t s = h->s;
+    const Enq q{h->s, nullptr};
     const int k = n < RPN_PRE_NMS ? n : RPN_PRE_NMS;
     const int grid = (n + 255) / 256, histGrid = std::min((n + 2047) / 2048, 2 * num_sms());
-    k_rpn_keys<<<grid, 256, 0, s>>>((const float2*)logits, n, k, h->keys, h->st);
+    launch(q, nullptr, k_rpn_keys, grid, 256, 0, (const float2*)logits, n, k, h->keys.p, h->st.p);
     int shifts[8], np = 0;
     for (int sh = 56; sh >= 32; sh -= 8) shifts[np++] = sh;
     int idxBits = 0;
@@ -273,26 +273,44 @@ static int propose(mf_rpn* h, const float* logits, const float* deltas, const fl
     for (int sh = 24; sh >= 0; sh -= 8)
         if (sh < idxBits) shifts[np++] = sh;
     for (int p = 0; p < np; ++p) {
-        k_sel_hist<<<histGrid, 256, 0, s>>>(h->keys, n, h->st, shifts[p]);
-        k_sel_pick<<<1, 256, 0, s>>>(h->st, shifts[p]);
+        launch(q, nullptr, k_sel_hist, histGrid, 256, 0, h->keys.p, n, h->st.p, shifts[p]);
+        launch(q, nullptr, k_sel_pick, 1, 256, 0, h->st.p, shifts[p]);
     }
-    k_sel_compact<<<grid, 256, 0, s>>>(h->keys, n, h->st, h->sel);
-    k_sort_decode<<<1, 1024, SORT_CAP * sizeof(unsigned long long), s>>>(h->sel, k, (const float4*)deltas, (const float4*)anchors, h->boxes);
+    launch(q, nullptr, k_sel_compact, grid, 256, 0, h->keys.p, n, h->st.p, h->sel.p);
+    launch(q, nullptr, k_sort_decode, 1, 1024, SORT_CAP * sizeof(unsigned long long), h->sel.p, k, (const float4*)deltas, (const float4*)anchors,
+           h->boxes.p);
     const int words = (k + 63) / 64;
-    k_nms_mask<<<dim3(words, words), 64, 0, s>>>(h->boxes, k, words, h->mask);
-    k_nms_scan<<<1, 32, 0, s>>>(h->boxes, h->mask, k, words, (float4*)h->rois.p, h->count);
-    return cnn_check_launch("proposal layer");
+    launch(q, nullptr, k_nms_mask, dim3(words, words), 64, 0, h->boxes.p, k, words, h->mask.p);
+    launch(q, nullptr, k_nms_scan, 1, 32, 0, h->boxes.p, h->mask.p, k, words, (float4*)h->rois.p, h->count.p);
+}
+
+void mfb::rpn_run(mf_rpn* h, int stages)
+{
+    const cudaStream_t s = h->s;
+    if (stages & MF_RPN_CONV)
+        for (int l = 0; l < 5; ++l) {
+            int d[3];
+            const void* in = backbone_level(h->bb, 4 + l, d);
+            cnn_conv(in, d[0], d[1], RPN_CH, RPN_MID, 3, 1, 1, h->w.w(0), h->w.b(0), h->col, h->conv.p + (size_t)h->pixOff[l] * RPN_MID, 1, s);
+        }
+    if (stages & MF_RPN_HEADS) {
+        launch_gemm_bf16(h->conv, h->w.w(1), h->w.b(1), nullptr, h->head, h->pixels, RPN_HEAD_N, RPN_MID, 0, s, nullptr, true);
+        launch(Enq{s, nullptr}, nullptr, k_rpn_split, std::min((h->pixels * 18 + 255) / 256, 8 * num_sms()), 256, 0, h->head.p, h->pixels, h->logits.p,
+               h->deltas.p);
+    }
+    if (stages & MF_RPN_PROPOSALS) propose(h, h->logits, h->deltas, h->anchors, h->A);
+    if (stages & MF_RPN_ROI_ALIGN) roi_align(h->bb, h->rois, RPN_POST_NMS, RPN_POOL, h->pooled);
 }
 
 // ==========================================================================================
 // C ABI (declared in include/maskfusion_b200.h)
 // ==========================================================================================
-mf_rpn::mf_rpn(mf_backbone* bb_, unsigned seed) : bb(bb_), s((cudaStream_t)mf_backbone_stream(bb_)), w(MRCNN_RPN, seed, s)
+mf_rpn::mf_rpn(mf_backbone* bb_, unsigned seed) : bb(bb_), s(backbone_stream(bb_)), w(MRCNN_RPN, seed, s)
 {
     const LayerGeom c = mrcnn_layer(MRCNN_RPN, 0), hd = mrcnn_layer(MRCNN_RPN, 1);
     assert(c.cin == RPN_CH && c.rows == RPN_MID && hd.K == RPN_MID && hd.rows == RPN_HEAD_N);     // the shapes the kernels are compiled for
     int d[3];
-    mf_backbone_output(bb, 4, d);
+    backbone_level(bb, 4, d);
     S = d[0] * 4;
     for (int l = 0; l < 5; ++l) {
         lh[l] = S >> (l + 2);
@@ -335,7 +353,7 @@ mf_rpn::mf_rpn(mf_backbone* bb_, unsigned seed) : bb(bb_), s((cudaStream_t)mf_ba
 extern "C" mf_rpn* mf_rpn_create(mf_backbone* bb, unsigned seed)
 {
     MF_TRY
-    if (!bb) { cnn_fail("rpn: no backbone"); return nullptr; }
+    if (!bb) { mf_set_error("rpn: no backbone"); return nullptr; }
     return new mf_rpn(bb, seed);
     MF_CATCH_AS(nullptr, "rpn: ")
 }
@@ -345,47 +363,43 @@ extern "C" void mf_rpn_destroy(mf_rpn* h) { delete h; }
 extern "C" int mf_rpn_run(mf_rpn* h, int stages)
 {
     MF_TRY
-    if (!h) return cnn_fail("rpn: null handle");
-    const cudaStream_t s = h->s;
-    if (stages & MF_RPN_CONV)
-        for (int l = 0; l < 5; ++l) {
-            int d[3];
-            const void* in = mf_backbone_output(h->bb, 4 + l, d);
-            if (cnn_conv(in, d[0], d[1], RPN_CH, RPN_MID, 3, 1, 1, h->w.w(0), h->w.b(0), h->col, h->conv.p + (size_t)h->pixOff[l] * RPN_MID, 1, s)) return -2;
-        }
-    if (stages & MF_RPN_HEADS) {
-        if (launch_gemm_bf16(h->conv, h->w.w(1), h->w.b(1), nullptr, h->head, h->pixels, RPN_HEAD_N, RPN_MID, 0, s, nullptr, true)) return -2;
-        k_rpn_split<<<std::min((h->pixels * 18 + 255) / 256, 8 * num_sms()), 256, 0, s>>>(h->head, h->pixels, h->logits, h->deltas);
-        if (cnn_check_launch("k_rpn_split")) return -3;
-    }
-    if ((stages & MF_RPN_PROPOSALS) && propose(h, h->logits, h->deltas, h->anchors, h->A)) return -3;
-    if ((stages & MF_RPN_ROI_ALIGN) && roi_align(h->bb, h->rois, RPN_POST_NMS, RPN_POOL, h->pooled, s)) return -3;
+    if (!h) throw CudaError{"rpn: null handle"};
+    rpn_run(h, stages);
     return 0;
     MF_CATCH(-1)
 }
 
-extern "C" int mf_rpn_forward(mf_rpn* h) { MF_TRY return mf_rpn_run(h, MF_RPN_CONV | MF_RPN_HEADS | MF_RPN_PROPOSALS | MF_RPN_ROI_ALIGN); MF_CATCH(-1) }
+extern "C" int mf_rpn_forward(mf_rpn* h)
+{
+    MF_TRY
+    if (!h) throw CudaError{"rpn: null handle"};
+    rpn_run(h, MF_RPN_CONV | MF_RPN_HEADS | MF_RPN_PROPOSALS | MF_RPN_ROI_ALIGN);
+    return 0;
+    MF_CATCH(-1)
+}
 
 extern "C" int mf_rpn_propose(mf_rpn* h, const float* d_logits, const float* d_deltas, const float* d_anchors, int n_anchors)
 {
     MF_TRY
-    if (!h) return cnn_fail("rpn: null handle");
+    if (!h) throw CudaError{"rpn: null handle"};
     if (n_anchors < 1 || n_anchors > h->A)
-        return cnn_fail("rpn_propose: n_anchors = " + std::to_string(n_anchors) + " outside [1, " + std::to_string(h->A) + "]");
+        throw CudaError{"rpn_propose: n_anchors = " + std::to_string(n_anchors) + " outside [1, " + std::to_string(h->A) + "]"};
     if (!d_logits || !d_deltas || !d_anchors || ((uintptr_t)d_logits & 7) || ((uintptr_t)d_deltas & 15) || ((uintptr_t)d_anchors & 15))
-        return cnn_fail("rpn_propose: logits need 8-byte, deltas and anchors 16-byte aligned device pointers");
-    return propose(h, d_logits, d_deltas, d_anchors, n_anchors) ? -3 : 0;
+        throw CudaError{"rpn_propose: logits need 8-byte, deltas and anchors 16-byte aligned device pointers"};
+    propose(h, d_logits, d_deltas, d_anchors, n_anchors);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_roi_align_bf16(mf_backbone* bb, const float* d_boxes, int n, int pool, void* d_out)
 {
     MF_TRY
-    if (!bb) return cnn_fail("roi_align: no backbone");
-    if (n < 0 || pool < 2 || pool > 64) return cnn_fail("roi_align: need n >= 0 and 2 <= pool <= 64");
+    if (!bb) throw CudaError{"roi_align: no backbone"};
+    if (n < 0 || pool < 2 || pool > 64) throw CudaError{"roi_align: need n >= 0 and 2 <= pool <= 64"};
     if (n > 0 && (!d_boxes || !d_out || ((uintptr_t)d_boxes & 15) || ((uintptr_t)d_out & 3)))
-        return cnn_fail("roi_align: boxes need a 16-byte, out a 4-byte aligned device pointer");
-    return roi_align(bb, d_boxes, n, pool, d_out, (cudaStream_t)mf_backbone_stream(bb)) ? -3 : 0;
+        throw CudaError{"roi_align: boxes need a 16-byte, out a 4-byte aligned device pointer"};
+    roi_align(bb, d_boxes, n, pool, d_out);
+    return 0;
     MF_CATCH(-1)
 }
 
@@ -394,8 +408,10 @@ extern "C" int mf_rpn_num_anchors(mf_rpn* h) { return h ? h->A : -1; }
 extern "C" int mf_rpn_get_weights(mf_rpn* h, float* conv_w, float* conv_b, float* head_w, float* head_b)
 {
     MF_TRY
-    if (!h) return cnn_fail("rpn: null handle");
-    return h->w.get(0, conv_w, conv_b) || h->w.get(1, head_w, head_b, 18) ? -1 : 0;     // head rows 0..5 logits, 6..17 deltas
+    if (!h) throw CudaError{"rpn: null handle"};
+    h->w.get(0, conv_w, conv_b);
+    h->w.get(1, head_w, head_b, 18);                         // head rows 0..5 logits, 6..17 deltas
+    return 0;
     MF_CATCH(-1)
 }
 
@@ -403,40 +419,48 @@ extern "C" int mf_rpn_get_weights(mf_rpn* h, float* conv_w, float* conv_b, float
 extern "C" int mf_rpn_load_weights(mf_rpn* h, const char* path)
 {
     MF_TRY
-    return h ? h->w.load(path, h->s) : cnn_fail("rpn: null handle");
+    if (!h) throw CudaError{"rpn: null handle"};
+    h->w.load(path, h->s);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_anchors(mf_rpn* h, float* anchors)
 {
     MF_TRY
-    return h ? cnn_download(h->s, anchors, h->anchors, (size_t)h->A * 16) : cnn_fail("rpn: null handle");
+    if (!h) throw CudaError{"rpn: null handle"};
+    cnn_read_back(h->s, anchors, h->anchors, (size_t)h->A * 16);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_head_outputs(mf_rpn* h, float* logits, float* deltas)
 {
     MF_TRY
-    if (!h) return cnn_fail("rpn: null handle");
-    return cnn_download(h->s, logits, h->logits, (size_t)h->A * 8) || cnn_download(h->s, deltas, h->deltas, (size_t)h->A * 16) ? -1 : 0;
+    if (!h) throw CudaError{"rpn: null handle"};
+    cnn_read_back(h->s, logits, h->logits, (size_t)h->A * 8);
+    cnn_read_back(h->s, deltas, h->deltas, (size_t)h->A * 16);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_download_conv(mf_rpn* h, int level, void* host_bf16)
 {
     MF_TRY
-    if (!h) return cnn_fail("rpn: null handle");
-    if (level < 0 || level > 4) return cnn_fail("rpn: level must be 0..4 (P2..P6)");
-    return cnn_download(h->s, host_bf16, h->conv.p + (size_t)h->pixOff[level] * RPN_MID, (size_t)h->lh[level] * h->lh[level] * RPN_MID * 2);
+    if (!h) throw CudaError{"rpn: null handle"};
+    if (level < 0 || level > 4) throw CudaError{"rpn: level must be 0..4 (P2..P6)"};
+    cnn_read_back(h->s, host_bf16, h->conv.p + (size_t)h->pixOff[level] * RPN_MID, (size_t)h->lh[level] * h->lh[level] * RPN_MID * 2);
+    return 0;
     MF_CATCH(-1)
 }
 
 extern "C" int mf_rpn_get_proposals(mf_rpn* h, float* rois)
 {
     MF_TRY
+    if (!h) throw CudaError{"rpn: null handle"};
     int n = 0;
-    if (!h) return cnn_fail("rpn: null handle");
-    if (cnn_download(h->s, rois, h->rois, RPN_POST_NMS * 16) || cnn_download(h->s, &n, h->count, 4)) return -1;
+    cnn_read_back(h->s, rois, h->rois, RPN_POST_NMS * 16);
+    cnn_read_back(h->s, &n, h->count, 4);
     return n;
     MF_CATCH(-1)
 }
@@ -444,7 +468,9 @@ extern "C" int mf_rpn_get_proposals(mf_rpn* h, float* rois)
 extern "C" int mf_rpn_get_pooled(mf_rpn* h, void* host_bf16)
 {
     MF_TRY
-    return h ? cnn_download(h->s, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2) : cnn_fail("rpn: null handle");
+    if (!h) throw CudaError{"rpn: null handle"};
+    cnn_read_back(h->s, host_bf16, h->pooled, (size_t)RPN_POST_NMS * RPN_POOL * RPN_POOL * RPN_CH * 2);
+    return 0;
     MF_CATCH(-1)
 }
 

@@ -422,28 +422,26 @@ WeightStore::WeightStore(int part_, unsigned seed, cudaStream_t s) : part(part_)
     cudaCheck(upload(*this, hW, hB, s), "weight upload");
 }
 
-int WeightStore::load(const char* path, cudaStream_t s)
+void WeightStore::load(const char* path, cudaStream_t s)
 {
     const std::vector<LayerSpec>& t = specs(part);
     std::vector<float> w(hW.size()), b(hB.size());
     WeightFile f;
     bool ok = f.open(path);
     for (size_t i = 0; ok && i < t.size(); ++i) ok = f.fold(t[i], &w[wOff[i]], &b[bOff[i]]);
-    if (!ok) return cnn_fail(f.err);
+    if (!ok) throw CudaError{f.err};
     const cudaError_t e = upload(*this, w, b, s);
-    if (e != cudaSuccess) { cnn_fail(std::string(HANDLE_NAME[part]) + ": weight upload: " + cudaGetErrorString(e)); return -2; }
+    if (e != cudaSuccess) throw CudaError{std::string(HANDLE_NAME[part]) + ": weight upload: " + cudaGetErrorString(e)};
     hW.swap(w); hB.swap(b);
-    return 0;
 }
 
-int WeightStore::get(int i, float* w, float* b, int rows) const
+void WeightStore::get(int i, float* w, float* b, int rows) const
 {
-    if (i < 0 || i >= (int)wOff.size()) return cnn_fail(std::string(HANDLE_NAME[part]) + ": bad layer index");
+    if (i < 0 || i >= (int)wOff.size()) throw CudaError{std::string(HANDLE_NAME[part]) + ": bad layer index"};
     const LayerSpec& l = specs(part)[i];
     if (rows < 0) rows = l.rows;
     if (w) memcpy(w, &hW[wOff[i]], (size_t)rows * l.K * sizeof(float));
     if (b) memcpy(b, &hB[bOff[i]], (size_t)rows * sizeof(float));
-    return 0;
 }
 
 }  // namespace mfb
@@ -458,9 +456,9 @@ extern "C" int mf_mrcnn_read_layer(const char* path, const char* layer, float* w
             if (dims) { dims[0] = s.rows; dims[1] = s.K; }
             if (!w_rows_K || !bias_rows) return 0;
             WeightFile f;
-            if (!f.open(path) || !f.fold(s, w_rows_K, bias_rows)) return mfb::cnn_fail(f.err);
+            if (!f.open(path) || !f.fold(s, w_rows_K, bias_rows)) throw mfb::CudaError{f.err};
             return 0;
         }
-    return mfb::cnn_fail(std::string("mrcnn_read_layer: no layer named '") + (layer ? layer : "(null)") + "'");
+    throw mfb::CudaError{std::string("mrcnn_read_layer: no layer named '") + (layer ? layer : "(null)") + "'"};
     MF_CATCH(-1)
 }

@@ -109,6 +109,44 @@ def test_every_family_reports_through_one_slot(product_lib, tmp_path):
                                         [-2, "not a JPEG stream"]]
 
 
+_MRCNN = r"""
+import ctypes as C, json
+import maskfusion_b200 as mfb
+L = mfb.load_library()
+i6 = (C.c_int * 6)()
+calls = [
+    lambda: L.mf_backbone_create(100, 0, None), lambda: L.mf_rpn_create(None, 0), lambda: L.mf_detector_create(None, 0),
+    lambda: L.mf_gemm_bf16(None, None, None, None, None, 0, 64, 64, 0, None),
+    lambda: L.mf_backbone_num_layers(None), lambda: L.mf_backbone_get_weights(None, 0, None, None),
+    lambda: L.mf_backbone_load_weights(None, b"x"), lambda: L.mf_backbone_mold(None, None, 640, 480), lambda: L.mf_backbone_forward(None, None),
+    lambda: L.mf_backbone_layer(None, 0, i6), lambda: L.mf_backbone_download(None, 4, None),
+    lambda: L.mf_rpn_run(None, 15), lambda: L.mf_rpn_forward(None), lambda: L.mf_rpn_propose(None, None, None, None, 1),
+    lambda: L.mf_rpn_get_weights(None, None, None, None, None), lambda: L.mf_rpn_load_weights(None, b"x"), lambda: L.mf_rpn_get_anchors(None, None),
+    lambda: L.mf_rpn_get_head_outputs(None, None, None), lambda: L.mf_rpn_download_conv(None, 0, None), lambda: L.mf_rpn_get_proposals(None, None),
+    lambda: L.mf_rpn_get_pooled(None, None),
+    lambda: L.mf_roi_align_bf16(None, None, 1, 7, None),
+    lambda: L.mf_detector_run(None, 15), lambda: L.mf_detector_forward(None, 640, 480), lambda: L.mf_detector_detect(None, None, 640, 480),
+    lambda: L.mf_detector_set_export(None, 0.5, None, 0, None, 0), lambda: L.mf_detector_refine(None, None, None, None, 1),
+    lambda: L.mf_detector_paste(None, None, None, 640, 480), lambda: L.mf_detector_load_weights(None, b"x"),
+    lambda: L.mf_detector_get_fc(None, None, None), lambda: L.mf_detector_get_head_outputs(None, None, None),
+    lambda: L.mf_detector_get_mask_layer(None, 0, None), lambda: L.mf_detector_get_detections(None, None), lambda: L.mf_detector_get_masks(None, None),
+    lambda: L.mf_detector_get_id_image(None, None, None, None), lambda: L.mf_detector_image_size(None, None, None),
+    lambda: L.mf_detector_layer(None, 0, i6), lambda: L.mf_detector_get_weights(None, 0, None, None),
+]
+print(json.dumps([[call(), L.mf_last_error().decode()] for call in calls]))
+"""
+
+
+def test_mask_rcnn_refusals_without_a_device(product_lib):
+    """every Mask R-CNN entry point that can fail, refused before device work: return code and text, as the library has always given them"""
+    want = [[None, "input size must be a multiple of 64 (mrcnn: IMAGE_MAX_DIM=1024)"], [None, "rpn: no backbone"],
+            [None, "detector: no region-proposal handle"], [-2, "gemm: need M > 0, and K > 0 and N > 0 multiples of 64"]]
+    want += [[-1, "backbone: null handle"]] * 5 + [[-1, "backbone: bad layer index"], [-1, "backbone: no handle or level outside 0..8"]]
+    want += [[-1, "rpn: null handle"]] * 10 + [[-1, "roi_align: no backbone"]]
+    want += [[-1, "detector: null handle"]] * 14 + [[-1, "detector: bad layer index"]] * 2
+    assert _child(_MRCNN) == want
+
+
 _THREADS = r"""
 import ctypes as C, json, threading
 import maskfusion_b200 as mfb
