@@ -12,7 +12,7 @@
 using namespace mfb;
 namespace mfb { bool decodeJPEG(const uint8_t* data, size_t size, int& W, int& H, std::vector<uint8_t>& rgb, std::string& err); }   // mf_jpeg.cu
 
-struct mf_context { MaskFusion* mf; };
+struct mf_context { std::unique_ptr<MaskFusion> mf; };
 
 // one message per calling thread: contexts and Mask R-CNN handles driven from different threads never see each other's errors
 static thread_local std::string g_err;
@@ -68,12 +68,11 @@ extern "C" mf_context* mf_create(const mf_config* cfg, int device, void* stream)
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n == 0) { mf_set_error(std::string("no CUDA device: this library has no CPU fallback (") + cudaGetErrorString(e) + ")"); return nullptr; }
-    mf_context* c = new mf_context;
-    c->mf = new MaskFusion(*cfg, device, (cudaStream_t)stream);
-    return c;
+    std::unique_ptr<MaskFusion> mf(new MaskFusion(*cfg, device, (cudaStream_t)stream));
+    return new mf_context{std::move(mf)};
     MF_CATCH(nullptr)
 }
-extern "C" void mf_destroy(mf_context* ctx) { if (ctx) { delete ctx->mf; delete ctx; } }
+extern "C" void mf_destroy(mf_context* ctx) { delete ctx; }
 
 extern "C" int mf_process_frame(mf_context* ctx, const uint8_t* rgb, const float* depth, int64_t ts, const uint8_t* mask, const float* in_pose,
                                 float weight_multiplier, int bootstrap)
@@ -116,7 +115,7 @@ extern "C" int mf_model_surfel_count(mf_context* ctx, int i) { MF_TRY MF_NEED(ct
 extern "C" int mf_download_surfels(mf_context* ctx, int i, float* out, int max_surfels)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     uint32_t n = m->lastCount();
     if ((int)n > max_surfels) n = (uint32_t)max_surfels;
     if (!n) return 0;
@@ -130,7 +129,7 @@ extern "C" int mf_download_surfels(mf_context* ctx, int i, float* out, int max_s
 extern "C" int mf_upload_surfels(mf_context* ctx, int i, const float* in, int n)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (n < 0 || (uint32_t)n > m->capacity) { mf_set_error("upload exceeds model capacity"); return -4; }
     if (n) {
         DevBuf<float4> tmp; tmp.alloc((size_t)n * 3);
@@ -185,7 +184,7 @@ extern "C" int mf_export_poses(mf_context* ctx, const char* export_dir)
 extern "C" int mf_set_frame(mf_context* ctx, const uint8_t* rgb, const float* depth, const uint8_t* mask)
 {
     MF_TRY MF_NEED(ctx) MF_UNQUEUED(ctx, "set_frame")
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (!mask) o->mask.zero(o->stream);
     o->setFrame(rgb, depth, mask, false);
     o->generateCUDATextures();
@@ -249,12 +248,12 @@ static void planarOut(MaskFusion* o, const float4* map, int P, float* out)
 }
 extern "C" int mf_download_filtered_depth(mf_context* ctx, float* out)
 {
-    MF_TRY MF_NEED(ctx) d2h(ctx->mf, out, ctx->mf->depthFilt, ctx->mf->P); ctx->mf->sync(); return 0; MF_CATCH(-1)
+    MF_TRY MF_NEED(ctx) d2h(ctx->mf.get(), out, ctx->mf->depthFilt, ctx->mf->P); ctx->mf->sync(); return 0; MF_CATCH(-1)
 }
 extern "C" int mf_download_frame_maps(mf_context* ctx, int level, float* depth, float* vmap, float* nmap)
 {
     MF_TRY MF_NEED(ctx)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (level < 0 || level > 2) { mf_set_error("level out of range"); return -2; }
     int Pl = (o->W >> level) * (o->H >> level);
     d2h(o, depth, level == 0 ? o->depthFilt : o->depthPyr[level].p, Pl); o->sync();
@@ -266,7 +265,7 @@ extern "C" int mf_download_frame_maps(mf_context* ctx, int level, float* depth, 
 extern "C" int mf_download_model_maps(mf_context* ctx, int i, int level, float* vmap, float* nmap)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (level < 0 || level > 2) { mf_set_error("level out of range"); return -2; }
     int Pl = (o->W >> level) * (o->H >> level);
     planarOut(o, m->vmapG[level], Pl, vmap);
@@ -277,7 +276,7 @@ extern "C" int mf_download_model_maps(mf_context* ctx, int i, int level, float* 
 extern "C" int mf_download_index_map(mf_context* ctx, int i, uint32_t* idx, float* vc, float* ct, float* nr)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     m->flushIndex();
     d2h(o, idx, m->idx.p, o->P); d2h(o, vc, m->vertConf.p, o->P); d2h(o, ct, m->colorTime.p, o->P); d2h(o, nr, m->normRad.p, o->P);
     o->sync(); return 0;
@@ -286,7 +285,7 @@ extern "C" int mf_download_index_map(mf_context* ctx, int i, uint32_t* idx, floa
 extern "C" int mf_download_prediction(mf_context* ctx, int i, uint8_t* image4, float* vc, float* nr, uint16_t* time)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     d2h(o, image4, m->splatImage.p, o->P); d2h(o, vc, m->splatVertex.p, o->P); d2h(o, nr, m->splatNormal.p, o->P); d2h(o, time, m->splatTime.p, o->P);
     o->sync(); return 0;
     MF_CATCH(-1)
@@ -294,7 +293,7 @@ extern "C" int mf_download_prediction(mf_context* ctx, int i, uint8_t* image4, f
 extern "C" int mf_download_fill_in(mf_context* ctx, int i, uint8_t* image4, float* v4, float* n4)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (!m->fillIn) { mf_set_error("model has no fill-in textures"); return -5; }
     d2h(o, image4, m->fillImage.p, o->P); d2h(o, v4, m->fillVertex.p, o->P); d2h(o, n4, m->fillNormal.p, o->P);
     o->sync(); return 0;
@@ -303,7 +302,7 @@ extern "C" int mf_download_fill_in(mf_context* ctx, int i, uint8_t* image4, floa
 extern "C" int mf_download_association(mf_context* ctx, int i, uint8_t* flag, uint32_t* best, float* meas12)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     d2h(o, flag, m->aflag.p, o->P); d2h(o, best, m->abest.p, o->P);
     if (meas12) {
         DevBuf<float4> tmp; tmp.alloc((size_t)o->P * 3);
@@ -317,7 +316,7 @@ extern "C" int mf_download_association(mf_context* ctx, int i, uint8_t* flag, ui
 extern "C" int mf_download_track_stats(mf_context* ctx, int i, double* A36, double* b6, float* err6)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     TrackState st;
     cudaCheck(cudaMemcpyAsync(&st, m->trackState.p, sizeof st, cudaMemcpyDeviceToHost, o->stream), "D2H");
     o->sync();
@@ -330,7 +329,7 @@ extern "C" int mf_download_track_stats(mf_context* ctx, int i, double* A36, doub
 extern "C" int mf_download_edge_map(mf_context* ctx, float* edge, uint8_t* binary)
 {
     MF_TRY MF_NEED(ctx)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     o->edgeMaps();
     d2h(o, edge, o->edgeMap.p, o->P); d2h(o, binary, o->edgeInv.p, o->P);
     o->sync(); return 0;
@@ -345,7 +344,7 @@ extern "C" int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int i
 {
     MF_TRY MF_NEED(ctx)
     if (!image || radius < 0 || iterations < 0) { mf_set_error("morph_close: bad arguments"); return -3; }
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     DevBuf<uint8_t> a, b, c; a.alloc(o->P); b.alloc(o->P); c.alloc(o->P);
     cudaCheck(cudaMemcpyAsync(a.p, image, o->P, cudaMemcpyHostToDevice, o->stream), "H2D");
     if (ellipse) launch_morph_close_ellipse(a, b, o->W, o->H, radius, iterations, nullptr, o->on());
@@ -377,7 +376,7 @@ extern "C" int mf_attach_detector(mf_context* ctx, mf_detector* detector, int ev
 extern "C" int mf_download_frame_masks(mf_context* ctx, uint8_t* mask, int32_t* class_ids_256, int* n_masks)
 {
     MF_TRY MF_NEED(ctx)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (!o->cfg.enableMultipleModels) { mf_set_error("not a multi-model context"); return -5; }
     // a queued frame popped by an in_pose call was detected at push time but does not segment, so nothing has waited for its hand-off yet
     o->waitHandoff(o->stream);
@@ -406,7 +405,7 @@ extern "C" int mf_set_frame_classes(mf_context* ctx, const int32_t* class_ids, i
 extern "C" int mf_download_segmentation(mf_context* ctx, uint8_t* mask, uint8_t* projected_ids)
 {
     MF_TRY MF_NEED(ctx)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     d2h(o, mask, o->mask.p, o->P);
     if (projected_ids) { if (!o->projectedIDs.p) { mf_set_error("not a multi-model context"); return -5; } d2h(o, projected_ids, o->projectedIDs.p, o->P); }
     o->sync(); return 0;
@@ -448,7 +447,7 @@ extern "C" int mf_shard_process_frame(mf_context* ctx, const uint8_t* rgb, const
                                       int n_class_ids, float weight_multiplier, int inputs_on_device)
 {
     MF_TRY MF_NEED(ctx)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (!o->shardNccl) { mf_set_error("mf_shard_process_frame needs a communicator (mf_shard_comm_init)"); return -2; }
     if (o->rank == 0) {
         if (!rgb || !depth || ts < 0) { mf_set_error("processFrame: rgb/depth must be non-null and timestamp >= 0 on the loader rank"); return -3; }
@@ -463,7 +462,7 @@ extern "C" int mf_shard_stats(mf_context* ctx, int64_t* out4)
 {
     MF_TRY
     if (!ctx || !ctx->mf || !out4) { mf_set_error("null argument"); return -1; }
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     out4[0] = (int64_t)o->shard.bytesMoved; out4[1] = o->shard.calls; out4[2] = o->shardNccl ? o->shard.world : 0; out4[3] = o->shard.version;
     return 0;
     MF_CATCH(-1)
@@ -532,7 +531,7 @@ extern "C" int mf_debug_set_poses(mf_context* ctx, int i, const float* pose16, c
 extern "C" int mf_icp_step(mf_context* ctx, int i, int level, const float* Rcurr9, const float* tcurr3, float* out29)
 {
     MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf;
+    MaskFusion* o = ctx->mf.get();
     if (level < 0 || level > 2) { mf_set_error("level out of range"); return -2; }
     TrackPoses pp; memset(&pp, 0, sizeof pp);
     memcpy(pp.p[0], Rcurr9, 9 * sizeof(float)); memcpy(pp.p[0] + 9, tcurr3, 3 * sizeof(float));

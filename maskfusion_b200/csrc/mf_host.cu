@@ -23,7 +23,7 @@ void Enq::mark(const char* name) const
     if (!rec || !rec->prof.on) return;
     Profiler* p = &rec->prof;
     if (p->used == (int)p->events.size()) {
-        cudaEvent_t e; cudaEventCreate(&e); p->events.push_back(e); p->names.push_back(nullptr);
+        Event e; e.create(cudaEventDefault); p->events.push_back(std::move(e)); p->names.push_back(nullptr);
     }
     p->names[p->used] = name;
     cudaEventRecord(p->events[p->used], s);
@@ -131,8 +131,8 @@ Model::Model(MaskFusion* o, unsigned char id_, float conf, bool enableFillIn, in
     // in-place clean: ONE copy of the store; Model::clean allocates the second plane set when it first needs the copy
     pos[0].alloc(capacity); col[0].alloc(capacity); nrm[0].alloc(capacity);
     count.alloc(2); count.zero(s);
-    cudaCheck(cudaMallocHost((void**)&hCount, 2 * sizeof(uint32_t)), "cudaMallocHost"); hCount[0] = hCount[1] = 0;
-    cudaCheck(cudaMallocHost((void**)&hTrackOut, 40 * sizeof(float)), "cudaMallocHost");
+    hCount.alloc(2);
+    hTrackOut.alloc(40);
     key.alloc(P); launch_fill_u64(key, KEY_EMPTY, P, o->on());
     idx.alloc(P); vertConf.alloc(P); colorTime.alloc(P); normRad.alloc(P); cleanTex.alloc((size_t)P); cleanTex.zero(s);
     idx.zero(s); vertConf.zero(s); colorTime.zero(s); normRad.zero(s);
@@ -147,7 +147,7 @@ Model::Model(MaskFusion* o, unsigned char id_, float conf, bool enableFillIn, in
     size_t nblk = ((size_t)capacity + P + 511) / 512 + 1;
     blockSums.alloc(nblk); blockSums2.alloc(nblk);
     cleanTicket.alloc(4); cleanTicket.zero(s); cleanLoaded.alloc(nblk); cleanLoaded.zero(s);
-    cudaCheck(cudaMallocHost((void**)&hCleanStat, 2 * sizeof(uint32_t)), "cudaMallocHost"); hCleanStat[0] = hCleanStat[1] = 0;
+    hCleanStat.alloc(2);
     cand.alloc((size_t)capacity + P); candCount.alloc(1); candCount.zero(s);
     for (int l = 0; l < 3; ++l) {
         size_t Pl = (size_t)(W >> l) * (H >> l);
@@ -165,13 +165,6 @@ void Model::pushPose()
 {
     if (!owned || !dpose.p) return;          // ghosts hold no device state; during construction the buffer appears last
     launch_set_pose(dpose, pose.m, lastPose.m, owner->on());
-}
-
-Model::~Model()
-{
-    if (hCount) cudaFreeHost(hCount);
-    if (hTrackOut) cudaFreeHost(hTrackOut);
-    if (hCleanStat) cudaFreeHost(hCleanStat);
 }
 
 unsigned Model::lastCount()
@@ -320,17 +313,14 @@ MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), d
     W = c.width; H = c.height; P = W * H;
     if (W % 4 || H % 4) throw CudaError{"width and height must be multiples of 4 (3-level pyramid)"};
     cam = Cam{c.fx, c.fy, c.cx, c.cy};
-    ownStream = (st == nullptr);
-    if (ownStream) cudaCheck(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking), "cudaStreamCreate"); else stream = st;
+    if (st) stream = st;
+    else { ownedStream.create(); stream = ownedStream; }
     for (int k = 0; k < 2; ++k) { ring.emplace_back(new FrameSlot(packetBytes(), stream)); rgbBuf[k].alloc(P); depthFiltBuf[k].alloc(P); }
     selectSlot(0); selectSet(0);
-    cudaCheck(cudaEventCreateWithFlags(&retired, cudaEventDisableTiming), "cudaEventCreate");
+    retired.create();
     mask.alloc(P); mask.zero(stream);
-    cudaCheck(cudaStreamCreateWithFlags(&preStream, cudaStreamNonBlocking), "cudaStreamCreate");
-    cudaCheck(cudaEventCreateWithFlags(&preDone, cudaEventDisableTiming), "cudaEventCreate");
-    cudaCheck(cudaEventCreateWithFlags(&inputsCopied, cudaEventDisableTiming), "cudaEventCreate");
-    cudaCheck(cudaEventCreateWithFlags(&evMain, cudaEventDisableTiming), "cudaEventCreate");
-    cudaCheck(cudaEventCreateWithFlags(&evComm, cudaEventDisableTiming), "cudaEventCreate");
+    preStream.create();
+    preDone.create(); inputsCopied.create(); evMain.create(); evComm.create(); trackDone.create();
     for (int l = 0; l < 3; ++l) {
         size_t Pl = (size_t)(W >> l) * (H >> l);
         if (l > 0) depthPyr[l].alloc(Pl);
@@ -338,14 +328,14 @@ MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), d
     }
     edgeMap.alloc(P); edgeBinary.alloc(P); edgeBuf.alloc(P); edgeInv.alloc(P);
     dJobs.alloc(TRACK_MAX_JOBS);
-    cudaCheck(cudaMallocHost((void**)&hJobs, TRACK_MAX_JOBS * sizeof(TrackJob)), "cudaMallocHost");
+    hJobs.alloc(TRACK_MAX_JOBS);
     initFlagR.alloc(P); initFlagF.alloc(P);
     scratch.alloc((size_t)P * 4);
     rayTab.alloc(P); launch_ray_table(cam, W, H, rayTab, on());
     if (c.enableMultipleModels) {
         dRes.alloc(1); dRes.zero(stream);
-        cudaCheck(cudaMallocHost((void**)&hRes, sizeof(FrameResult)), "cudaMallocHost"); memset(hRes, 0, sizeof(FrameResult));
-        cudaCheck(cudaEventCreateWithFlags(&resEvt, cudaEventDisableTiming), "cudaEventCreate");
+        hRes.alloc(1);
+        resEvt.create();
         poseTable.alloc((size_t)MF_MAX_MODELS * 32); poseTable.zero(stream);
         gathered.alloc((size_t)64 * MF_MAX_MODELS * 32); gathered.zero(stream);
         // component histograms for the worst case (every second pixel its own component): the counts of a frame live on the device
@@ -367,40 +357,14 @@ MaskFusion::~MaskFusion()
 {
     for (auto& f : ring) if (f->netUsed) cudaEventSynchronize(f->netDone);    // a network still reading a slot or writing its hand-off into one
     cudaStreamSynchronize(stream);
-    for (cudaEvent_t e : rec.prof.events) cudaEventDestroy(e);
-    if (trackDone) cudaEventDestroy(trackDone);
-    if (preStream) { cudaStreamSynchronize(preStream); cudaStreamDestroy(preStream); }
-    if (preDone) cudaEventDestroy(preDone);
-    if (inputsCopied) cudaEventDestroy(inputsCopied);
-    if (evMain) cudaEventDestroy(evMain);
-    if (evComm) cudaEventDestroy(evComm);
-    models.clear();
-    inactiveModels.clear();
-    if (hJobs) cudaFreeHost(hJobs);
-    if (hRes) cudaFreeHost(hRes);
-    if (resEvt) cudaEventDestroy(resEvt);
-    if (retired) cudaEventDestroy(retired);
-    ring.clear();
-    if (ownStream) cudaStreamDestroy(stream);
+    cudaStreamSynchronize(preStream);
+    // the members' owners then release every stream, event and buffer the context holds
 }
 
 MaskFusion::FrameSlot::FrameSlot(size_t bytes, cudaStream_t s)
 {
-    try {
-        cudaCheck(cudaEventCreateWithFlags(&uploaded, cudaEventDisableTiming), "cudaEventCreate");
-        cudaCheck(cudaEventCreateWithFlags(&netDone, cudaEventDisableTiming), "cudaEventCreate");
-        packet.alloc(bytes); packet.zero(s);
-    } catch (...) {
-        destroyEvents();            // the destructor of a partly constructed slot does not run
-        throw;
-    }
-}
-MaskFusion::FrameSlot::~FrameSlot() { destroyEvents(); }
-void MaskFusion::FrameSlot::destroyEvents()
-{
-    if (uploaded) cudaEventDestroy(uploaded);
-    if (netDone) cudaEventDestroy(netDone);
-    uploaded = netDone = nullptr;
+    uploaded.create(); netDone.create();
+    packet.alloc(bytes); packet.zero(s);
 }
 
 // MaskFusion::frameQueue with queueLength (-frameQ, MaskFusion.cpp:37,206-209): before the first frame, in one process
@@ -416,7 +380,6 @@ void MaskFusion::setFrameQueue(int length)
         try {
             for (size_t k = 1; k < n; ++k) fresh.emplace_back(new FrameSlot(packetBytes(), stream));
         } catch (const CudaError& e) {
-            fresh.clear();
             cudaGetLastError();
             throw CudaError{"setFrameQueue: cannot allocate " + std::to_string(n) + " frame slots of " + std::to_string(packetBytes()) + " bytes (" + e.what + ")"};
         }
@@ -554,7 +517,6 @@ void MaskFusion::trackModels(const std::vector<Model*>& ms, bool viaResult)
             cudaCheck(cudaMemcpyAsync(m->lastNextImage2, nextImage[2], (size_t)(W >> 2) * (H >> 2), cudaMemcpyDeviceToDevice, stream), "so3 swap");
     }
     if (viaResult) return;
-    if (!trackDone) cudaCheck(cudaEventCreateWithFlags(&trackDone, cudaEventDisableTiming), "cudaEventCreate");
     cudaCheck(cudaEventRecord(trackDone, stream), "cudaEventRecord");
     pendingModels = ms; pendingTrack = true;
 }

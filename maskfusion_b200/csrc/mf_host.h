@@ -27,7 +27,7 @@ Rt toRt(const Mat4& T);
 // in-stream stage timer: one CUDA event per mark; the interval up to the next mark is attributed to the mark's name.  Off by default.
 struct Profiler {
     bool on = false; int used = 0;
-    std::vector<cudaEvent_t> events; std::vector<const char*> names;
+    std::vector<Event> events; std::vector<const char*> names;     // events created with timing enabled
     std::map<std::string, std::pair<long, double>> acc;      // name -> (count, total ms)
     void resolve();
 };
@@ -42,6 +42,9 @@ class MaskFusion;
 // object-sharded mode: NCCL communicator of the ranks that share one replay (mf_sched.cu; libnccl is opened at run time)
 struct ShardComm {
     void* comm = nullptr; int rank = 0, world = 1, version = 0; size_t bytesMoved = 0; long calls = 0;
+    ShardComm() {}
+    ShardComm(const ShardComm&) = delete;
+    ShardComm& operator=(const ShardComm&) = delete;
     ~ShardComm();
     void init(const unsigned char* id128, int rank, int world);
     void broadcast(void* buf, size_t bytes, int root, cudaStream_t s);                               // frame packet (MaskFusion.cpp:212-217)
@@ -57,7 +60,6 @@ class Model {
 public:
     // ghost = replica of a model whose surfel store lives on another rank (SURVEY 8e): pose, ids and age only, no device buffers
     Model(MaskFusion* owner, unsigned char id, float confidenceThresh, bool enableFillIn, int capacity, int ownerRank = 0, bool ghost = false);
-    ~Model();
     Model(const Model&) = delete;
 
     // ---- reference API (Core/Model/Model.h:128-164) ----
@@ -89,7 +91,7 @@ public:
     int target = 0, countSel = 0;
     DevBuf<float4> pos[2], col[2], nrm[2];
     DevBuf<uint32_t> count;                 // [2] ping-pong, device-resident (no host round trip in the loop)
-    uint32_t* hCount = nullptr;             // pinned mirror
+    HostBuf<uint32_t> hCount;               // pinned mirror
     // index map
     DevBuf<uint64_t> key;
     DevBuf<uint32_t> idx; DevBuf<float4> vertConf, colorTime, normRad, cleanTex;
@@ -99,7 +101,7 @@ public:
     // association
     DevBuf<uint8_t> aflag; DevBuf<uint32_t> abest; DevBuf<float4> meas[3]; DevBuf<uint32_t> slot;
     DevBuf<uint8_t> keep; DevBuf<uint32_t> blockSums, blockSums2, cand, candCount;
-    uint32_t* hCleanStat = nullptr;          // pinned: {first moved sub-block, sub-blocks} of the previous clean (adaptive in-place / copy choice)
+    HostBuf<uint32_t> hCleanStat;            // pinned: {first moved sub-block, sub-blocks} of the previous clean (adaptive in-place / copy choice)
     DevBuf<uint32_t> cleanTicket, cleanLoaded; uint32_t cleanEpoch = 0;     // in-place compaction of Model::clean: [0] ticket, [1] first moved sub-block; published epochs
     // tracking
     DevBuf<float4> vmapG[3], nmapG[3], cloud[3];
@@ -108,7 +110,7 @@ public:
     DevBuf<uint32_t> validBits[3];           // object models: validity bitmask of nmapG (see k_valid_bits3)
     DevBuf<TrackState> trackState; DevBuf<float> partial;
     DevBuf<DevPose> dpose;                  // what every kernel reads: pose, inverse, fusion weight (device resident)
-    float* hTrackOut = nullptr;             // pinned: pose(16) transform(16) stats(8)
+    HostBuf<float> hTrackOut;               // pinned: pose(16) transform(16) stats(8)
     Mat4 lastTransform;
     std::vector<double> poseLog;            // 8 doubles per entry
     bool tracked = false;                   // took part in the tracking launch of the frame in flight (deferred bookkeeping)
@@ -141,7 +143,7 @@ public:
     // picked up (finalisePending) by the next processFrame / getPose / sync; the multi-model schedule finalises inside the frame.
     void finalisePending();
     void logPoses(int64_t timestamp);
-    bool pendingTrack = false, pendingLog = false; int64_t pendingTimestamp = 0; std::vector<Model*> pendingModels; cudaEvent_t trackDone = nullptr;
+    bool pendingTrack = false, pendingLog = false; int64_t pendingTimestamp = 0; std::vector<Model*> pendingModels; Event trackDone;
     // ---- multi-model path (MaskFusion.cpp:287-375) ----
     void globalProjection();                                                                      // GlobalProjection::project + downloadDirect (stays on the device)
     void checkModelCount() const;                                                                 // the ID projection and segmentation hold up to 63 models
@@ -177,12 +179,12 @@ public:
     // Mask R-CNN backbone on the frame path (MaskRCNN::executeSequential, MaskRCNN.cpp:147-151, is called from MfSegmentation.cpp:130):
     // every k-th frame the RGB image is letter-boxed into the backbone's input and the ResNet-101-FPN forward is enqueued on the
     // backbone's own stream, next to the dense pipeline of the same GPU (the reference runs its network as a ~5 Hz sidecar)
-    mf_backbone* backbone = nullptr; int backboneEvery = 0;
+    mf_backbone* backbone = nullptr; int backboneEvery = 0;      // borrowed: the caller owns the handle and its stream
     void attachBackbone(mf_backbone* bb, int everyK);
     // Mask R-CNN detector on the frame path (MfSegmentation.cpp:128-131): a segmentation frame that the caller gave no mask runs the
     // detector every k-th tick on the detector's (= its backbone's) stream; k_frame_masks writes the id image and class list into the
     // frame's mask / header in its slot; the main stream waits (the slot's netDone) just before segmentation reads them.
-    mf_detector* detector = nullptr; int detectorEvery = 0;
+    mf_detector* detector = nullptr; int detectorEvery = 0;      // borrowed: the caller owns the handle and its stream
     void attachDetector(mf_detector* det, int everyK);
     // the backbone and the detector share one network stream and read one RGBA copy of the frame (netRGBA, unpacked on that stream)
     void attachNetwork(const char* who, bool asDetector, mf_detector* det);
@@ -198,11 +200,11 @@ public:
     void attachShardDetector(mf_detector* det, int everyK, int detectorRank);
     bool shardFrameMasks(void** ptr, size_t* bytes);            // external transport: the range to broadcast from detRank on this frame
     // overlapped frames run the inputs / preprocessing (and, sharded, every collective) on preStream (MaskFusion::processFrame)
-    bool spawnedInApply = false, commOnPre = false; cudaEvent_t evMain = nullptr, evComm = nullptr;
+    bool spawnedInApply = false, commOnPre = false; Event evMain, evComm;
     void waitMain(cudaStream_t s);                              // `s` waits for the work queued on the main stream so far
     cudaStream_t commStream();                                  // the stream of the next collective, ordered behind the main stream
     void joinComm(bool now);                                    // the main stream waits for it: now, or where segmentation reads the mask
-    FrameResult* hRes = nullptr; DevBuf<FrameResult> dRes; cudaEvent_t resEvt = nullptr; bool pendingResult = false;
+    HostBuf<FrameResult> hRes; DevBuf<FrameResult> dRes; Event resEvt; bool pendingResult = false;
     DevBuf<float> poseTable, gathered;
     float fWeight = 1.f; int fTick = 0; bool fTracked = false;
     std::vector<std::unique_ptr<Model>> inactiveModels;        // MaskFusion::inactiveModels (MaskFusion.cpp:699-713): kept for exportPoses / savePly
@@ -212,7 +214,9 @@ public:
     int rank = 0, world = 1;
     int64_t fTimestamp = 0; Mat4 fInPose; bool fHasPose = false, fBootstrap = false;
 
-    mf_config cfg; Cam cam; int W, H, P; int device; cudaStream_t stream; bool ownStream;
+    mf_config cfg; Cam cam; int W, H, P; int device;
+    cudaStream_t stream;                    // the main stream: the caller's (borrowed) or ownedStream
+    Stream ownedStream;
     int numSMs = 132;
     int tick = 1;
     LaunchRecord rec;
@@ -229,22 +233,20 @@ public:
     // writes its hand-off into the frame's own slot.  The filtered depth and the RGBA copy are derived per processed frame, in two sets.
     struct FrameSlot {
         DevBuf<uint8_t> packet;
-        cudaEvent_t uploaded = nullptr;     // the packet is written: the processing stream (if another one) and the network wait for it
-        cudaEvent_t netDone = nullptr;      // the network has read the packet and (detector) written its mask and header
-        cudaStream_t upStream = nullptr;    // stream of the upload
+        Event uploaded;                     // the packet is written: the processing stream (if another one) and the network wait for it
+        Event netDone;                      // the network has read the packet and (detector) written its mask and header
+        cudaStream_t upStream = nullptr;    // stream of the upload (borrowed: the main stream or preStream)
         bool netUsed = false;               // netDone has been recorded: a reuse of the slot waits for it
         bool handoff = false;               // a detector writes this frame's mask / header: segmentation waits for netDone
         int64_t timestamp = 0;
         FrameSlot(size_t bytes, cudaStream_t s);
-        ~FrameSlot();
-        void destroyEvents();
     };
     std::vector<std::unique_ptr<FrameSlot>> ring;
     int curSlot = 0, queued = 0, queueLength = 0;    // slot of the frame being (or last) processed; frames queued after it; -frameQ
     void setFrameQueue(int length);
     void pushFrame(const uint8_t* rgb, const float* depth, int64_t timestamp, const uint8_t* mask, bool onDevice, cudaStream_t s, int ptick, bool detWanted);
     void popFrame(cudaStream_t s);
-    cudaEvent_t retired = nullptr; bool retiredValid = false;   // main stream at the last pop: frames processed before it are done with their data
+    Event retired; bool retiredValid = false;   // main stream at the last pop: frames processed before it are done with their data
     DevBuf<uchar4> rgbBuf[2]; DevBuf<float> depthFiltBuf[2];
     uint8_t* rgb3 = nullptr; uchar4* rgb = nullptr; float* depthRaw = nullptr; float* depthFilt = nullptr;   // the current frame
     uint8_t* frameMask = nullptr; FrameHdr* dHdr = nullptr;                                                   // FrameData::mask / classIDs of the current frame
@@ -257,13 +259,13 @@ public:
         curSlot = k; rgb3 = ring[k]->packet.p; depthRaw = reinterpret_cast<float*>(rgb3 + (size_t)P * 3); frameMask = slotMask(k); dHdr = slotHdr(k);
     }
     void selectSet(int k) { curSet = k; rgb = rgbBuf[k]; depthFilt = depthFiltBuf[k]; }
-    cudaStream_t preStream = nullptr; cudaEvent_t preDone = nullptr, inputsCopied = nullptr; bool preWaitPending = false, copyPending = false;
-    cudaEvent_t inputReady = nullptr;        // caller's producer event for device inputs (mf_set_input_event): waited on before the next frame's copies
+    Stream preStream; Event preDone, inputsCopied; bool preWaitPending = false, copyPending = false;
+    cudaEvent_t inputReady = nullptr;        // caller's producer event for device inputs (mf_set_input_event, borrowed): waited on before the next frame's copies
     DevBuf<uint8_t> mask;
     DevBuf<float> depthPyr[3]; DevBuf<float4> vmap[3], nmap[3];
     DevBuf<uint8_t> nextImage[3]; DevBuf<short2> nextGrad[3]; DevBuf<uint8_t> rgbValid[3];
     DevBuf<float> edgeMap; DevBuf<uint8_t> edgeBinary, edgeBuf, edgeInv;
-    DevBuf<TrackJob> dJobs; TrackJob* hJobs = nullptr;
+    DevBuf<TrackJob> dJobs; HostBuf<TrackJob> hJobs;
     DevBuf<uint8_t> initFlagR, initFlagF;
     DevBuf<float> scratch;                  // read-back staging
     DevBuf<float4> rayTab;                  // viewing ray of every pixel centre (camera constant): read by the splat rasteriser

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <string.h>
 #include <exception>
 #include <string>
 #include <utility>
@@ -33,6 +34,9 @@ struct SurfelPlanes { float4* pos; float4* col; float4* nrm; };
 struct CudaError { std::string what; };
 void cudaCheck(cudaError_t e, const char* where);        // throws CudaError
 
+// Owners of the CUDA resources a context holds: empty when constructed, acquired by an explicit call, released by the destructor (errors
+// ignored there), so a throw anywhere in a constructor unwinds what it acquired.  Acquisition is not the owner's constructor because a
+// context's members are constructed before it selects its device.
 template <typename T>
 struct DevBuf {
     T* p = nullptr; size_t n = 0;
@@ -43,6 +47,36 @@ struct DevBuf {
     void alloc(size_t count) { if (p) cudaFree(p); p = nullptr; n = 0; if (count) cudaCheck(cudaMalloc((void**)&p, count * sizeof(T)), "cudaMalloc"); n = count; }
     void zero(cudaStream_t s) { if (n) cudaCheck(cudaMemsetAsync(p, 0, n * sizeof(T), s), "memset"); }
     operator T*() const { return p; }
+};
+// pinned host memory, zero-filled by alloc
+template <typename T>
+struct HostBuf {
+    T* p = nullptr;
+    HostBuf() {}
+    HostBuf(const HostBuf&) = delete;
+    HostBuf& operator=(const HostBuf&) = delete;
+    ~HostBuf() { if (p) cudaFreeHost(p); }
+    void alloc(size_t count) { if (p) cudaFreeHost(p); p = nullptr; cudaCheck(cudaMallocHost((void**)&p, count * sizeof(T)), "cudaMallocHost"); memset(p, 0, count * sizeof(T)); }
+    operator T*() const { return p; }
+};
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() {}
+    Event(Event&& o) noexcept : e(o.e) { o.e = nullptr; }
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { if (e) cudaEventDestroy(e); }
+    void create(unsigned flags = cudaEventDisableTiming) { if (e) cudaEventDestroy(e); e = nullptr; cudaEvent_t h; cudaCheck(cudaEventCreateWithFlags(&h, flags), "cudaEventCreate"); e = h; }
+    operator cudaEvent_t() const { return e; }
+};
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() {}
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() { if (s) cudaStreamDestroy(s); }
+    void create() { if (s) cudaStreamDestroy(s); s = nullptr; cudaStream_t h; cudaCheck(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking), "cudaStreamCreate"); s = h; }
+    operator cudaStream_t() const { return s; }
 };
 
 // photometric correspondence record (reference: DataTerm, Core/Cuda/types.cuh:75-81)
