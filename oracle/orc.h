@@ -116,6 +116,11 @@ void orc_combined_predict(const float* surfels, int count, const float* pose, or
                           int W, int H, float maxDepth, float confThreshold, int time, int maxTime,
                           int timeDelta, uint8_t* image4, float* vertexConf4, float* normalRad4,
                           uint16_t* timeTex);
+/* splat.vert for one surfel and the pixel range of its sprite (R-PS / R-PR / R-PC), for tests that craft sprites at those edges.
+ * out[16] = ok, size, xw, yw, x0, x1, y0, y1 (x1 < x0: no pixel), camera-space position xyz, normal xyz, radius, confidence;
+ * fields after ok are meaningful only when the vertex stage accepted the surfel (ok = 1; size, xw, yw also when clipped by R-PC) */
+void orc_splat_extent(const float* surfel, const float* pose, orc_cam cam, int W, int H, float maxDepth, float confThreshold,
+                      int time, int maxTime, int timeDelta, float* out);
 /* fill_{vertex,normal,rgb}.frag, FillIn.cpp:43-166 */
 void orc_fill_in(const float* vertexConf4, const float* normalRad4, const uint8_t* image4,
                  const float* depthFilt, const uint8_t* rgb3, orc_cam cam, int W, int H,

@@ -447,6 +447,21 @@ static void splat_range(const splat_vs* v, int W, int H, int* x0, int* x1, int* 
     *y0 = lo < 0 ? 0 : (int)lo; *y1 = hi > (float)(H - 1) ? H - 1 : (int)hi;
 }
 
+void orc_splat_extent(const float* surfel, const float* pose, orc_cam cam, int W, int H, float maxDepth, float confThreshold,
+                      int time, int maxTime, int timeDelta, float* out)
+{
+    float tinv[16];
+    orc_pose_inverse(pose, tinv);
+    splat_vs v;
+    memset(&v, 0, sizeof v);
+    splat_vertex(surfel, tinv, cam, W, H, maxDepth, confThreshold, time, maxTime, timeDelta, &v);
+    int x0 = 0, x1 = -1, y0 = 0, y1 = -1;
+    if (v.ok) splat_range(&v, W, H, &x0, &x1, &y0, &y1);
+    const float o[16] = { (float)v.ok, v.size, v.xw, v.yw, (float)x0, (float)x1, (float)y0, (float)y1,
+                          v.pos[0], v.pos[1], v.pos[2], v.n[0], v.n[1], v.n[2], v.rad, v.conf };
+    memcpy(out, o, sizeof o);
+}
+
 static void splat_keys(const float* surfels, int count, const float* tinv, orc_cam cam, int W, int H,
                        float maxDepth, float confThreshold, int time, int maxTime, int timeDelta,
                        uint32_t drawBase, uint64_t* key)
