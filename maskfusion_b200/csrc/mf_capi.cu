@@ -547,7 +547,7 @@ extern "C" int mf_icp_step(mf_context* ctx, int i, int level, const float* Rcurr
     DevBuf<float> out; out.alloc(32);
     DevBuf<unsigned> ticket; ticket.alloc(1); ticket.zero(o->stream);
     launch_icp_only(o->vmap[level], o->nmap[level], m->vmapG[level], m->nmapG[level], o->W >> level, o->H >> level, camLevel(o->cam, level), pp,
-                    m->partial, ticket, out, o->numSMs, o->on());
+                    m->partial, ticket, out, o->on());
     cudaCheck(cudaMemcpyAsync(out29, out.p, 29 * sizeof(float), cudaMemcpyDeviceToHost, o->stream), "D2H");
     o->sync();
     return 0;

@@ -29,7 +29,6 @@
 #include <string.h>
 #include <map>
 #include <mutex>
-#include <set>
 #include <array>
 #include <type_traits>
 
@@ -328,9 +327,8 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // The GEMM launcher's process-wide state, behind one lock (handles may run on several threads and devices): the driver's
-// cuTensorMapEncodeTiled, looked up once; the tensor maps, which are pure functions of (pointer, geometry) -- the backbone's buffers never
-// move, so every map is encoded once (first forward) and reused by all later launches; and, per kernel instantiation, the devices on which
-// its dynamic shared-memory attribute is set (the attribute belongs to a (function, device) pair).
+// cuTensorMapEncodeTiled, looked up once; and the tensor maps, which are pure functions of (pointer, geometry) -- the backbone's buffers
+// never move, so every map is encoded once (first forward) and reused by all later launches.
 static std::mutex g_gemmLock;
 static PFN_encodeTiled g_encode = nullptr;
 static std::map<std::array<uint64_t, 6>, CUtensorMap> g_mapCache;
@@ -377,23 +375,22 @@ template <int BN, typename OutT>
 static void launch_wgmma(const void* A, const void* B, const float* bias, const void* residual, void* out, int M, int N, int K, int relu,
                          cudaStream_t s, const ConvGeom& geo, int Cin)
 {
-    static std::set<int> attrSet;                             // devices with this instantiation's attribute set (under g_gemmLock)
-    int dev = 0;
-    cudaCheck(cudaGetDevice(&dev), "cudaGetDevice");
+    // the dynamic shared memory this instantiation is opted in for: the attribute belongs to a (function, device) pair
+    static PerDevice<size_t> smem([](int) {
+        cudaCheck(cudaFuncSetAttribute(k_gemm_bf16_wgmma<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<BN>()),
+                  "cudaFuncSetAttribute");
+        return gemm_smem_bytes<BN>();
+    });
+    const size_t smemBytes = smem.get();
     const cuuint64_t dimsA[3] = {(cuuint64_t)(geo.mode ? Cin : K), (cuuint64_t)(geo.mode ? geo.Wimg : M), (cuuint64_t)geo.Himg}, dimsB[2] = {(cuuint64_t)K, (cuuint64_t)N};
     const cuuint32_t boxA[3] = {64, (cuuint32_t)(geo.mode ? geo.Wbox : GEMM_BM), (cuuint32_t)geo.Hbox}, boxB[2] = {64, BN};
     CUtensorMap mA, mB;
     {
         std::lock_guard<std::mutex> lock(g_gemmLock);
-        if (!attrSet.count(dev)) {
-            cudaCheck(cudaFuncSetAttribute(k_gemm_bf16_wgmma<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes<BN>()),
-                      "cudaFuncSetAttribute");
-            attrSet.insert(dev);
-        }
         mA = cached_map(A, geo.mode ? 3 : 2, dimsA, boxA);
         mB = cached_map(B, 2, dimsB, boxB);
     }
-    launch(Enq{s, nullptr}, nullptr, k_gemm_bf16_wgmma<BN, OutT>, dim3((M + GEMM_BM - 1) / GEMM_BM, N / BN), dim3(GEMM_THREADS), gemm_smem_bytes<BN>(),
+    launch(Enq{s, nullptr}, nullptr, k_gemm_bf16_wgmma<BN, OutT>, dim3((M + GEMM_BM - 1) / GEMM_BM, N / BN), dim3(GEMM_THREADS), smemBytes,
            mA, mB, bias, (const __nv_bfloat16*)residual, (OutT*)out, M, N, K, relu, geo);
 }
 

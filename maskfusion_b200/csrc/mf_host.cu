@@ -151,7 +151,7 @@ Model::Model(MaskFusion* o, unsigned char id_, float conf, bool enableFillIn, in
     cand.alloc((size_t)capacity + P); candCount.alloc(1); candCount.zero(s);
     for (int l = 0; l < 3; ++l) {
         size_t Pl = (size_t)(W >> l) * (H >> l);
-        vmapG[l].alloc(Pl); nmapG[l].alloc(Pl); cloud[l].alloc(Pl); lastDepth[l].alloc(Pl); lastImage[l].alloc(Pl); corres[l].alloc(l == 0 ? Pl + (size_t)o->numSMs * 512 : 1);   // level 0 only: scratch when the correspondences do not fit in shared memory
+        vmapG[l].alloc(Pl); nmapG[l].alloc(Pl); cloud[l].alloc(Pl); lastDepth[l].alloc(Pl); lastImage[l].alloc(Pl); corres[l].alloc(l == 0 ? Pl + (size_t)num_sms() * 512 : 1);   // level 0 only: scratch when the correspondences do not fit in shared memory
         vmapG[l].zero(s); nmapG[l].zero(s); lastDepth[l].zero(s); lastImage[l].zero(s);
     }
     if (id_ != 0) for (int l = 0; l < 3; ++l) { validBits[l].alloc(((size_t)(W >> l) * (H >> l) + 31) / 32 + 1); validBits[l].zero(s); }
@@ -306,10 +306,6 @@ void Model::combinedPredict(float depthCutoff, int time, int maxTime, int timeDe
 MaskFusion::MaskFusion(const mf_config& c, int dev, cudaStream_t st) : cfg(c), device(dev)
 {
     cudaCheck(cudaSetDevice(dev), "cudaSetDevice");
-    cudaDeviceProp prop;
-    cudaCheck(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
-    numSMs = prop.multiProcessorCount;
-    set_num_sms(numSMs);
     W = c.width; H = c.height; P = W * H;
     if (W % 4 || H % 4) throw CudaError{"width and height must be multiples of 4 (3-level pyramid)"};
     cam = Cam{c.fx, c.fy, c.cx, c.cy};
@@ -506,8 +502,9 @@ void MaskFusion::trackModels(const std::vector<Model*>& ms, bool viaResult)
     on().mark("copy_jobs");
     // hJobs is reused every frame: the next frameBegin first waits (finalisePending) for an event recorded behind this copy
     cudaCheck(cudaMemcpyAsync(dJobs, hJobs, ms.size() * sizeof(TrackJob), cudaMemcpyHostToDevice, stream), "jobs upload");
-    launch_tracking(dJobs, (int)ms.size(), W, H, cam, cfg.rgbOnly != 0, cfg.icpWeight, cfg.pyramid != 0, cfg.fastOdom != 0, cfg.so3 != 0, numSMs, on(),
-                    lightMask);
+    if ((++trackEpoch << 6) == 0u) ++trackEpoch;                     // flag 0 = "never written"
+    launch_tracking(dJobs, (int)ms.size(), W, H, cam, cfg.rgbOnly != 0, cfg.icpWeight, cfg.pyramid != 0, cfg.fastOdom != 0, cfg.so3 != 0, trackEpoch,
+                    on(), lightMask);
     on().mark("copy_pose_d2h");
     for (Model* m : ms) {
         if (!viaResult)

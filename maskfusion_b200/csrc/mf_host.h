@@ -217,8 +217,8 @@ public:
     mf_config cfg; Cam cam; int W, H, P; int device;
     cudaStream_t stream;                    // the main stream: the caller's (borrowed) or ownedStream
     Stream ownedStream;
-    int numSMs = 132;
     int tick = 1;
+    unsigned trackEpoch = 0;                // flag epoch of the tracker's partial-row exchange (launch_tracking), one per launch
     LaunchRecord rec;
     Enq on(cudaStream_t s = nullptr) { return Enq{s ? s : stream, &rec}; }     // where this context's launches go (nullptr: the main stream)
     std::vector<std::unique_ptr<Model>> models;

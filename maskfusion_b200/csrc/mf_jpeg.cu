@@ -307,17 +307,18 @@ bool decodeJPEG(const uint8_t* data, size_t size, int& W, int& H, std::vector<ui
         }
     }
     // jdcolor.c build_ycc_rgb_table
-    static int crR[256], cbB[256], crG[256], cbG[256]; static bool tab = false;
-    if (!tab) {
+    struct YccTables { int crR[256], cbB[256], crG[256], cbG[256]; };
+    static const YccTables tab = [] {
+        YccTables t;
         for (int i = 0; i < 256; ++i) {
             const int x = i - 128;
-            crR[i] = (int)((91881LL * x + 32768) >> 16);          // FIX(1.40200)
-            cbB[i] = (int)((116130LL * x + 32768) >> 16);         // FIX(1.77200)
-            crG[i] = -46802 * x;                                  // FIX(0.71414)
-            cbG[i] = -22554 * x + 32768;                          // FIX(0.34414) + ONE_HALF
+            t.crR[i] = (int)((91881LL * x + 32768) >> 16);        // FIX(1.40200)
+            t.cbB[i] = (int)((116130LL * x + 32768) >> 16);       // FIX(1.77200)
+            t.crG[i] = -46802 * x;                                // FIX(0.71414)
+            t.cbG[i] = -22554 * x + 32768;                        // FIX(0.34414) + ONE_HALF
         }
-        tab = true;
-    }
+        return t;
+    }();
     const Comp& Y = comps[0];
     for (int y = 0; y < H; ++y)
         for (int x = 0; x < W; ++x) {
@@ -325,7 +326,7 @@ bool decodeJPEG(const uint8_t* data, size_t size, int& W, int& H, std::vector<ui
             int cb, cr;
             if (h2) { const int outW = comps[1].dsW * 2; cb = up[0][(size_t)y * outW + x]; cr = up[1][(size_t)y * (comps[2].dsW * 2) + x]; }
             else { cb = comps[1].plane[(size_t)y * comps[1].planeW + x]; cr = comps[2].plane[(size_t)y * comps[2].planeW + x]; }
-            int r = yy + crR[cr], g = yy + ((cbG[cb] + crG[cr]) >> 16), b = yy + cbB[cb];
+            int r = yy + tab.crR[cr], g = yy + ((tab.cbG[cb] + tab.crG[cr]) >> 16), b = yy + tab.cbB[cb];
             uint8_t* o = &rgb[((size_t)y * W + x) * 3];
             o[0] = (uint8_t)(r < 0 ? 0 : (r > 255 ? 255 : r)); o[1] = (uint8_t)(g < 0 ? 0 : (g > 255 ? 255 : g)); o[2] = (uint8_t)(b < 0 ? 0 : (b > 255 ? 255 : b));
         }

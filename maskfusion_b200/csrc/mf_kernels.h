@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <string.h>
 #include <exception>
+#include <mutex>
 #include <string>
 #include <utility>
 #include <vector>
@@ -77,6 +78,30 @@ struct Stream {
     ~Stream() { if (s) cudaStreamDestroy(s); }
     void create() { if (s) cudaStreamDestroy(s); s = nullptr; cudaStream_t h; cudaCheck(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking), "cudaStreamCreate"); s = h; }
     operator cudaStream_t() const { return s; }
+};
+
+// A value that belongs to a device (an SM count, an occupancy, a kernel attribute set on it): `make(device)` runs the first time get() is
+// called with that device current, from whichever thread gets there first, and its result is kept for the process.  If `make` throws,
+// the exception reaches that caller and the next get() on the device runs it again.
+template <typename T>
+class PerDevice {
+public:
+    explicit PerDevice(T (*make)(int device)) : make_(make) {}
+    PerDevice(const PerDevice&) = delete;
+    PerDevice& operator=(const PerDevice&) = delete;
+    const T& get()
+    {
+        int dev = 0;
+        cudaCheck(cudaGetDevice(&dev), "cudaGetDevice");
+        if (dev < 0 || dev >= kMaxDevices) throw CudaError{"device ordinal above 63"};
+        std::call_once(once_[dev], [&] { value_[dev] = make_(dev); });
+        return value_[dev];
+    }
+private:
+    static constexpr int kMaxDevices = 64;
+    T (*make_)(int);
+    std::once_flag once_[kMaxDevices];
+    T value_[kMaxDevices] = {};
 };
 
 // photometric correspondence record (reference: DataTerm, Core/Cuda/types.cuh:75-81)
@@ -211,8 +236,7 @@ struct TrackJob {
     const uint32_t* validBits[3];   // object models: one bit per model-map pixel, set where the model normal is valid (nullptr: not used)
 };
 
-void set_num_sms(int n);
-int num_sms();
+int num_sms();                  // SMs of the current device
 
 // Where a dense-pipeline launcher enqueues: the stream and the launch record of the context it works for (mf_host.h: the launch
 // count of mf_kernel_launches and the stage timer).  A null record counts and times nothing.
@@ -362,11 +386,13 @@ void launch_aos_to_planes(const float4* in, uint32_t n, const SurfelPlanes& sp, 
 
 // ---- mf_track.cu ----
 void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* G);   // CTAs per model of the persistent tracking grid
+// epoch: the flag epoch of this launch's partial-row exchange, advanced by the caller for every launch on the same partial buffers, never
+// a value whose << 6 is 0 (TrackJob::partial; mf_track.cu)
 void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
-                     bool pyramid, bool fastOdom, bool so3, int numSMs, Enq q, unsigned lightMask = false);
+                     bool pyramid, bool fastOdom, bool so3, unsigned epoch, Enq q, unsigned lightMask = false);
 int debug_track_timing(long long* out, int cap);
 void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
-                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, int numSMs, Enq q);
+                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, Enq q);
 
 // ---- mf_seg.cu ----
 void launch_geometric_edges(const float4* vmap, const float4* nmap, int W, int H, float wD, float wC, float thr, float* edge, uint8_t* binary, Enq q);

@@ -84,7 +84,6 @@ enum { ncclUint8 = 1, ncclUint64 = 5, ncclFloat32 = 7 };          // ncclDataTyp
 enum { ncclMin = 3 };                                            // ncclRedOp_t: sum 0, prod 1, max 2, min 3
 
 struct NcclApi {
-    void* lib = nullptr;
     int (*GetUniqueId)(ncclUniqueId*) = nullptr;
     int (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
     int (*CommDestroy)(ncclComm_t) = nullptr;
@@ -94,28 +93,29 @@ struct NcclApi {
     int (*GetVersion)(int*) = nullptr;
     const char* (*GetErrorString)(int) = nullptr;
 };
-static NcclApi g_nccl;
-
-static NcclApi& nccl()
+// the entry points, opened on first use (a failed open is tried again by the next call)
+static const NcclApi& nccl()
 {
-    if (g_nccl.lib) return g_nccl;
-    // RTLD_NOLOAD first: if the process (torch) already mapped a libnccl, use that copy; else the default search path
-    void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);
-    if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) throw CudaError{std::string("object-sharded mode needs NCCL: dlopen(libnccl.so.2) failed: ") + dlerror()};
-    NcclApi a; a.lib = h;
+    static const NcclApi api = [] {
+        // RTLD_NOLOAD first: if the process (torch) already mapped a libnccl, use that copy; else the default search path
+        void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);
+        if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
+        if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
+        if (!h) throw CudaError{std::string("object-sharded mode needs NCCL: dlopen(libnccl.so.2) failed: ") + dlerror()};
+        NcclApi a;
 #define MF_SYM(field, name) *(void**)(&a.field) = dlsym(h, name); if (!a.field) throw CudaError{std::string("libnccl lacks ") + name};
-    MF_SYM(GetUniqueId, "ncclGetUniqueId") MF_SYM(CommInitRank, "ncclCommInitRank") MF_SYM(CommDestroy, "ncclCommDestroy")
-    MF_SYM(Broadcast, "ncclBroadcast") MF_SYM(AllGather, "ncclAllGather") MF_SYM(AllReduce, "ncclAllReduce")
-    MF_SYM(GetVersion, "ncclGetVersion") MF_SYM(GetErrorString, "ncclGetErrorString")
+        MF_SYM(GetUniqueId, "ncclGetUniqueId") MF_SYM(CommInitRank, "ncclCommInitRank") MF_SYM(CommDestroy, "ncclCommDestroy")
+        MF_SYM(Broadcast, "ncclBroadcast") MF_SYM(AllGather, "ncclAllGather") MF_SYM(AllReduce, "ncclAllReduce")
+        MF_SYM(GetVersion, "ncclGetVersion") MF_SYM(GetErrorString, "ncclGetErrorString")
 #undef MF_SYM
-    g_nccl = a;
-    return g_nccl;
+        return a;
+    }();
+    return api;
 }
+// r comes from an entry point, so the library is open
 static void ncclCheck(int r, const char* where)
 {
-    if (r != ncclSuccess) throw CudaError{std::string(where) + ": " + (g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "NCCL error")};
+    if (r != ncclSuccess) throw CudaError{std::string(where) + ": " + nccl().GetErrorString(r)};
 }
 
 void shardUniqueId(unsigned char* out128)
@@ -125,7 +125,7 @@ void shardUniqueId(unsigned char* out128)
     memcpy(out128, id.internal, 128);
 }
 
-ShardComm::~ShardComm() { if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy((ncclComm_t)comm); }
+ShardComm::~ShardComm() { if (comm) nccl().CommDestroy((ncclComm_t)comm); }     // comm is set only once the library is open
 void ShardComm::init(const unsigned char* id128, int rank_, int world_)
 {
     ncclUniqueId id; memcpy(id.internal, id128, 128);

@@ -1082,12 +1082,14 @@ __global__ void k_aos_to_planes(const float4* __restrict__ in, uint32_t n, float
 }
 
 // ------------------------------ host launchers ----------------------------------------
-static int g_numSMs = 0;                 // set by the context; a standalone backbone reads the current device
-void set_num_sms(int n) { g_numSMs = n > 0 ? n : 132; }
 int num_sms()
 {
-    if (!g_numSMs) { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); set_num_sms(n); }
-    return g_numSMs;
+    static PerDevice<int> sms([](int dev) {
+        int n = 0;
+        cudaCheck(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev), "cudaDeviceGetAttribute");
+        return n;
+    });
+    return sms.get();
 }
 static inline int persistentBlocks(int perSM) { return num_sms() * perSM; }
 
@@ -1176,13 +1178,13 @@ void launch_ray_table(Cam cam, int W, int H, float4* tab, Enq q)
 static dim3 splatGrid(uint32_t capacity, int W, int H)
 {
     if ((size_t)W * H > (1u << 24)) throw CudaError{"splat rasteriser: more than 2^24 pixels (its exact-path queue keeps 24-bit pixel indices)"};
-    static const int perSM = [] {
+    static PerDevice<int> perSM([](int) {
         int n = 0;
         cudaCheck(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_splat_project, SPLAT_BS, 0), "k_splat_project occupancy");
         if (n < 1) throw CudaError{"k_splat_project does not fit on an SM"};
         return n;
-    }();
-    const int persistent = persistentBlocks(perSM);
+    });
+    const int persistent = persistentBlocks(perSM.get());
     if (capacity == 0 || capacity >= (1u << 20)) return dim3(persistent);
     const int cols = (int)std::min<uint32_t>((capacity + SPLAT_BS - 1) / SPLAT_BS, (uint32_t)persistent);
     return dim3(cols, 8);

@@ -468,8 +468,10 @@ MF_D int fragIndex(int q)
 // are single transactions, so a reader that finds both flags holds the value -- no release fence on the producer, no arrival counter,
 // no second round trip for the data: the consumers poll the rows themselves.  The software barrier cost one fence + one atomic + one
 // polled counter + one row read per reduction (48 reductions per frame); this costs the row read alone.
-// Flags are unique per reduction and launch (llBase advances by 64 per launch, 0 is never used), rows ping-pong between two buffers:
-// a CTA writes reduction g + 2 only after it has consumed g + 1 from every peer, which every peer produced after consuming g.
+// Flags are unique per reduction and launch on one Model::partial buffer: llBase comes from the context's epoch (MaskFusion::trackEpoch),
+// which advances by one per launch and skips the value whose llBase is 0, so a flag is never 0 -- the value of a fresh, zeroed buffer.
+// Rows ping-pong between two buffers: a CTA writes reduction g + 2 only after it has consumed g + 1 from every peer, which every peer
+// produced after consuming g.
 MF_D void llStore(uint4* p, double v, unsigned flag)
 {
     asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"((unsigned)__double2loint(v)), "r"(flag), "r"((unsigned)__double2hiint(v)), "r"(flag) : "memory");
@@ -1206,10 +1208,10 @@ float track_min_scale(int level)
     return (float)(pow((double)minGrad[level], 2.0) / pow((double)sobelScale, 2.0));
 }
 
-static int trackBlocks(int N, int numSMs)
+static int trackBlocks(int N)
 {
     int need = (N + TRK_THREADS - 1) / TRK_THREADS;
-    int cap = numSMs * 2;
+    int cap = num_sms() * 2;
     if (cap > TRACK_MAX_BLOCKS) cap = TRACK_MAX_BLOCKS;
     return need < cap ? need : cap;
 }
@@ -1235,27 +1237,25 @@ void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* 
     for (int j = 0; j < nJobs; ++j) G[j] = ((lightMask >> j) & 1u) ? Glight : Gheavy;
 }
 
+// launch limits of the persistent tracking kernel on one device: CTAs that fit on it at once, and the dynamic shared memory it is opted in for
+struct TrackLimits { int coResident; size_t dynMax; };
+
 void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
-                     bool pyramid, bool fastOdom, bool so3, int numSMs, Enq q, unsigned lightMask)
+                     bool pyramid, bool fastOdom, bool so3, unsigned epoch, Enq q, unsigned lightMask)
 {
     const bool anyValidBits = lightMask != 0;          // bit j: job j is an object model with a validity bitmask (nearly all of its pixels are rejected early)
-    // per-device launch limits (several contexts on different GPUs may live in one process): occupancy and the opt-in
-    // dynamic shared memory attribute are properties of (function, device)
-    static int coResidentDev[64]; static size_t dynMaxDev[64]; static bool devInit[64];
-    int dev = 0; cudaCheck(cudaGetDevice(&dev), "cudaGetDevice");
-    if (dev < 0 || dev >= 64) throw CudaError{"device ordinal above 63"};
-    if (!devInit[dev]) {
+    static PerDevice<TrackLimits> limits([](int dev) {
         int perSM = 0;
         cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, k_track_persistent, PT_THREADS, 0);
         if (e != cudaSuccess || perSM < 1) throw CudaError{std::string("k_track_persistent does not fit on an SM: ") + cudaGetErrorString(e)};
-        coResidentDev[dev] = perSM * numSMs;
-        int optin = 0; cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        int optin = 0; cudaCheck(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "cudaDeviceGetAttribute");
         cudaFuncAttributes fa; cudaCheck(cudaFuncGetAttributes(&fa, k_track_persistent), "cudaFuncGetAttributes");
-        dynMaxDev[dev] = (size_t)optin > fa.sharedSizeBytes + 2048 ? (size_t)optin - fa.sharedSizeBytes - 2048 : 0;
-        cudaCheck(cudaFuncSetAttribute(k_track_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dynMaxDev[dev]), "cudaFuncSetAttribute");
-        devInit[dev] = true;
-    }
-    const int coResident = coResidentDev[dev];
+        TrackLimits l{perSM * num_sms(), (size_t)optin > fa.sharedSizeBytes + 2048 ? (size_t)optin - fa.sharedSizeBytes - 2048 : 0};
+        cudaCheck(cudaFuncSetAttribute(k_track_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.dynMax), "cudaFuncSetAttribute");
+        return l;
+    });
+    const TrackLimits& lim = limits.get();
+    const int numSMs = num_sms(), coResident = lim.coResident;
     TrackParams tp;
     tp.W = W; tp.H = H; tp.cam = cam;
     tp.icp = (!rgbOnly && icpWeight > 0) ? 1 : 0;
@@ -1266,10 +1266,7 @@ void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rg
     tp.angleThres = (float)sin(20.f * 3.14159254f / 180.f);
     tp.distThres = 0.10f; tp.sobelScale = (float)(1.0 / 8.0); tp.maxDepthDelta = 0.07f;
     for (int l = 0; l < 3; ++l) tp.minScale[l] = track_min_scale(l);
-    static unsigned llEpoch[64];    // per device; every launch owns 64 flag values
-    unsigned ep = ++llEpoch[dev];
-    if ((ep << 6) == 0u) ep = ++llEpoch[dev];           // flag 0 means "never written"
-    tp.llBase = ep << 6;
+    tp.llBase = epoch << 6;                      // every launch owns 64 flag values
     int G = numSMs / nJobs;                      // one CTA per SM, the SMs split between the tracked models
     if (G * nJobs > coResident) G = coResident / nJobs;
     if (G > TRACK_MAX_BLOCKS / 2) G = TRACK_MAX_BLOCKS / 2;
@@ -1289,15 +1286,15 @@ void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rg
     // sized for the models with the largest share (the heavy ones); a CTA whose share needs more slots uses its model's global scratch stripe
     const int rounds0 = (W * H + Gheavy * PT_THREADS - 1) / (Gheavy * PT_THREADS);
     size_t dyn = (size_t)rounds0 * PT_THREADS * sizeof(int2);
-    if (tp.rgb && dyn <= dynMaxDev[dev]) tp.corrSlots = rounds0 * PT_THREADS; else { tp.corrSlots = 0; dyn = 0; }
+    if (tp.rgb && dyn <= lim.dynMax) tp.corrSlots = rounds0 * PT_THREADS; else { tp.corrSlots = 0; dyn = 0; }
     dyn = (dyn + 15) & ~(size_t)15;
     // shared-memory words for the bitmask of a level: only when a job carries one (object models) and it fits behind the correspondences
     tp.bitWords = anyValidBits ? (W * H + 31) / 32 : 0;
     const size_t bitBytes = ((size_t)tp.bitWords * 4 + 15) & ~(size_t)15;
-    if (dyn + bitBytes > dynMaxDev[dev]) tp.bitWords = 0;
-    static int cacheOn = -1;        // MFB200_TRACK_CACHE=0: every iteration re-reads its pose-independent inputs from global memory (A/B)
-    if (cacheOn < 0) { const char* e = getenv("MFB200_TRACK_CACHE"); cacheOn = e ? (e[0] != '0') : MFB200_DEFAULT_TRACK_CACHE; }
-    tp.cacheRounds = cacheOn ? (int)std::min<size_t>((size_t)rounds0, (dynMaxDev[dev] - dyn - (tp.bitWords ? bitBytes : 0)) / ((size_t)PT_THREADS * CACHE_BYTES_PER_SLOT)) : 0;
+    if (dyn + bitBytes > lim.dynMax) tp.bitWords = 0;
+    // MFB200_TRACK_CACHE=0: every iteration re-reads its pose-independent inputs from global memory (A/B)
+    static const bool cacheOn = [] { const char* e = getenv("MFB200_TRACK_CACHE"); return e ? e[0] != '0' : MFB200_DEFAULT_TRACK_CACHE != 0; }();
+    tp.cacheRounds = cacheOn ? (int)std::min<size_t>((size_t)rounds0, (lim.dynMax - dyn - (tp.bitWords ? bitBytes : 0)) / ((size_t)PT_THREADS * CACHE_BYTES_PER_SLOT)) : 0;
     dyn += (size_t)tp.cacheRounds * PT_THREADS * CACHE_BYTES_PER_SLOT + (tp.bitWords ? bitBytes : 0);
     q.mark("k_track_persistent");
     const TrackJob* jp = d_jobs;
@@ -1323,10 +1320,10 @@ int debug_track_timing(long long* out, int cap)
 }
 
 void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
-                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, int numSMs, Enq q)
+                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, Enq q)
 {
     const float angleThres = (float)sin(20.f * 3.14159254f / 180.f);
-    launch(q, "k_icp_only", k_icp_only, trackBlocks(W * H, numSMs), TRK_THREADS, 0, vmapC, nmapC, vmapG, nmapG, W, H, cam, pp, 0.10f, angleThres,
+    launch(q, "k_icp_only", k_icp_only, trackBlocks(W * H), TRK_THREADS, 0, vmapC, nmapC, vmapG, nmapG, W, H, cam, pp, 0.10f, angleThres,
            reinterpret_cast<double*>(partial), ticket, out29);
 }
 
