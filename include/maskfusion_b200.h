@@ -232,7 +232,6 @@ int mf_shard_pick_owner(const int64_t* loads, int world);                     /*
 int mf_set_profiling(mf_context* ctx, int on);
 int mf_get_stage_times(mf_context* ctx, char* buf, int bufsize);   /* lines: "name count total_ms" */
 int mf_debug_set_poses(mf_context* ctx, int i, const float pose16[16], const float last_pose16[16]);   /* sets Model::pose and Model::lastPose verbatim */
-int mf_icp_step(mf_context* ctx, int i, int level, const float Rcurr9[9], const float tcurr3[3], float out29[29]);  /* icpStep, reduce.cu:446-525 */
 
 /* ---- Mask R-CNN backbone: ResNet-101 + FPN as wgmma GEMMs (replaces the dense part of the Keras/TF sidecar,
  *      Core/Segmentation/MaskRCNN/MaskRCNN.py.in:55-58,101-111; weights are synthetic/seeded unless loaded with mf_*_load_weights).

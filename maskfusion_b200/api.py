@@ -230,12 +230,6 @@ class Model:
         self._ck(self.mf.L.mf_download_track_stats(self.mf.h, self.i, _p(A), _p(b), _p(e)))
         return A, b, e
 
-    def icpStep(self, level: int, Rcurr: np.ndarray, tcurr: np.ndarray) -> np.ndarray:
-        out = np.zeros(29, np.float32)
-        R = np.ascontiguousarray(Rcurr, np.float32).ravel(); t = np.ascontiguousarray(tcurr, np.float32).ravel()
-        self._ck(self.mf.L.mf_icp_step(self.mf.h, self.i, level, _p(R), _p(t), _p(out)))
-        return out
-
     def poseLog(self) -> np.ndarray:
         n = self._ck(self.mf.L.mf_pose_log_size(self.mf.h, self.i))
         out = np.zeros((max(n, 1), 8))

@@ -528,32 +528,6 @@ extern "C" int mf_debug_set_poses(mf_context* ctx, int i, const float* pose16, c
     return 0;
     MF_CATCH(-1)
 }
-extern "C" int mf_icp_step(mf_context* ctx, int i, int level, const float* Rcurr9, const float* tcurr3, float* out29)
-{
-    MF_TRY MF_NEED(ctx) MF_MODEL(ctx, i) MF_OWNED(m)
-    MaskFusion* o = ctx->mf.get();
-    if (level < 0 || level > 2) { mf_set_error("level out of range"); return -2; }
-    TrackPoses pp; memset(&pp, 0, sizeof pp);
-    memcpy(pp.p[0], Rcurr9, 9 * sizeof(float)); memcpy(pp.p[0] + 9, tcurr3, 3 * sizeof(float));
-    // Rprev^-1 / tprev of the model's current pose (RGBDOdometry.cpp:331-334)
-    const float* P = m->pose.m;
-    float R[9] = {P[0], P[1], P[2], P[4], P[5], P[6], P[8], P[9], P[10]};
-    float c00 = R[4] * R[8] - R[5] * R[7], c01 = R[5] * R[6] - R[3] * R[8], c02 = R[3] * R[7] - R[4] * R[6];
-    float det = (R[0] * c00 + R[1] * c01) + R[2] * c02, id = 1.0f / det;
-    float Ri[9] = {c00 * id, (R[2] * R[7] - R[1] * R[8]) * id, (R[1] * R[5] - R[2] * R[4]) * id,
-                   c01 * id, (R[0] * R[8] - R[2] * R[6]) * id, (R[2] * R[3] - R[0] * R[5]) * id,
-                   c02 * id, (R[1] * R[6] - R[0] * R[7]) * id, (R[0] * R[4] - R[1] * R[3]) * id};
-    memcpy(pp.p[1], Ri, sizeof Ri); pp.p[1][9] = P[3]; pp.p[1][10] = P[7]; pp.p[1][11] = P[11];
-    DevBuf<float> out; out.alloc(32);
-    DevBuf<unsigned> ticket; ticket.alloc(1); ticket.zero(o->stream);
-    launch_icp_only(o->vmap[level], o->nmap[level], m->vmapG[level], m->nmapG[level], o->W >> level, o->H >> level, camLevel(o->cam, level), pp,
-                    m->partial, ticket, out, o->on());
-    cudaCheck(cudaMemcpyAsync(out29, out.p, 29 * sizeof(float), cudaMemcpyDeviceToHost, o->stream), "D2H");
-    o->sync();
-    return 0;
-    MF_CATCH(-1)
-}
-
 // ======================================================================================
 // .klg reader / writer (GUI/Tools/KlgLogReader.cpp:29-113): raw or zlib-compressed depth, raw or JPEG-compressed colour
 // (decoded by mf_jpeg.cu, a restatement of libjpeg's default decode path).

@@ -36,6 +36,64 @@ MF_D float3 rotate(const Rt& T, float3 n) {
                        (T.m[4] * n.x + T.m[5] * n.y) + T.m[6] * n.z,
                        (T.m[8] * n.x + T.m[9] * n.y) + T.m[10] * n.z);
 }
+// Rigid-pose arithmetic on row-major 4x4 float arrays, the one definition for the host classes and the kernels.
+// Rule R-INV (DESIGN.md): pose.inverse() of a rigid pose is [R^T | -R^T t] in fp32.
+MF_HD void rigidInverse(const float* m, float* inv) {
+    const float R[9] = {m[0], m[1], m[2], m[4], m[5], m[6], m[8], m[9], m[10]}, t[3] = {m[3], m[7], m[11]};
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) inv[r * 4 + c] = R[c * 3 + r];
+        inv[r * 4 + 3] = -((R[0 * 3 + r] * t[0] + R[1 * 3 + r] * t[1]) + R[2 * 3 + r] * t[2]);
+    }
+    inv[12] = 0.f; inv[13] = 0.f; inv[14] = 0.f; inv[15] = 1.f;
+}
+// C = A * B, each entry summed as s += A[r][k] * B[k][c], k = 0..3; C must not alias A or B
+MF_HD void mul(const float* A, const float* B, float* C) {
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) {
+            float s = 0;
+            for (int k = 0; k < 4; ++k) s += A[r * 4 + k] * B[k * 4 + c];
+            C[r * 4 + c] = s;
+        }
+}
+// Model::rodrigues2 (Model.cpp:890-932) without the SVD re-orthonormalisation (rule R-SVD, DESIGN.md); R row-major 3x3
+MF_HD void rodrigues2(const float* R, float* out) {
+    double rx = R[7] - R[5], ry = R[2] - R[6], rz = R[3] - R[1];
+    double s = sqrt((rx * rx + ry * ry + rz * rz) * 0.25);
+    double c = ((double)(R[0] + R[4] + R[8]) - 1) * 0.5;
+    c = c > 1. ? 1. : c < -1. ? -1. : c;
+    double theta = acos(c);
+    if (s < 1e-5) {
+        double t;
+        if (c > 0) rx = ry = rz = 0;
+        else {
+            t = (R[0] + 1) * 0.5; rx = sqrt(t > 0 ? t : 0.0);
+            t = (R[4] + 1) * 0.5; ry = sqrt(t > 0 ? t : 0.0) * (R[1] < 0 ? -1.0 : 1.0);
+            t = (R[8] + 1) * 0.5; rz = sqrt(t > 0 ? t : 0.0) * (R[2] < 0 ? -1.0 : 1.0);
+            if (fabs(rx) < fabs(ry) && fabs(rx) < fabs(rz) && (R[5] > 0) != (ry * rz > 0)) rz = -rz;
+            theta /= sqrt(rx * rx + ry * ry + rz * rz);
+            rx *= theta; ry *= theta; rz *= theta;
+        }
+    } else {
+        double vth = 1 / (2 * s); vth *= theta; rx *= vth; ry *= vth; rz *= vth;
+    }
+    out[0] = (float)rx; out[1] = (float)ry; out[2] = (float)rz;
+}
+// Model::computeFusionWeight(1.0) (Model.cpp:449-464): max(1 - min(max(|t|, |rotation vector|), 0.01) / 0.01, 0.5) of the last motion
+// pose^-1 * lastPose; poseInv = rigidInverse(pose)
+MF_HD float fusionWeight(const float* poseInv, const float* last) {
+    float diff[16];
+    mul(poseInv, last, diff);
+    const float R[9] = {diff[0], diff[1], diff[2], diff[4], diff[5], diff[6], diff[8], diff[9], diff[10]};
+    float tn = sqrtf((diff[3] * diff[3] + diff[7] * diff[7]) + diff[11] * diff[11]);
+    float rv[3]; rodrigues2(R, rv);
+    float rn = sqrtf((rv[0] * rv[0] + rv[1] * rv[1]) + rv[2] * rv[2]);
+    float weighting = tn > rn ? tn : rn;
+    const float largest = 0.01f, minWeight = 0.5f;
+    if (weighting > largest) weighting = largest;
+    float w = 1.0f - (weighting / largest);
+    return w > minWeight ? w : minWeight;
+}
+
 MF_D float dot3(float3 a, float3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
 MF_D float3 cross3(float3 a, float3 b) {
     return make_float3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);

@@ -50,55 +50,7 @@ void Profiler::resolve()
     used = 0;
 }
 
-Mat4 rigidInverse(const Mat4& T)
-{
-    // [R^T | -R^T t] in fp32 (reference: Eigen::Matrix4f::inverse(); rule fixed in DESIGN.md)
-    Mat4 o = Mat4::identity();
-    const float* m = T.m;
-    float R[9] = {m[0], m[1], m[2], m[4], m[5], m[6], m[8], m[9], m[10]}, t[3] = {m[3], m[7], m[11]};
-    for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) o.m[r * 4 + c] = R[c * 3 + r];
-        o.m[r * 4 + 3] = -((R[0 * 3 + r] * t[0] + R[1 * 3 + r] * t[1]) + R[2 * 3 + r] * t[2]);
-    }
-    return o;
-}
-Mat4 mul(const Mat4& A, const Mat4& B)
-{
-    Mat4 o;
-    for (int r = 0; r < 4; ++r)
-        for (int c = 0; c < 4; ++c) {
-            float s = 0;
-            for (int k = 0; k < 4; ++k) s += A.m[r * 4 + k] * B.m[k * 4 + c];
-            o.m[r * 4 + c] = s;
-        }
-    return o;
-}
 Rt toRt(const Mat4& T) { Rt r; for (int i = 0; i < 12; ++i) r.m[i] = T.m[i]; return r; }
-
-// Model::rodrigues2 (Model.cpp:890-932) without the SVD re-orthonormalisation (see DESIGN.md)
-static void rodrigues2(const float* R, float* out)
-{
-    double rx = R[7] - R[5], ry = R[2] - R[6], rz = R[3] - R[1];
-    double s = sqrt((rx * rx + ry * ry + rz * rz) * 0.25);
-    double c = ((double)(R[0] + R[4] + R[8]) - 1) * 0.5;
-    c = c > 1. ? 1. : c < -1. ? -1. : c;
-    double theta = acos(c);
-    if (s < 1e-5) {
-        double t;
-        if (c > 0) rx = ry = rz = 0;
-        else {
-            t = (R[0] + 1) * 0.5; rx = sqrt(t > 0 ? t : 0.0);
-            t = (R[4] + 1) * 0.5; ry = sqrt(t > 0 ? t : 0.0) * (R[1] < 0 ? -1.0 : 1.0);
-            t = (R[8] + 1) * 0.5; rz = sqrt(t > 0 ? t : 0.0) * (R[2] < 0 ? -1.0 : 1.0);
-            if (fabs(rx) < fabs(ry) && fabs(rx) < fabs(rz) && (R[5] > 0) != (ry * rz > 0)) rz = -rz;
-            theta /= sqrt(rx * rx + ry * ry + rz * rz);
-            rx *= theta; ry *= theta; rz *= theta;
-        }
-    } else {
-        double vth = 1 / (2 * s); vth *= theta; rx *= vth; ry *= vth; rz *= vth;
-    }
-    out[0] = (float)rx; out[1] = (float)ry; out[2] = (float)rz;
-}
 
 // Eigen::Quaternionf(Matrix3f) as used by the pose log (MaskFusion.cpp:585-590)
 static void rotToQuat(const float* R, float* q)
@@ -207,21 +159,6 @@ void Model::prepareTracking()
         float4* c3[3] = {cloud[0].p, cloud[1].p, cloud[2].p};
         launch_project_points3(d3, W, H, o->cam, c3, q);
     }
-}
-
-float Model::computeFusionWeight(float weightMultiplier) const
-{
-    Mat4 diff = mul(rigidInverse(pose), lastPose);       // Model::getLastTransform, Model.h:239
-    const float* d = diff.m;
-    float R[9] = {d[0], d[1], d[2], d[4], d[5], d[6], d[8], d[9], d[10]};
-    float tn = sqrtf((d[3] * d[3] + d[7] * d[7]) + d[11] * d[11]);
-    float rv[3]; rodrigues2(R, rv);
-    float rn = sqrtf((rv[0] * rv[0] + rv[1] * rv[1]) + rv[2] * rv[2]);
-    float weighting = tn > rn ? tn : rn;
-    const float largest = 0.01f, minWeight = 0.5f;
-    if (weighting > largest) weighting = largest;
-    float w = 1.0f - (weighting / largest);
-    return (w > minWeight ? w : minWeight) * weightMultiplier;
 }
 
 void Model::predictIndices(int time, float depthCutoff, int timeDelta, bool forClean)

@@ -20,8 +20,8 @@ struct Mat4 {
     float m[16];
     static Mat4 identity() { Mat4 r; for (int i = 0; i < 16; ++i) r.m[i] = (i % 5 == 0) ? 1.f : 0.f; return r; }
 };
-Mat4 rigidInverse(const Mat4& T);
-Mat4 mul(const Mat4& A, const Mat4& B);
+inline Mat4 rigidInverse(const Mat4& T) { Mat4 o; rigidInverse(T.m, o.m); return o; }
+inline Mat4 mul(const Mat4& A, const Mat4& B) { Mat4 o; mul(A.m, B.m, o.m); return o; }
 Rt toRt(const Mat4& T);
 
 // in-stream stage timer: one CUDA event per mark; the interval up to the next mark is attributed to the mark's name.  Off by default.
@@ -69,7 +69,6 @@ public:
     void fuse(int time, float depthCutoff, float weightMultiplier);   // Model::fuse
     void clean(int time, int timeDelta, float depthCutoff);           // Model::clean
     void combinedPredict(float depthCutoff, int time, int maxTime, int timeDelta);   // Model::combinedPredict + performFillIn
-    float computeFusionWeight(float weightMultiplier) const;          // Model::computeFusionWeight
     void overridePose(const Mat4& p) { lastPose = pose; pose = p; pushPose(); }
     void makeStatic(const Mat4& globalPose) { initialC2Winv = mul(pose, rigidInverse(globalPose)); isStatic = true; }
     void updateStaticPose(const Mat4& globalPose) { overridePose(mul(initialC2Winv, globalPose)); }

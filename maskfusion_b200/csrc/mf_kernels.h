@@ -109,7 +109,6 @@ struct DataTerm { short2 zero; short2 one; float diff; int valid; };
 
 #define TRACK_MAX_JOBS 32        // tracked models of one batched launch (configs[4]: 16 objects + background)
 #define TRACK_MAX_BLOCKS 1024
-struct TrackPoses { float p[TRACK_MAX_JOBS][16]; };
 
 // Pose of one model as the kernels see it: DEVICE resident, so that the passes after tracking (index map, association,
 // fusion, clean, splat) are enqueued without waiting for the tracked pose on the host.  Written by the tracking kernel's
@@ -120,63 +119,13 @@ struct TrackPoses { float p[TRACK_MAX_JOBS][16]; };
 struct DevPose { Rt pose; Rt tinv; float fusionW; float pad[7]; };
 
 #ifdef __CUDACC__
-// Model::rodrigues2 (Model.cpp:890-932) without the SVD re-orthonormalisation (rule R-SVD, DESIGN.md); R row-major 3x3
-__device__ inline void rodrigues2Dev(const float* R, float* out)
-{
-    double rx = R[7] - R[5], ry = R[2] - R[6], rz = R[3] - R[1];
-    double s = sqrt((rx * rx + ry * ry + rz * rz) * 0.25);
-    double c = ((double)(R[0] + R[4] + R[8]) - 1) * 0.5;
-    c = c > 1. ? 1. : c < -1. ? -1. : c;
-    double theta = acos(c);
-    if (s < 1e-5) {
-        double t;
-        if (c > 0) rx = ry = rz = 0;
-        else {
-            t = (R[0] + 1) * 0.5; rx = sqrt(t > 0 ? t : 0.0);
-            t = (R[4] + 1) * 0.5; ry = sqrt(t > 0 ? t : 0.0) * (R[1] < 0 ? -1.0 : 1.0);
-            t = (R[8] + 1) * 0.5; rz = sqrt(t > 0 ? t : 0.0) * (R[2] < 0 ? -1.0 : 1.0);
-            if (fabs(rx) < fabs(ry) && fabs(rx) < fabs(rz) && (R[5] > 0) != (ry * rz > 0)) rz = -rz;
-            theta /= sqrt(rx * rx + ry * ry + rz * rz);
-            rx *= theta; ry *= theta; rz *= theta;
-        }
-    } else {
-        double vth = 1 / (2 * s); vth *= theta; rx *= vth; ry *= vth; rz *= vth;
-    }
-    out[0] = (float)rx; out[1] = (float)ry; out[2] = (float)rz;
-}
-
-// pose (row-major 4x4, rigid) + the pose before this frame's update -> everything the surfel passes read.
-// One thread.  tinv: [R^T | -R^T t] in fp32 with the operation order of the host rule (R-INV);
-// fusionW: max(1 - max(|t|, |rotation vector|) of (pose^-1 * lastPose) / 0.01, 0.5)  (Model.cpp:449-464)
+// pose (row-major 4x4, rigid) + the pose before this frame's update -> everything the surfel passes read.  One thread.
 __device__ inline void derivePose(DevPose* d, const float* m, const float* last)
 {
     float inv[16];
-    {
-        const float R[9] = {m[0], m[1], m[2], m[4], m[5], m[6], m[8], m[9], m[10]}, t[3] = {m[3], m[7], m[11]};
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) inv[r * 4 + c] = R[c * 3 + r];
-            inv[r * 4 + 3] = -((R[0 * 3 + r] * t[0] + R[1 * 3 + r] * t[1]) + R[2 * 3 + r] * t[2]);
-        }
-        inv[12] = 0.f; inv[13] = 0.f; inv[14] = 0.f; inv[15] = 1.f;
-    }
+    rigidInverse(m, inv);
     for (int k = 0; k < 12; ++k) { d->pose.m[k] = m[k]; d->tinv.m[k] = inv[k]; }
-    // diff = pose^-1 * lastPose, full 4x4 product in the order of the host routine (s += A[r][k] * B[k][c], k = 0..3)
-    float diff[16];
-    for (int r = 0; r < 4; ++r)
-        for (int c = 0; c < 4; ++c) {
-            float s = 0;
-            for (int k = 0; k < 4; ++k) s += inv[r * 4 + k] * last[k * 4 + c];
-            diff[r * 4 + c] = s;
-        }
-    const float R[9] = {diff[0], diff[1], diff[2], diff[4], diff[5], diff[6], diff[8], diff[9], diff[10]};
-    float tn = sqrtf((diff[3] * diff[3] + diff[7] * diff[7]) + diff[11] * diff[11]);
-    float rv[3]; rodrigues2Dev(R, rv);
-    float rn = sqrtf((rv[0] * rv[0] + rv[1] * rv[1]) + rv[2] * rv[2]);
-    float weighting = tn > rn ? tn : rn;
-    const float largest = 0.01f, minWeight = 0.5f;
-    if (weighting > largest) weighting = largest;
-    float w = 1.0f - (weighting / largest);
-    d->fusionW = w > minWeight ? w : minWeight;
+    d->fusionW = fusionWeight(inv, last);
 }
 #endif
 
@@ -391,8 +340,6 @@ void track_shares(int nJobs, unsigned lightMask, int totalCTAs, int ratio, int* 
 void launch_tracking(TrackJob* d_jobs, int nJobs, int W, int H, Cam cam, bool rgbOnly, float icpWeight,
                      bool pyramid, bool fastOdom, bool so3, unsigned epoch, Enq q, unsigned lightMask = false);
 int debug_track_timing(long long* out, int cap);
-void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
-                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, Enq q);
 
 // ---- mf_seg.cu ----
 void launch_geometric_edges(const float4* vmap, const float4* nmap, int W, int H, float wD, float wC, float thr, float* edge, uint8_t* binary, Enq q);

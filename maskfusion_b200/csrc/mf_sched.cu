@@ -47,14 +47,8 @@ __global__ void k_lifecycle(LifeParams lp, const float* __restrict__ gathered, F
             if (m.owned) { res->deadCount[i] = *m.count; *m.count = 0; }
         }
     } else {
-        // Model::updateStaticPose: pose = initialC2Winv * globalPose, products summed in the order of the host routine mfb::mul
-        const float* g = gathered;                                 // the background model is tracked by rank 0, slot 0
-        for (int r = 0; r < 4; ++r)
-            for (int c = 0; c < 4; ++c) {
-                float s = 0;
-                for (int k = 0; k < 4; ++k) s += m.initialC2Winv[r * 4 + k] * g[k * 4 + c];
-                pose[r * 4 + c] = s;
-            }
+        // Model::updateStaticPose: pose = initialC2Winv * globalPose
+        mul(m.initialC2Winv, gathered, pose);                      // the background model is tracked by rank 0, slot 0
         for (int k = 0; k < 16; ++k) last[k] = (k % 5 == 0) ? 1.f : 0.f;
         if (m.owned) {
             float old[16];

@@ -15,7 +15,6 @@
 // fixed order and runs the same 6x6 solve (pivoted LDLT, double), so the solver state is
 // replicated bit for bit without a broadcast.  Results are deterministic for a fixed launch shape.
 // MFB200_TRACK_CACHE=1 keeps the pose-independent pixel inputs of a level in shared memory (same bits).
-// k_icp_only is a stand-alone ICP reduction at a given pose (last-block ticket) for the parity tests.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 #include "mf_host.h"
@@ -31,7 +30,6 @@ namespace mfb {
 #define MFB200_DEFAULT_TRACK_CACHE 0
 #endif
 #define CACHE_BYTES_PER_SLOT 44        // float4 vertex + float4 normal + depth + packed (valid, intensity, x, y) + Sobel gradient
-#define TRK_THREADS 256
 #define NACC_ICP 29
 #define NACC_RGB 27
 #define NACC (NACC_ICP + NACC_RGB)
@@ -267,121 +265,6 @@ __device__ void computeWarp(TrackState* st, Cam c)
     inv3d(K, Kinv); mul3d(K, Ri, tmp); mul3d(tmp, Kinv, KRK);
     for (int q = 0; q < 9; ++q) st->krk[q] = (float)KRK[q];
     for (int r = 0; r < 3; ++r) st->kt[r] = (float)(K[r * 3] * ti[0] + K[r * 3 + 1] * ti[1] + K[r * 3 + 2] * ti[2]);
-}
-
-// ---------------------------------------------------------------------------------------
-// block reduction helpers
-// ---------------------------------------------------------------------------------------
-template <int N>
-MF_D void blockReduceStore(double* acc, double* partialOut)
-{
-    __shared__ double sh[TRK_THREADS / 32][N];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-        double v = acc[k];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) v += __hiloint2double(__shfl_down_sync(0xffffffffu, __double2hiint(v), off), __shfl_down_sync(0xffffffffu, __double2loint(v), off));
-        if (lane == 0) sh[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < N) {
-        double s = 0;
-#pragma unroll
-        for (int w = 0; w < TRK_THREADS / 32; ++w) s += sh[w][threadIdx.x];
-        partialOut[threadIdx.x] = s;
-    }
-}
-
-// Sum the per-block partials (rows of 32 doubles, N used) with the WHOLE last block: warp w takes blocks
-// w, w+8, ...; lanes take columns lane and lane+32 (coalesced 128-byte rows, independent loads), doubles
-// throughout; the 8 warp sums are combined in fixed order.  Deterministic for a fixed launch shape.
-// (A single thread per column walking all partials serially exposes the L2 latency of every partial.)
-template <int N>
-MF_D void sumPartials(const double* __restrict__ partial, unsigned nblocks, double* tot /* shared, >= N */)
-{
-    __shared__ double ws[TRK_THREADS / 32][32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double a0 = 0;
-#pragma unroll 4
-    for (unsigned b = warp; b < nblocks; b += TRK_THREADS / 32) a0 += partial[(size_t)b * 32 + lane];
-    ws[warp][lane] = a0;
-    __syncthreads();
-    if (threadIdx.x < N) {
-        double s = 0;
-#pragma unroll
-        for (int w = 0; w < TRK_THREADS / 32; ++w) s += ws[w][threadIdx.x];
-        tot[threadIdx.x] = s;
-    }
-    __syncthreads();
-}
-
-// returns true in ALL threads of the last block to arrive
-MF_D bool lastBlock(unsigned* ticket)
-{
-    __shared__ bool isLast;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned t = atomicAdd(ticket, 1u);
-        isLast = (t == gridDim.x - 1);
-        if (isLast) *ticket = 0;
-    }
-    __syncthreads();
-    if (isLast) __threadfence();
-    return isLast;
-}
-
-// stand-alone ICP reduction at a caller-given pose (parity tests; mirrors icpStep's outputs)
-__global__ void __launch_bounds__(TRK_THREADS) k_icp_only(const float4* __restrict__ vmapC, const float4* __restrict__ nmapC,
-                                                          const float4* __restrict__ vmapG, const float4* __restrict__ nmapG,
-                                                          int W, int H, Cam cam, TrackPoses pp, float distThres, float angleThres,
-                                                          double* __restrict__ partial, unsigned* ticket, float* out29)
-{
-    // pp.p[0] = Rcurr(9) tcurr(3); pp.p[1] = RprevInv(9) tprev(3)
-    double acc[NACC_ICP];
-#pragma unroll
-    for (int k = 0; k < NACC_ICP; ++k) acc[k] = 0.0;
-    const float* Rc = pp.p[0]; const float* tc = pp.p[0] + 9; const float* Rpi = pp.p[1]; const float* tp = pp.p[1] + 9;
-    const float3 tprev = make_float3(tp[0], tp[1], tp[2]);
-    const int N = W * H;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
-        float4 vc4 = vmapC[i];
-        float3 vg = m3v(Rc, make_float3(vc4.x, vc4.y, vc4.z));
-        vg = make_float3(vg.x + tc[0], vg.y + tc[1], vg.z + tc[2]);
-        float3 vcp = m3v(Rpi, sub3(vg, tprev));
-        int ux = __float2int_rn(vcp.x * cam.fx / vcp.z + cam.cx);
-        int uy = __float2int_rn(vcp.y * cam.fy / vcp.z + cam.cy);
-        if (ux < 0 || uy < 0 || ux >= W || uy >= H || vcp.z < 0) continue;
-        int j = uy * W + ux;
-        float4 vp4 = __ldg(vmapG + j), np4 = __ldg(nmapG + j), nc4 = nmapC[i];
-        float3 vp = make_float3(vp4.x, vp4.y, vp4.z), np_ = make_float3(np4.x, np4.y, np4.z);
-        float3 ng = m3v(Rc, make_float3(nc4.x, nc4.y, nc4.z));
-        float3 d = sub3(vp, vg);
-        float dist = sqrtf((d.x * d.x + d.y * d.y) + d.z * d.z);
-        float3 c = cross3(ng, np_);
-        float sine = sqrtf((c.x * c.x + c.y * c.y) + c.z * c.z);
-        if (!(sine < angleThres && dist <= distThres && !isnan(nc4.x) && !isnan(np4.x))) continue;
-        float3 s_cp = vcp, d_cp = m3v(Rpi, sub3(vp, tprev)), n_cp = m3v(Rpi, np_);
-        float row[7];
-        row[0] = n_cp.x; row[1] = n_cp.y; row[2] = n_cp.z;
-        row[3] = s_cp.y * n_cp.z - s_cp.z * n_cp.y;
-        row[4] = s_cp.z * n_cp.x - s_cp.x * n_cp.z;
-        row[5] = s_cp.x * n_cp.y - s_cp.y * n_cp.x;
-        row[6] = (n_cp.x * (s_cp.x - d_cp.x) + n_cp.y * (s_cp.y - d_cp.y)) + n_cp.z * (s_cp.z - d_cp.z);
-        int q = 0;
-#pragma unroll
-        for (int a = 0; a < 6; ++a)
-#pragma unroll
-            for (int b = a; b < 7; ++b) { acc[q] = fma((double)row[a], (double)row[b], acc[q]); ++q; }
-        acc[27] = fma((double)row[6], (double)row[6], acc[27]);
-        acc[28] += 1.0;
-    }
-    blockReduceStore<NACC_ICP>(acc, partial + (size_t)blockIdx.x * 32);
-    if (!lastBlock(ticket)) return;
-    __shared__ double tot[NACC_ICP];
-    sumPartials<NACC_ICP>(partial, gridDim.x, tot);
-    if (threadIdx.x < NACC_ICP) out29[threadIdx.x] = (float)tot[threadIdx.x];
 }
 
 // =======================================================================================
@@ -1208,14 +1091,6 @@ float track_min_scale(int level)
     return (float)(pow((double)minGrad[level], 2.0) / pow((double)sobelScale, 2.0));
 }
 
-static int trackBlocks(int N)
-{
-    int need = (N + TRK_THREADS - 1) / TRK_THREADS;
-    int cap = num_sms() * 2;
-    if (cap > TRACK_MAX_BLOCKS) cap = TRACK_MAX_BLOCKS;
-    return need < cap ? need : cap;
-}
-
 // CTAs of the persistent tracking grid per model (host logic, exported as mf_track_shares for the CPU tests).  A light model (bit set in
 // lightMask: an object model with a validity bitmask) gets one share, a heavy one (full-frame maps) `ratio` shares (launch_tracking passes 2, the
 // fastest of 1, 2, 3 and 5 on the 8- and 3-object scenes).  Without both kinds in the batch, or when the grid is too small for 4 CTAs per light model, the shares are equal.
@@ -1317,14 +1192,6 @@ int debug_track_timing(long long* out, int cap)
     (void)out; (void)cap;
     return 0;
 #endif
-}
-
-void launch_icp_only(const float4* vmapC, const float4* nmapC, const float4* vmapG, const float4* nmapG, int W, int H, Cam cam,
-                     const TrackPoses& pp, float* partial, unsigned* ticket, float* out29, Enq q)
-{
-    const float angleThres = (float)sin(20.f * 3.14159254f / 180.f);
-    launch(q, "k_icp_only", k_icp_only, trackBlocks(W * H), TRK_THREADS, 0, vmapC, nmapC, vmapG, nmapG, W, H, cam, pp, 0.10f, angleThres,
-           reinterpret_cast<double*>(partial), ticket, out29);
 }
 
 }  // namespace mfb

@@ -61,9 +61,9 @@ print(json.dumps({n: [name(getattr(L, n).restype), [name(t) for t in getattr(L, 
 """
 
 
-def test_bindings_follow_the_header(product_lib):
+def test_ctypes_bindings_follow_the_header(product_lib):
     hdr = _header()
-    assert len(hdr) == 138 and set(hdr) == set(product_lib.EXPORTS)
+    assert len(hdr) == 137 and set(hdr) == set(product_lib.EXPORTS)
     got = _child(_BINDINGS)
     for name, (ret, params) in hdr.items():
         assert got[name] == [ret, params], name

@@ -86,7 +86,7 @@ def test_multi_model_frames_that_spawn(tmp_path, multi_frames):
     assert counted == traced
 
 
-def test_stagewise_calls_and_readbacks(tmp_path, static_frames):
+def test_stage_calls_and_readbacks(tmp_path, static_frames):
     (rgb0, d0), (rgb1, d1) = static_frames[:2]
 
     def run():
@@ -101,7 +101,6 @@ def test_stagewise_calls_and_readbacks(tmp_path, static_frames):
         g.fuse(2, 4.0)
         g.clean(2)
         g.combinedPredict(2, 2)
-        g.icpStep(0, np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
         g.overridePose(np.eye(4, dtype=np.float32))
         g.uploadMap(g.downloadMap())
         g.indexMap(); g.prediction(); g.fillIn(); g.association(); g.modelMaps(1); g.trackStats()
