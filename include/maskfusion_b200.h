@@ -163,6 +163,16 @@ int mf_attach_detector(mf_context* ctx, struct mf_detector* detector, int every_
 int mf_download_frame_masks(mf_context* ctx, uint8_t* mask, int32_t* class_ids_256, int* n_masks);
 int mf_debug_track_timing(int64_t* out, int cap);   /* profiling builds only (-DMF_TRACK_TIMING): (tag, SM clock) pairs of the last tracking launch; else 0 */
 int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int iterations, int ellipse, uint8_t* inverted);
+/* Test hook: MfSegmentation::performSegmentation after the edge map (MfSegmentation.cpp:221-522), the frame path's own kernels, on host
+ * inputs of the context's W x H: the inverted edge map (255 = no edge), raw depth, the instance mask (values below n_masks; may be NULL
+ * when n_masks is 0) with its n_masks class ids, the projected-ID image (model ids or 0) and a model list of n_models (1..63) ids and
+ * classes, the id a new model would take and whether one may be created.  The segmentation thresholds are the context's (mf_config).
+ * Out: fullSegmentation (W x H), the component labels after edge removal (labels_out, may be NULL; numbering arbitrary) and
+ * {hasNewLabel, newClassID, nComponents} (result3_out, may be NULL).  The ignore map and maskToID persist from call to call as across
+ * frames; textureMask and the next frame's bookkeeping are untouched.  Multi-model contexts only (-5); bad counts or values: -3. */
+int mf_debug_segment(mf_context* ctx, const uint8_t* edges_inv, const float* depth, const uint8_t* mask, int n_masks, const int32_t* class_ids,
+                     const uint8_t* projected_ids, int n_models, const uint8_t* model_ids, const int32_t* model_class_ids, int next_model_id,
+                     int allow_new, uint8_t* segmentation_out, int32_t* labels_out, int32_t* result3_out);
 
 /* ---- stand-alone kernels exposed for parity tests (device work, host buffers) ---- */
 /* ---- multi-model inputs / outputs ---- */

@@ -385,6 +385,22 @@ class MaskFusion:
         self._ck(self.L.mf_morph_close(self.h, _p(a), int(radius), int(iterations), int(ellipse), None if ellipse else _p(inv)))
         return a if ellipse else (a, inv)
 
+    def debugSegment(self, edgesInv, depth, mask, classIDs, projectedIDs, modelIDs, modelClassIDs, nextModelID: int, allowNew: bool = True):
+        """test hook (mf_debug_segment): the segmentation after the edge map on host inputs and a given model list; the ignore map and
+        maskToID carry over from call to call.  mask may be None when classIDs is empty.
+        -> (fullSegmentation H x W uint8, labels after edge removal H x W int32, hasNewLabel, newClassID, nComponents)"""
+        shape = (self.H, self.W)
+        e = np.ascontiguousarray(edgesInv, np.uint8); d = np.ascontiguousarray(depth, np.float32)
+        p = np.ascontiguousarray(projectedIDs, np.uint8)
+        cls = np.ascontiguousarray(classIDs, np.int32); ids = np.ascontiguousarray(modelIDs, np.uint8)
+        mcls = np.ascontiguousarray(modelClassIDs, np.int32)
+        m = None if mask is None else np.ascontiguousarray(mask, np.uint8)
+        assert e.shape == d.shape == p.shape == shape and (m is None or m.shape == shape) and ids.shape == mcls.shape
+        seg = np.zeros(shape, np.uint8); lab = np.zeros(shape, np.int32); r = np.zeros(3, np.int32)
+        self._ck(self.L.mf_debug_segment(self.h, _p(e), _p(d), _p(m), int(cls.shape[0]), _p(cls), _p(p), int(ids.shape[0]), _p(ids), _p(mcls),
+                                         int(nextModelID), int(allowNew), _p(seg), _p(lab), _p(r)))
+        return seg, lab, int(r[0]), int(r[1]), int(r[2])
+
 
 class KlgLogReader:
     """reference: class KlgLogReader (GUI/Tools/KlgLogReader.{h,cpp})"""

@@ -355,6 +355,59 @@ extern "C" int mf_morph_close(mf_context* ctx, uint8_t* image, int radius, int i
     MF_CATCH(-1)
 }
 
+// test hook: the segmentation after the edge map (MaskFusion::segmentEdges, the code the frame path runs) on caller-given inputs and a
+// caller-given model list.  The inputs go into the buffers the frame path reads (the inverted edge map, the current slot's raw depth, mask
+// and header, the projected-ID image); the segmentation is written to a buffer of the call, so the context's textureMask is untouched,
+// and no FrameResult is left for the next processFrame to apply.  On purpose the call advances the state that persists across frames
+// like the members of the reference class: the person ignore map and maskToID.  projected_ids must hold model ids (or 0), as the
+// global projection gives them.
+extern "C" int mf_debug_segment(mf_context* ctx, const uint8_t* edges_inv, const float* depth, const uint8_t* mask, int n_masks,
+                                const int32_t* class_ids, const uint8_t* projected_ids, int n_models, const uint8_t* model_ids,
+                                const int32_t* model_class_ids, int next_model_id, int allow_new, uint8_t* segmentation_out,
+                                int32_t* labels_out, int32_t* result3_out)
+{
+    MF_TRY MF_NEED(ctx)
+    MF_UNQUEUED(ctx, "debug_segment")
+    MaskFusion* o = ctx->mf.get();
+    if (!o->cfg.enableMultipleModels) { mf_set_error("not a multi-model context"); return -5; }
+    if (n_masks < 0 || n_masks > 256 || n_models < 1 || n_models > MF_MAX_MODELS - 1 || next_model_id < 0 || next_model_id > 255) {
+        mf_set_error("debug_segment: need n_masks in 0..256, n_models in 1..63 and next_model_id in 0..255"); return -3;
+    }
+    if (!edges_inv || !depth || !projected_ids || !model_ids || !model_class_ids || !segmentation_out || (n_masks && (!mask || !class_ids))) {
+        mf_set_error("debug_segment: null input or output"); return -3;
+    }
+    bool isModel[256] = {};
+    for (int i = 0; i < n_models; ++i) isModel[model_ids[i]] = true;
+    for (int i = 0; i < o->P; ++i) {
+        if (projected_ids[i] && !isModel[projected_ids[i]]) { mf_set_error("debug_segment: projected_ids holds an id that is no model's"); return -3; }
+        if (n_masks && mask[i] >= n_masks) { mf_set_error("debug_segment: a mask value is not below n_masks"); return -3; }
+    }
+    o->waitHandoff(o->stream);                                      // a detector's hand-off into the current slot lands before ours
+    SegModels sm; memset(&sm, 0, sizeof sm);
+    sm.n = n_models; sm.nextID = (unsigned char)next_model_id;
+    for (int i = 0; i < n_models; ++i) { sm.id[i] = model_ids[i]; sm.classID[i] = model_class_ids[i]; }
+    FrameHdr h; memset(&h, 0, sizeof h);
+    h.nMasks = n_masks; h.maskGiven = n_masks > 0;
+    for (int i = 0; i < n_masks; ++i) h.classIDs[i] = class_ids[i];
+    const size_t P = (size_t)o->P;
+    cudaCheck(cudaMemcpyAsync(o->edgeInv.p, edges_inv, P, cudaMemcpyHostToDevice, o->stream), "H2D");
+    cudaCheck(cudaMemcpyAsync(o->depthRaw, depth, P * sizeof(float), cudaMemcpyHostToDevice, o->stream), "H2D");
+    if (n_masks) cudaCheck(cudaMemcpyAsync(o->frameMask, mask, P, cudaMemcpyHostToDevice, o->stream), "H2D");
+    cudaCheck(cudaMemcpyAsync(o->projectedIDs.p, projected_ids, P, cudaMemcpyHostToDevice, o->stream), "H2D");
+    launch_frame_header(h, o->dHdr, o->on());
+    DevBuf<uint8_t> seg; seg.alloc(P);
+    o->segTables(sm);
+    o->segmentEdges(sm, allow_new != 0, seg);
+    FrameResult r;
+    d2h(o, segmentation_out, seg.p, P);
+    d2h(o, labels_out, o->ccLabB.p, P);
+    cudaCheck(cudaMemcpyAsync(&r, o->dRes.p, sizeof r, cudaMemcpyDeviceToHost, o->stream), "D2H");
+    o->sync();
+    if (result3_out) { result3_out[0] = r.hasNewLabel; result3_out[1] = r.newClassID; result3_out[2] = r.nComponents; }
+    return 0;
+    MF_CATCH(-1)
+}
+
 // Mask R-CNN backbone on the frame path: every k-th processFrame enqueues mold_inputs + the ResNet-101-FPN forward of `backbone`
 // (mf_backbone_create) on the backbone's own stream (MaskRCNN::executeSequential is called from MfSegmentation.cpp:130). NULL detaches.
 extern "C" int mf_attach_backbone(mf_context* ctx, void* backbone, int every_k)

@@ -492,19 +492,29 @@ void MaskFusion::predict()
 
 // GlobalProjection::project (GlobalProjection.cpp:43-107): all models into one depth-tested key image; the key's low word
 // is (model list index << 26 | surfel id), i.e. the reference's draw order.  The ID image stays on the device.
-void MaskFusion::globalProjection() { segTables(); projectLocal(); projectResolve(); }
+void MaskFusion::globalProjection() { segTables(segModels()); projectLocal(); projectResolve(); }
 
 void MaskFusion::checkModelCount() const
 {
     if (models.size() > MF_MAX_MODELS - 1) throw CudaError{"global projection / segmentation support up to 63 models"};
 }
 
-// id <-> list-index tables of this frame's model list, as a kernel argument (no staging buffer, no synchronisation)
-void MaskFusion::segTables()
+// the model list as segmentation sees it: list order, ids, classes and the id a new model would take
+SegModels MaskFusion::segModels()
 {
     checkModelCount();
+    SegModels sm; memset(&sm, 0, sizeof sm);
+    sm.n = (int)models.size();
+    for (int i = 0; i < sm.n; ++i) { sm.id[i] = models[i]->id; sm.classID[i] = models[i]->classID; }
+    sm.nextID = getNextModelID(false);
+    return sm;
+}
+
+// id <-> list-index tables of a model list, as a kernel argument (no staging buffer, no synchronisation)
+void MaskFusion::segTables(const SegModels& sm)
+{
     SegTables t; memset(&t, 0, sizeof t);
-    for (size_t i = 0; i < models.size(); ++i) { t.idToIndex[models[i]->id] = (uint8_t)i; t.indexToId[i] = models[i]->id; t.isModel[models[i]->id] = 1; }
+    for (int i = 0; i < sm.n; ++i) { t.idToIndex[sm.id[i]] = (uint8_t)i; t.indexToId[i] = sm.id[i]; t.isModel[sm.id[i]] = 1; }
     launch_seg_tables(t, tblIdToIndex, tblIndexToId, tblIsModel, on());
 }
 
@@ -536,14 +546,22 @@ void MaskFusion::edgeMaps()
 // MfSegmentation::performSegmentation (MfSegmentation.cpp:83-538) with the CPU tail on the GPU (mf_seg.cu) and NO host round trip:
 // the number of components, the number of masks and their classes are read by the kernels from device memory; the mask -> model vote
 // (:433-492) is a kernel; its decision (new label?) travels to the host inside the FrameResult and is applied by applyFrameResult().
-void MaskFusion::performSegmentation(bool allowNew)
+void MaskFusion::performSegmentation(const SegModels& sm, bool allowNew)
 {
-    const int nModels = (int)models.size();
     edgeMaps();
     // the first readers of the frame's mask and of the header's mask fields: a detector's hand-off must have landed (tracking and the ID
     // projection above ran next to the detector)
     waitHandoff(stream);
     if (maskCommPending) { cudaCheck(cudaStreamWaitEvent(stream, evComm, 0), "cudaStreamWaitEvent"); maskCommPending = false; }   // sharded: the masks' broadcast
+    segmentEdges(sm, allowNew, mask);                       // writes textureMask directly (:297)
+}
+
+// everything of performSegmentation after the edge map (:221-522), on the inverted edge map (edgeInv), the frame's raw depth, mask and
+// header, and the projected-ID image, for the model list `sm` (whose tables segTables(sm) has set); the segmentation goes to `out`, the
+// vote's decision to dRes.  The ignore map and maskToID persist across calls like the members of the reference class.
+void MaskFusion::segmentEdges(const SegModels& sm, bool allowNew, uint8_t* out)
+{
+    const int nModels = sm.n;
     const Enq q = on();
     // ignore map (:221-235)
     launch_person_table(dHdr, personClassID, tblIsPerson, q);
@@ -566,10 +584,10 @@ void MaskFusion::performSegmentation(bool allowNew)
     VoteParams vp; memset(&vp, 0, sizeof vp);
     vp.nModels = nModels; vp.allowNew = allowNew ? 1 : 0; vp.personClassID = personClassID;
     vp.minNew = (unsigned)(size_t)(cfg.minRelSizeNew * (size_t)P); vp.maxNew = (unsigned)(size_t)(cfg.maxRelSizeNew * (size_t)P);
-    vp.minMaskModelOverlap = minMaskModelOverlap; vp.nextModelID = getNextModelID(false);
-    for (int i = 0; i < nModels; ++i) { vp.modelClass[i] = models[i]->classID; vp.modelID[i] = models[i]->id; }
+    vp.minMaskModelOverlap = minMaskModelOverlap; vp.nextModelID = sm.nextID;
+    for (int i = 0; i < nModels; ++i) { vp.modelClass[i] = sm.classID[i]; vp.modelID[i] = sm.id[i]; }
     launch_vote(dHdr, vp, maskPixels, maskOverlap, ccCounter, tblMaskToID, dRes, q);
-    launch_seg_final(segTmp, lab, mapToMask, absorbId, tblMaskToID, ccBox, P, W, mask, q);      // writes textureMask directly (:297)
+    launch_seg_final(segTmp, lab, mapToMask, absorbId, tblMaskToID, ccBox, P, W, out, q);
 }
 
 // MaskFusion::getNextModelID (MaskFusion.cpp:712-730)
@@ -977,10 +995,11 @@ void MaskFusion::frameEnd(float weightMultiplier)
                         joinComm(false);
                     }
                 }
-                segTables();
+                const SegModels sm = segModels();
+                segTables(sm);
                 projectResolve();
                 if (spawnOffset < cfg.modelSpawnOffset) spawnOffset++;
-                performSegmentation(spawnOffset >= cfg.modelSpawnOffset);
+                performSegmentation(sm, spawnOffset >= cfg.modelSpawnOffset);
                 // what the host needs from this frame, in one copy behind the vote kernel; picked up by the next finalisePending()
                 on().mark("copy_result_d2h");
                 cudaCheck(cudaMemcpyAsync(hRes, dRes.p, sizeof(FrameResult), cudaMemcpyDeviceToHost, stream), "result D2H");

@@ -146,9 +146,11 @@ public:
     // ---- multi-model path (MaskFusion.cpp:287-375) ----
     void globalProjection();                                                                      // GlobalProjection::project + downloadDirect (stays on the device)
     void checkModelCount() const;                                                                 // the ID projection and segmentation hold up to 63 models
-    void segTables();
+    SegModels segModels();                                                                        // the model list of this frame (ids, classes, next id)
+    void segTables(const SegModels& sm);
     void edgeMaps();                                                                              // MfSegmentation floatEdgeMap -> binary -> close -> invert
-    void performSegmentation(bool allowNew);                                                      // MfSegmentation::performSegmentation (result -> FrameResult)
+    void performSegmentation(const SegModels& sm, bool allowNew);                                 // MfSegmentation::performSegmentation (result -> FrameResult)
+    void segmentEdges(const SegModels& sm, bool allowNew, uint8_t* out);                          // its part after the edge map (also mf_debug_segment)
     unsigned char getNextModelID(bool assign);                                                    // MaskFusion::getNextModelID
     void initFirstRGB(Model* m);                                                                  // RGBDOdometry::initFirstRGB of the current frame
     Model* spawnObjectModel();                                                                    // MaskFusion::spawnObjectModel + moveNewModelToList

@@ -147,6 +147,8 @@ struct FrameResult {
     int detectError;
 };
 struct SegTables { unsigned char idToIndex[256], indexToId[256], isModel[256]; };
+// a model list as segmentation reads it (host side): list order, ids, classes, and the id a new model would take
+struct SegModels { int n; unsigned char id[MF_MAX_MODELS]; int classID[MF_MAX_MODELS]; unsigned char nextID; };
 struct VoteParams {
     int nModels, allowNew, personClassID; unsigned minNew, maxNew; float minMaskModelOverlap; unsigned char nextModelID;
     int modelClass[MF_MAX_MODELS]; unsigned char modelID[MF_MAX_MODELS];

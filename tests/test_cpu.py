@@ -355,12 +355,20 @@ def test_oracle_opencv_restatements_match_cv2(oracle):
     L.orc_morph_close_ellipse.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
     libc = C.CDLL(None)
     libc.free.argtypes = [C.c_void_p]
+    from tests import seg_cases
     rng = np.random.default_rng(3)
+    images = []
     for (W, H, p) in [(64, 48, 0.55), (97, 61, 0.7), (640, 480, 0.62), (33, 17, 0.9), (16, 16, 0.0), (16, 16, 1.0)]:
         img = (rng.random((H, W)) < p).astype(np.uint8) * 255
         if W == 640:                      # realistic: blobs with thin bridges
             yy, xx = np.mgrid[0:H, 0:W]
             img = (((np.sin(xx / 9.0) * np.cos(yy / 7.0) > -0.2) & (rng.random((H, W)) < 0.97)) * 255).astype(np.uint8)
+        images.append(img)
+    # the crafted images of the segmentation cases at the sizes that leave a remainder tile (or no tile edge at all)
+    for (W, H) in [(644, 484), (36, 20), (28, 12)]:
+        images += [seg_cases.checkerboard(W, H), seg_cases.spiral(W, H), seg_cases.comb(W, H)]
+    for img in images:
+        H, W = img.shape
         labels = np.zeros((H, W), np.int32)
         stats_p = C.POINTER(C.c_int32)()
         n = L.orc_connected_components4(oracle.ptr(img), W, H, oracle.ptr(labels), C.byref(stats_p))

@@ -63,7 +63,10 @@ print(json.dumps({n: [name(getattr(L, n).restype), [name(t) for t in getattr(L, 
 
 def test_ctypes_bindings_follow_the_header(product_lib):
     hdr = _header()
-    assert len(hdr) == 137 and set(hdr) == set(product_lib.EXPORTS)
+    assert len(hdr) == 138 and set(hdr) == set(product_lib.EXPORTS)
+    # the segmentation test hook: context, 3 input images + mask count + classes, projected ids, model list, next id, allow-new, 3 outputs
+    assert hdr["mf_debug_segment"] == ("c_int", ["c_void_p"] * 4 + ["c_int", "c_void_p", "c_void_p", "c_int", "c_void_p", "c_void_p", "c_int",
+                                                                     "c_int", "c_void_p", "c_void_p", "c_void_p"])
     got = _child(_BINDINGS)
     for name, (ret, params) in hdr.items():
         assert got[name] == [ret, params], name
